@@ -300,7 +300,7 @@ typedef enum {
     MDN_INFO_QUERY_INDICES = 7,    /* num_queries u64 */
     MDN_INFO_JIT = 8,              /* per AIR (proof order) of the last proof: 1 = NVRTC kernel, 0 = interpreter */
     MDN_INFO_POOL = 9,             /* cudaMallocAsync pool reserved now / high, used now / high (bytes); proof arena capacity (bytes), slabs, driver allocations so far, live blocks */
-    MDN_INFO_BUILD = 10,           /* { generation of the field arithmetic (1 = poseidon2_fast.cuh, 2 = poseidon2_fast2.cuh), generation of the NTT kernels (1 = kernels.cu, 2 = ntt2.cuh) } this library was built with */
+    MDN_INFO_BUILD = 10,           /* { generation of the field arithmetic, generation of the NTT kernels }: always { 2, 2 } (poseidon2_fast2.cuh, ntt2.cuh) */
 } mdn_info;
 /* QUOTIENT_ACC / DEEP_EVALS are only recorded (extra device->host copies) after mdn_set_debug(s, 1). */
 int mdn_set_debug(mdn_session* s, int enable);

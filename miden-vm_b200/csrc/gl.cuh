@@ -19,14 +19,9 @@ typedef unsigned int u32;
 static constexpr u64 P = 0xFFFFFFFF00000001ULL;
 static constexpr u64 EPS = 0xFFFFFFFFULL;  // 2^64 mod p = 2^32 - 1
 
-#if !defined(MDN_GL_SLOW) && !defined(MDN_GL_FAST)
-#define MDN_GL_FAST 1
-#endif
-#ifdef MDN_GL_FAST
 // add / sub / mul of the kernels that use gl:: directly (constraint interpreter, LogUp rows, DEEP tail, OOD, FRI fold) on
-// the carry flag and one 128-bit product, like poseidon2_fast2.cuh; same contracts (canonical operands for add / sub,
-// canonical results everywhere), same PTX templates, unsigned __int128 on the host.  The default (identical proof
-// bytes); -DMDN_GL_SLOW restores the branchy forms (the first-generation A/B library uses them).
+// the carry flag and one 128-bit product, like poseidon2_fast2.cuh: canonical operands for add / sub, canonical results
+// everywhere, the same PTX templates, unsigned __int128 on the host.
 GL_HD void fast_subb64(u64 a, u64 b, u64& r, unsigned& m) {
 #ifdef __CUDA_ARCH__
     asm("sub.cc.u64 %0, %2, %3;\n\tsubc.u32 %1, 0, 0;" : "=l"(r), "=r"(m) : "l"(a), "l"(b));
@@ -43,23 +38,9 @@ GL_HD void fast_addc64(u64 a, u64 b, u64& r, unsigned& c) {
 }
 GL_HD u64 sub(u64 a, u64 b) { u64 d; unsigned m; fast_subb64(a, b, d, m); return d - (u64)m; }
 GL_HD u64 add(u64 a, u64 b) { return sub(a, P - b); }
-#else
-GL_HD u64 add(u64 a, u64 b) {
-    u64 s = a + b;
-    if (s < a) s += EPS;        // overflowed 2^64: fold the carry back (result < p)
-    else if (s >= P) s -= P;
-    return s;
-}
-GL_HD u64 sub(u64 a, u64 b) {
-    u64 d = a - b;
-    if (a < b) d -= EPS;        // borrowed 2^64: add p
-    return d;
-}
-#endif
 GL_HD u64 neg(u64 a) { return a ? P - a : 0; }
 GL_HD u64 dbl(u64 a) { return add(a, a); }
 
-#ifdef MDN_GL_FAST
 GL_HD u64 mul(u64 a, u64 b) {
     unsigned __int128 q = (unsigned __int128)a * b;
     u64 lo = (u64)q, hi = (u64)(q >> 64);
@@ -77,28 +58,6 @@ GL_HD u64 mul(u64 a, u64 b) {
     fast_subb64(r, P, t, m);
     return t - (u64)m;
 }
-#else
-GL_HD u64 mulhi(u64 a, u64 b) {
-#ifdef __CUDA_ARCH__
-    return __umul64hi(a, b);
-#else
-    return (u64)(((unsigned __int128)a * b) >> 64);
-#endif
-}
-
-// Reduce a 128-bit value (hi, lo) using 2^64 = 2^32 - 1 and 2^96 = -1 (mod p).
-GL_HD u64 reduce128(u64 lo, u64 hi) {
-    u64 hh = hi >> 32, hl = hi & EPS;
-    u64 t = lo - hh;
-    if (lo < hh) t -= EPS;
-    u64 m = (hl << 32) - hl;    // hl * (2^32 - 1)
-    u64 r = t + m;
-    if (r < t) r += EPS;
-    if (r >= P) r -= P;
-    return r;
-}
-GL_HD u64 mul(u64 a, u64 b) { return reduce128(a * b, mulhi(a, b)); }
-#endif
 GL_HD u64 sqr(u64 a) { return mul(a, a); }
 
 // Halve: a/2 mod p.

@@ -70,23 +70,8 @@ __device__ __forceinline__ u64 fsub(u64 a, u64 b) {
 __device__ __forceinline__ u64 fadd(u64 a, u64 b) { return fsub(a, GP - b); }
 __device__ __forceinline__ u64 fneg(u64 a) { return a ? GP - a : 0ull; }
 )CUDA";
-// first-generation multiplication (the one every JIT measurement so far ran with)
-static const char PRELUDE_FMUL_G1[] = R"CUDA(__device__ __forceinline__ u64 fmul(u64 x, u64 y) {
-    u64 lo = x * y, hi = __umul64hi(x, y);
-    u32 hl = (u32)hi, hh = (u32)(hi >> 32);
-    u64 t, m, r; u32 b, c;
-    asm("sub.cc.u64 %0, %2, %3;\n\tsubc.u32 %1, 0, 0;" : "=l"(t), "=r"(b) : "l"(lo), "l"((u64)hh));
-    t -= (u64)b;
-    asm("mul.wide.u32 %0, %1, %2;" : "=l"(m) : "r"(hl), "r"(0xFFFFFFFFu));
-    asm("add.cc.u64 %0, %2, %3;\n\taddc.u32 %1, 0, 0;" : "=l"(r), "=r"(c) : "l"(t), "l"(m));
-    r += (u64)(0u - c);
-    u64 q; u32 k;
-    asm("sub.cc.u64 %0, %2, %3;\n\tsubc.u32 %1, 0, 0;" : "=l"(q), "=r"(k) : "l"(r), "l"(GP));
-    return q - (u64)k;
-}
-)CUDA";
-// second-generation multiplication (poseidon2_fast2.cuh: one 128-bit product, the carry folded by an IMAD.WIDE);
-// the default (tools/realistic_air_probe.py times both on Miden-size constraint programs)
+// field multiplication: one 128-bit product as in poseidon2_fast2.cuh (needs --device-int128), the carry folded by an
+// IMAD.WIDE
 static const char PRELUDE_FMUL_G2[] = R"CUDA(__device__ __forceinline__ u64 fmul(u64 x, u64 y) {
     unsigned __int128 q = (unsigned __int128)x * y;
     u64 lo = (u64)q, hi = (u64)(q >> 64);
@@ -138,7 +123,6 @@ struct GenInfo { uint32_t n_constraints = 0; bool uses_sel = false; uint32_t n_c
 // Leaves (trace cells, constants, challenges ...) are re-materialised in every chunk that reads them; arithmetic
 // values that live across a chunk boundary travel through two small per-thread arrays (Sb: base, Se: extension)
 // whose slots are assigned by chunk-granular liveness.
-inline bool jit_arith2() { const char* e = getenv("MDN_JIT_ARITH"); return !(e && atoi(e) == 1); }   // MDN_JIT_ARITH=1 restores the first generation
 inline uint32_t chunk_nodes() { const char* e = getenv("MDN_JIT_CHUNK"); uint32_t v = e ? (uint32_t)atoi(e) : 0; return v ? v : 512; }
 
 // lookup == true: `w` is a lowered LookupAir ("MLKP": 4-word interactions instead of constraint ids) and the
@@ -253,7 +237,7 @@ inline std::string generate(const uint32_t* w, GenInfo* info, bool lookup = fals
     std::string s;
     s.reserve(80 * (size_t)nn + 16384);
     s += PRELUDE;
-    s += jit_arith2() ? PRELUDE_FMUL_G2 : PRELUDE_FMUL_G1;
+    s += PRELUDE_FMUL_G2;
     s += PRELUDE_B;
     s += lookup ? "typedef LookupJitArgs KArgs;\n" : "typedef JitArgs KArgs;\n";
     s += "struct Ctx { size_t L, pos, pn, per_idx, per_stride; u64 is_first, is_last, is_trans; };\n";
@@ -426,7 +410,7 @@ inline std::vector<char> compile(const std::string& src) {
     std::vector<const char*> opts = {"--gpu-architecture=sm_90a", "-std=c++17", "-lineinfo", "-default-device"};
     std::string po = std::string("--ptxas-options=") + (getenv("MDN_JIT_PTXAS") ? getenv("MDN_JIT_PTXAS") : "-O3");
     opts.push_back(po.c_str());
-    if (jit_arith2()) opts.push_back("--device-int128");
+    opts.push_back("--device-int128");
     rc = n.CompileProgram(prog, (int)opts.size(), opts.data());
     if (rc) {
         size_t ls = 0; n.GetProgramLogSize(prog, &ls);

@@ -4,20 +4,8 @@
 // permutations held entirely in registers, (c) streaming reductions over LDE columns.
 #include "kernels.cuh"
 #include "poseidon2.cuh"
-// Second-generation field arithmetic and NTT are the default (tools/ab_check.py checks that both generations prove the
-// same bytes); -DMDN_GEN1 builds the first generation (libmiden_b200_gen1.so, the A/B baseline).
-#ifndef MDN_GEN1
-#define MDN_ARITH_V2 1
-#define MDN_NTT_V2 1
-#endif
-#ifdef MDN_ARITH_V2
 #include "poseidon2_fast2.cuh"    // host-checked by tests/cpp/test_arith_v2.cpp
-#else
-#include "poseidon2_fast.cuh"     // r1b..r1k measurements
-#endif
-#ifdef MDN_NTT_V2
 #include "ntt2.cuh"               // host-checked by tests/cpp/test_ntt_v2.cpp
-#endif
 #include "blake3.cuh"
 #include "keccak.cuh"
 #include "rescue.cuh"
@@ -170,212 +158,6 @@ __device__ __forceinline__ u64 w_pow(const u64* __restrict__ hi, const u64* __re
     return gl::mul(hi[e >> lo_bits], lo[e & ((1ull << lo_bits) - 1)]);
 }
 
-#ifndef MDN_NTT_V2
-// ---------------------------------------------------------------------------------------------
-// Register-tiled radix-2 stages over a shared-memory tile.
-//   tile element (idx, cc), idx < 2^m, cc < 2^log_cols, lives at off(idx, cc); contiguous tiles
-//   (log_cols == 0) are padded by one word every 8 to keep the strided accesses conflict-free.
-//   Each thread takes groups of 2^LOGR elements idx = base + k * 2^b and runs LOGR stages on them in
-//   registers, so a size-2^m transform needs ceil(m / 3) shared-memory round trips instead of m.
-// ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ u32 tile_off(u32 idx, u32 cc, u32 log_cols) {
-    u32 o = (idx << log_cols) + cc;
-    return log_cols ? o : o + (o >> 3);
-}
-__host__ __device__ __forceinline__ u32 tile_words(u32 m, u32 log_cols) {
-    u32 n = 1u << (m + log_cols);
-    return log_cols ? n : n + (n >> 3) + 1;
-}
-
-// DIT (bit-reversed -> natural) stages b .. b+LOGR-1 (butterfly spans 2^b .. 2^(b+LOGR-1)).
-template <int LOGR>
-__device__ __forceinline__ void dit_round(u64* x, const u64* tw, u32 m, u32 b, u32 log_cols) {
-    constexpr int R = 1 << LOGR;
-    u32 groups = 1u << (m - LOGR + log_cols);
-    for (u32 g = threadIdx.x; g < groups; g += blockDim.x) {
-        u32 cc = g & ((1u << log_cols) - 1), gg = g >> log_cols;
-        u32 lo = gg & ((1u << b) - 1), hi = gg >> b;
-        u32 base = (hi << (b + LOGR)) | lo;
-        u64 v[R];
-#pragma unroll
-        for (int k = 0; k < R; k++) v[k] = x[tile_off(base + ((u32)k << b), cc, log_cols)];
-#pragma unroll
-        for (int st = 0; st < LOGR; st++) {
-            // span 2^(b+st): pairs (k, k + 2^st) with bit st of k clear; j = lo + (k mod 2^st) * 2^b
-#pragma unroll
-            for (int k = 0; k < R; k++) {
-                if (k & (1 << st)) continue;
-                u32 j = lo + ((u32)(k & ((1 << st) - 1)) << b);
-                u64 w = tw[j << (m - 1 - b - st)];
-                u64 a = v[k], c = glf::cmul(v[k + (1 << st)], w);
-                v[k] = glf::cadd(a, c);
-                v[k + (1 << st)] = glf::csub(a, c);
-            }
-        }
-#pragma unroll
-        for (int k = 0; k < R; k++) x[tile_off(base + ((u32)k << b), cc, log_cols)] = v[k];
-    }
-}
-// DIF (natural -> bit-reversed) stages with spans 2^(b+LOGR-1) .. 2^b (descending).
-template <int LOGR>
-__device__ __forceinline__ void dif_round(u64* x, const u64* tw, u32 m, u32 b, u32 log_cols) {
-    constexpr int R = 1 << LOGR;
-    u32 groups = 1u << (m - LOGR + log_cols);
-    for (u32 g = threadIdx.x; g < groups; g += blockDim.x) {
-        u32 cc = g & ((1u << log_cols) - 1), gg = g >> log_cols;
-        u32 lo = gg & ((1u << b) - 1), hi = gg >> b;
-        u32 base = (hi << (b + LOGR)) | lo;
-        u64 v[R];
-#pragma unroll
-        for (int k = 0; k < R; k++) v[k] = x[tile_off(base + ((u32)k << b), cc, log_cols)];
-#pragma unroll
-        for (int st = LOGR - 1; st >= 0; st--) {
-#pragma unroll
-            for (int k = 0; k < R; k++) {
-                if (k & (1 << st)) continue;
-                u32 j = lo + ((u32)(k & ((1 << st) - 1)) << b);
-                u64 w = tw[j << (m - 1 - b - st)];
-                u64 a = v[k], c = v[k + (1 << st)];
-                v[k] = glf::cadd(a, c);
-                v[k + (1 << st)] = glf::cmul(glf::csub(a, c), w);
-            }
-        }
-#pragma unroll
-        for (int k = 0; k < R; k++) x[tile_off(base + ((u32)k << b), cc, log_cols)] = v[k];
-    }
-}
-__device__ __forceinline__ void smem_dit(u64* x, const u64* tw, u32 m, u32 log_cols) {
-    u32 b = 0;
-    while (b < m) {
-        u32 left = m - b;
-        if (left >= 3 && left != 4) { dit_round<3>(x, tw, m, b, log_cols); b += 3; }
-        else if (left == 4 || left == 2) { dit_round<2>(x, tw, m, b, log_cols); b += 2; }
-        else { dit_round<1>(x, tw, m, b, log_cols); b += 1; }
-        __syncthreads();
-    }
-}
-__device__ __forceinline__ void smem_dif(u64* x, const u64* tw, u32 m, u32 log_cols) {
-    u32 top = m;   // stages with spans below 2^top remain
-    while (top > 0) {
-        if (top >= 3 && top != 4) { dif_round<3>(x, tw, m, top - 3, log_cols); top -= 3; }
-        else if (top == 4 || top == 2) { dif_round<2>(x, tw, m, top - 2, log_cols); top -= 2; }
-        else { dif_round<1>(x, tw, m, top - 1, log_cols); top -= 1; }
-        __syncthreads();
-    }
-}
-
-// inverse step 1: strided tile [N1][C]
-__global__ void __launch_bounds__(NTT_THREADS) k_intt_strided(u64* cols, size_t col_stride, NttTables T, u32 log_c) {
-    u32 C = 1u << log_c;
-    extern __shared__ u64 sm[];
-    u32 N1 = 1u << T.n1, N2 = 1u << T.n2;
-    u64* x = sm; u64* tw = sm + tile_words(T.n1, log_c);
-    u64* col = cols + blockIdx.y * col_stride;
-    u32 j2_0 = blockIdx.x * C;
-    for (u32 i = threadIdx.x; i < N1 / 2; i += blockDim.x) tw[i] = T.twi_n1[i];
-    for (u32 idx = threadIdx.x; idx < N1 * C; idx += blockDim.x) {
-        u32 j1 = idx >> log_c, cc = idx & (C - 1);
-        x[tile_off(j1, cc, log_c)] = col[(size_t)j1 * N2 + j2_0 + cc];
-    }
-    __syncthreads();
-    smem_dif(x, tw, T.n1, log_c);
-    for (u32 idx = threadIdx.x; idx < N1 * C; idx += blockDim.x) {
-        u32 slot = idx >> log_c, cc = idx & (C - 1);
-        u32 k1 = gl::bitrev32(slot, T.n1);
-        u32 j2 = j2_0 + cc;
-        u64 f = w_pow(T.wi_hi, T.wi_lo, T.lo_bits, (u64)j2 * k1);
-        col[(size_t)slot * N2 + j2] = glf::cmul(x[tile_off(slot, cc, log_c)], f);
-    }
-}
-// inverse step 3 (or the whole transform when n1 == 0): contiguous chunk of N2
-__global__ void __launch_bounds__(NTT_THREADS) k_intt_contig(u64* cols, size_t col_stride, NttTables T) {
-    extern __shared__ u64 sm[];
-    u32 N2 = 1u << T.n2;
-    u64* x = sm; u64* tw = sm + tile_words(T.n2, 0);
-    u64* chunk = cols + blockIdx.y * col_stride + (size_t)blockIdx.x * N2;
-    for (u32 i = threadIdx.x; i < N2 / 2; i += blockDim.x) tw[i] = T.twi_n2[i];
-    for (u32 i = threadIdx.x; i < N2; i += blockDim.x) x[tile_off(i, 0, 0)] = chunk[i];
-    __syncthreads();
-    smem_dif(x, tw, T.n2, 0);
-    for (u32 i = threadIdx.x; i < N2; i += blockDim.x) chunk[i] = x[tile_off(i, 0, 0)];
-}
-void launch_intt(u64* cols, size_t col_stride, u32 n_cols, const NttTables& T, cudaStream_t st) {
-    u32 N1 = 1u << T.n1, N2 = 1u << T.n2;
-    if (T.n1 > 0) {
-        u32 log_c = T.n1 >= 12 ? 0 : 12 - T.n1; if (log_c > T.n2) log_c = T.n2;
-        u32 C = 1u << log_c;
-        size_t smem = ((size_t)tile_words(T.n1, log_c) + N1 / 2) * sizeof(u64);
-        cudaFuncSetAttribute(k_intt_strided, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        k_intt_strided<<<dim3(N2 / C, n_cols), ntt_threads(T.n1, log_c), smem, st>>>(cols, col_stride, T, log_c);
-        COUNT_LAUNCH();
-    }
-    size_t smem = ((size_t)tile_words(T.n2, 0) + N2 / 2 + 1) * sizeof(u64);
-    k_intt_contig<<<dim3(N1, n_cols), ntt_threads(T.n2, 0), smem, st>>>(cols, col_stride, T);
-    COUNT_LAUNCH();
-}
-
-// forward step 1: contiguous chunk, premultiplied by base^j / N
-__global__ void __launch_bounds__(NTT_THREADS) k_fwd_contig(const FwdItem* __restrict__ items, NttTables T, PremulTables Pm) {
-    extern __shared__ u64 sm[];
-    u32 N1 = 1u << T.n1, N2 = 1u << T.n2;
-    u64* x = sm; u64* tw = sm + tile_words(T.n2, 0);
-    FwdItem it = items[blockIdx.y];
-    u32 p_hi = blockIdx.x;
-    u32 j1 = gl::bitrev32(p_hi, T.n1);
-    const u64* src = it.src + (size_t)p_hi * N2;
-    u64* dst = it.dst + (size_t)p_hi * N2;
-    u64 fb = Pm.tab_b[(size_t)it.base * N1 + j1];
-    const u64* ta = Pm.tab_a + (size_t)it.base * N2;
-    for (u32 i = threadIdx.x; i < N2 / 2; i += blockDim.x) tw[i] = T.tw_n2[i];
-    for (u32 i = threadIdx.x; i < N2; i += blockDim.x) {
-        u32 j2 = gl::bitrev32(i, T.n2);
-        x[tile_off(i, 0, 0)] = glf::cmul(src[i], glf::mul(ta[j2], fb));
-    }
-    __syncthreads();
-    smem_dit(x, tw, T.n2, 0);
-    if (T.n1 > 0) {
-        for (u32 k2 = threadIdx.x; k2 < N2; k2 += blockDim.x)
-            dst[k2] = glf::cmul(x[tile_off(k2, 0, 0)], glf::mul(T.w_hi[((u64)j1 * k2) >> T.lo_bits], T.w_lo[((u64)j1 * k2) & ((1ull << T.lo_bits) - 1)]));
-    } else {
-        for (u32 k2 = threadIdx.x; k2 < N2; k2 += blockDim.x) dst[k2] = x[tile_off(k2, 0, 0)];
-    }
-}
-// forward step 3: strided tile [N1][C], DIT along p_hi, in place
-__global__ void __launch_bounds__(NTT_THREADS) k_fwd_strided(const FwdItem* __restrict__ items, NttTables T, u32 log_c) {
-    u32 C = 1u << log_c;
-    extern __shared__ u64 sm[];
-    u32 N1 = 1u << T.n1, N2 = 1u << T.n2;
-    u64* x = sm; u64* tw = sm + tile_words(T.n1, log_c);
-    u64* col = items[blockIdx.y].dst;
-    u32 k2_0 = blockIdx.x * C;
-    for (u32 i = threadIdx.x; i < N1 / 2; i += blockDim.x) tw[i] = T.tw_n1[i];
-    for (u32 idx = threadIdx.x; idx < N1 * C; idx += blockDim.x) {
-        u32 p_hi = idx >> log_c, cc = idx & (C - 1);
-        x[tile_off(p_hi, cc, log_c)] = col[(size_t)p_hi * N2 + k2_0 + cc];
-    }
-    __syncthreads();
-    smem_dit(x, tw, T.n1, log_c);
-    for (u32 idx = threadIdx.x; idx < N1 * C; idx += blockDim.x) {
-        u32 k1 = idx >> log_c, cc = idx & (C - 1);
-        col[(size_t)k1 * N2 + k2_0 + cc] = x[tile_off(k1, cc, log_c)];
-    }
-}
-void launch_fwd_ntt(const FwdItem* d_items, u32 n_items, const NttTables& T, const PremulTables& Pm, cudaStream_t st) {
-    u32 N1 = 1u << T.n1, N2 = 1u << T.n2;
-    size_t smem = ((size_t)tile_words(T.n2, 0) + N2 / 2 + 1) * sizeof(u64);
-    k_fwd_contig<<<dim3(N1, n_items), ntt_threads(T.n2, 0), smem, st>>>(d_items, T, Pm);
-    COUNT_LAUNCH();
-    if (T.n1 > 0) {
-        u32 log_c = T.n1 >= 12 ? 0 : 12 - T.n1; if (log_c > T.n2) log_c = T.n2;
-        u32 C = 1u << log_c;
-        size_t smem2 = ((size_t)tile_words(T.n1, log_c) + N1 / 2) * sizeof(u64);
-        cudaFuncSetAttribute(k_fwd_strided, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem2);
-        k_fwd_strided<<<dim3(N2 / C, n_items), ntt_threads(T.n1, log_c), smem2, st>>>(d_items, T, log_c);
-        COUNT_LAUNCH();
-    }
-}
-
-#else   // MDN_NTT_V2: block functions of ntt2.cuh (host-checked by tests/cpp/test_ntt_v2.cpp) ------------------------
 // ptxas chooses the register count (no minimum-resident-blocks bound)
 #define NTT_BOUNDS __launch_bounds__(NTT_THREADS)
 // Kernels are instantiated with the split (n1, n2) as compile-time constants for the trace heights that matter
@@ -443,7 +225,6 @@ void launch_fwd_ntt(const FwdItem* d_items, u32 n_items, const NttTables& T, con
 #undef X
     launch_fwd_t<-1, -1>(d_items, n_items, T, Pm, log_c, st);
 }
-#endif  // MDN_NTT_V2
 
 // =============================================================================================
 // Poseidon2 hashing
@@ -451,11 +232,8 @@ void launch_fwd_ntt(const FwdItem* d_items, u32 n_items, const NttTables& T, con
 static constexpr int HASH_THREADS = 128;
 // Minimum resident blocks the compiler must allow: the kernels are bound by the two integer pipes and more warps per
 // scheduler interleave their FMA and ALU bursts.  For sm_90a ptxas gives the Poseidon2 kernels about 62 registers
-// without the bound (8 blocks per SM), under the cap of any value up to 8; -DHASH_MIN_BLOCKS=k builds other variants
-// (tools/tune_hash.py).
-#ifndef HASH_MIN_BLOCKS
-#define HASH_MIN_BLOCKS 6
-#endif
+// without the bound (8 blocks per SM), under the cap of any value up to 8.
+static constexpr int HASH_MIN_BLOCKS = 6;
 
 // The permutation of the algebraic configurations (air/src/config.rs:225-273: one LMCS / challenger type, generic in P):
 // PERM_P2 = Poseidon2 (the metric's; lazy representatives, canonicalised on store), PERM_RPO / PERM_RPX = rescue.cuh (canonical in,
@@ -1257,10 +1035,8 @@ struct DeepKArgs {
 // PTS points per thread: point k lies k/PTS of the rank's range further on, so every stream stays coalesced; PTS points multiply
 // the independent column loads in flight (4 columns x PTS points) and share ONE field inversion for their denominators
 // (z0 - x)(z1 - x) (Montgomery's trick) -- the inversion (a Fermat power, ~100 multiplications) is as much arithmetic as the
-// 121-column dot products of a point.  PTS = 2 takes 64 registers for sm_90a; -DDEEP_PTS=k builds other variants (tools/tune_hash.py).
-#ifndef DEEP_PTS
-#define DEEP_PTS 2
-#endif
+// 121-column dot products of a point.  PTS = 2 takes 64 registers for sm_90a.
+static constexpr int DEEP_PTS = 2;
 template <int PTS>
 __global__ void __launch_bounds__(256) k_deep(DeepKArgs a) {
     extern __shared__ u64 sm_apow[];
@@ -1348,7 +1124,7 @@ void launch_deep(const DeepArgs& a, cudaStream_t st) {
     u32 B = 1u << a.log_blowup;
     k.t0 = a.nt ? a.t0 : 0; k.nt = a.nt ? a.nt : B;
     size_t cnt = (size_t)k.nt << a.log_n_max;
-    if (DEEP_PTS > 1 && cnt % (256 * DEEP_PTS) == 0) k_deep<DEEP_PTS><<<(unsigned)(cnt / (256 * DEEP_PTS)), 256, 2 * a.total_w * sizeof(u64), st>>>(k);
+    if (cnt % (256 * DEEP_PTS) == 0) k_deep<DEEP_PTS><<<(unsigned)(cnt / (256 * DEEP_PTS)), 256, 2 * a.total_w * sizeof(u64), st>>>(k);
     else k_deep<1><<<(unsigned)((cnt + 255) / 256), 256, 2 * a.total_w * sizeof(u64), st>>>(k);
     COUNT_LAUNCH();
 }

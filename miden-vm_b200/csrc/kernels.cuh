@@ -51,7 +51,6 @@ void launch_push(const u64* src, const PeerPtrs& dst, u32 rank, u32 world, size_
 struct NttTables {
     u32 n, n1, n2, lo_bits;
     const u64* tw_n1;       // w_{N1}^i, i < N1/2       (forward)
-    const u64* tw_n2;       // w_{N2}^i, i < N2/2
     const u64* twi_n1;      // inverse roots
     const u64* twi_n2;
     const u64* w_lo;        // w_N^i,               i < 2^lo_bits
@@ -59,12 +58,11 @@ struct NttTables {
     const u64* wi_lo;       // inverse
     const u64* wi_hi;
 };
-// Pre-multiplication tables for a coset base g: premul(j) = g^j / N with j = j2*N1 + j1:
-//   tab_a[j2] = (g^N1)^j2 (j2 < N2),  tab_b[j1] = g^j1 / N (j1 < N1).  One pair per base.
+// Pre-multiplication tables for a coset base g: premul(j) = g^j / N with j = j2*N1 + j1, one pair per base:
+//   tab_b[j1] = g^j1 / N (j1 < N1);
 //   tab_c[(1 << s) - 1 + j] = (g^N1)^(N2 / 2^(s+1)) * w_{2^(s+1)}^j: per-stage twiddles of the contiguous pass with
-//   the coset shift folded in (second-generation kernels, ntt2.cuh); built by ntt_tables.hpp.
+//   the coset shift (g^N1)^j2 folded in (ntt2.cuh); built by ntt_tables.hpp.
 struct PremulTables {
-    const u64* tab_a;   // n_bases x N2
     const u64* tab_b;   // n_bases x N1
     const u64* tab_c;   // n_bases x N2 (N2 - 1 used)
 };

@@ -1,13 +1,12 @@
-// Second-generation NTT block functions: the product's NTT since r1l (-DMDN_GEN1 builds the first
-// generation of kernels.cu instead).  Same data layout, index conventions and results as the first generation in
-// kernels.cu (DESIGN.md "NTT index conventions"; reference: Radix2DitParallel::coset_lde_batch at
-// crates/lifted-stark/src/prover/commit.rs:173, quotient.rs:186-209), fewer instructions per point:
+// NTT block functions: the bodies of the NTT kernels of kernels.cu.  Data layout and index conventions in DESIGN.md
+// "NTT index conventions"; reference: Radix2DitParallel::coset_lde_batch at crates/lifted-stark/src/prover/commit.rs:173,
+// quotient.rs:186-209.  What keeps the instruction count per point down:
 //
 //   * the coset shift of the contiguous pass lives in the butterfly twiddles: stage s of the DIT over a
 //     chunk evaluates polynomials in y^(N2/2^(s+1)) at G^(N2/2^(s+1)) * w_{2^(s+1)}^j (G = g^N1), so a
 //     per-coset table of N2 - 1 "staged" twiddles replaces the premultiplication of every coefficient;
 //   * the remaining per-chunk scalar g^j1 / N rides on the inter-pass twiddle, which each lane advances
-//     geometrically (one multiplication to advance + one to apply per element, was four);
+//     geometrically (one multiplication to advance + one to apply per element);
 //   * butterflies keep lazy representatives: only the multiplied operand is canonicalised (x + c and x - c
 //     with c < p need a single carry fix each); values are canonicalised where they leave the transform;
 //   * in the round with the smallest spans of the plain-table transforms the unit twiddles are skipped.
@@ -169,7 +168,7 @@ GL_HD void dif_round(u64* x, const u64* tw, u32 m, u32 b, u32 log_cols) {
     NTT2_FOR(g, 1u << (m - LOGR + log_cols)) dif_group<LOGR, UNIT0>(x, tw, m, b, log_cols, g);
     NTT2_SYNC();
 }
-// radix-8 rounds, finishing with 4 + ... never 1 + 3: the same schedule as the first generation
+// radix-8 rounds, finishing with 4 + ... never 1 + 3
 template <bool STAGED>
 GL_HD void smem_dit(u64* x, const u64* tw, u32 m, u32 log_cols) {
     u32 b = 0;

@@ -25,9 +25,9 @@ inline std::vector<u64> powers(u64 base, size_t count) {
 struct NttHost {
     u32 n, n1, n2, lo_bits;
     std::vector<u64> data;
-    size_t o_tw1, o_tw2, o_twi1, o_twi2, o_lo, o_hi, o_ilo, o_ihi;
+    size_t o_tw1, o_twi1, o_twi2, o_lo, o_hi, o_ilo, o_ihi;
     mk::NttTables view(const u64* b) const {
-        return mk::NttTables{n, n1, n2, lo_bits, b + o_tw1, b + o_tw2, b + o_twi1, b + o_twi2, b + o_lo, b + o_hi, b + o_ilo, b + o_ihi};
+        return mk::NttTables{n, n1, n2, lo_bits, b + o_tw1, b + o_twi1, b + o_twi2, b + o_lo, b + o_hi, b + o_ilo, b + o_ihi};
     }
 };
 inline NttHost build_ntt(u32 n) {
@@ -42,7 +42,6 @@ inline NttHost build_ntt(u32 n) {
     };
     u64 w1 = gl::two_adic_generator(n1), w2 = gl::two_adic_generator(n2);
     h.o_tw1 = push(powers(w1, n1 ? (size_t)1 << (n1 - 1) : 1));
-    h.o_tw2 = push(powers(w2, n2 ? (size_t)1 << (n2 - 1) : 1));
     h.o_twi1 = push(powers(gl::inv(w1), n1 ? (size_t)1 << (n1 - 1) : 1));
     h.o_twi2 = push(powers(gl::inv(w2), n2 ? (size_t)1 << (n2 - 1) : 1));
     h.o_lo = push(powers(w, (size_t)1 << lo_bits));
@@ -53,13 +52,15 @@ inline NttHost build_ntt(u32 n) {
 }
 
 // Per coset base g of a size-2^n forward transform:
-//   tab_a[j2] = (g^N1)^j2, tab_b[j1] = g^j1 / N                       (first-generation premultiplication)
+//   tab_b[j1] = g^j1 / N
 //   tab_c[(1 << s) - 1 + j] = (g^N1)^(N2 / 2^(s+1)) * w_{2^(s+1)}^j,  s < n2, j < 2^s   (staged twiddles, ntt2.cuh)
+// A base's tab_c block is the source of a bulk copy (table_load, ntt2.cuh) when it is 16-byte aligned: the blocks start at
+// nb * N1 + b * N2 words, even unless N1 = 1 and nb is odd (then table_load falls back to a plain copy).
 struct PremulHost {
     u32 n_bases;
     std::vector<u64> data;
-    size_t o_a, o_b, o_c;
-    mk::PremulTables view(const u64* b) const { return mk::PremulTables{b + o_a, b + o_b, b + o_c}; }
+    size_t o_b, o_c;
+    mk::PremulTables view(const u64* b) const { return mk::PremulTables{b + o_b, b + o_c}; }
 };
 inline PremulHost build_premul(const std::vector<u64>& bases, u32 n) {
     u32 n1, n2; split_n(n, n1, n2);
@@ -67,13 +68,11 @@ inline PremulHost build_premul(const std::vector<u64>& bases, u32 n) {
     u64 n_inv = gl::inv((u64)1 << n);
     PremulHost h;
     h.n_bases = (u32)nb;
-    h.o_a = 0; h.o_b = nb * N2; h.o_c = nb * (N1 + N2);
-    h.data.assign(nb * (N1 + 2 * N2), 0);
+    h.o_b = 0; h.o_c = nb * N1;
+    h.data.assign(nb * (N1 + N2), 0);
     for (size_t b = 0; b < nb; b++) {
         u64 g = bases[b], gN1 = gl::exp_pow2(g, n1);
-        u64 x = 1;
-        for (size_t j2 = 0; j2 < N2; j2++) { h.data[h.o_a + b * N2 + j2] = x; x = gl::mul(x, gN1); }
-        x = n_inv;
+        u64 x = n_inv;
         for (size_t j1 = 0; j1 < N1; j1++) { h.data[h.o_b + b * N1 + j1] = x; x = gl::mul(x, g); }
         u64* tc = &h.data[h.o_c + b * N2];
         for (u32 s = 0; s < n2; s++) {

@@ -1,18 +1,19 @@
-// Second-generation lazy-reduction Goldilocks arithmetic + Poseidon2 (width 12) for the sm_90a
-// integer pipes: the product's arithmetic.  Same interface and same function values as
-// poseidon2_fast.cuh (the first generation, still built as libmiden_b200_gen1.so with -DMDN_GEN1); reference: crates/crypto/src/hash/algebraic_sponge/poseidon2/
-// mod.rs:226-319 (layer structure), constants.rs:18-31 (internal diagonal).
+// Lazy-reduction Goldilocks arithmetic + Poseidon2 (width 12) for the sm_90a integer pipes: the field
+// arithmetic of the hash and NTT kernels.  Same permutation as the canonical p2::permute (poseidon2.cuh) up to the
+// choice of representatives; reference: crates/crypto/src/hash/algebraic_sponge/poseidon2/mod.rs:226-319 (layer structure),
+// constants.rs:18-31 (internal diagonal).
 //
-// What changed against v1 (fewer SASS instructions per permutation):
+// What keeps the SASS instruction count per permutation down:
 //   * the 128-bit product comes from ONE unsigned __int128 multiplication (4 IMAD.WIDE + 3) instead
 //     of a separate mul.lo / mul.hi pair (11);
-//   * every "fold the carry back" is c * (2^32 - 1) + r as one IMAD.WIDE.U32 with a 64-bit addend;
+//   * every "fold the carry back" adds a 0 / 2^32 - 1 mask on the ALU pipe (fold);
 //   * the 4x4 MDS uses the 8-addition evaluation order (t01, t23, t0123, t01123, t01233);
 //   * negative diagonal entries subtract from (sum + 8p) instead of adding (8p - x);
-//   * x/4 and x/8 are one exact division by 2^k: (x + n p) >> k with n = -x mod 2^k.
+//   * x/4 and x/8 are one exact division by 2^k: (x + n p) >> k with n = -x mod 2^k;
+//   * the internal rounds reduce lanes 1..11 once every 8 rounds only (internal_rounds_lazy).
 //
-// Every function is __host__ __device__: the device side uses the carry flag through the same PTX
-// idioms v1 used (add.cc/addc, sub.cc/subc inside ONE asm statement), the host side restates each
+// Every function is __host__ __device__: the device side uses the carry flag through PTX idioms
+// (add.cc/addc, sub.cc/subc inside ONE asm statement), the host side restates each
 // primitive with unsigned __int128, so that tests/cpp/test_arith_v2.cpp runs THIS source on the CPU
 // against the canonical p2::permute and the reference's KAT.  Elements travel as arbitrary u64
 // representatives (value mod p, not necessarily < p); callers canonicalise what they store.
@@ -58,27 +59,9 @@ GL_HD u64 mul_eps(u32 a) {
 #endif
 }
 // c * (2^32 - 1) + r for c in {0, 1}.  Callers guarantee no overflow.  Added as the mask 0 / 2^32 - 1 on the ALU pipe:
-// the hash kernels are bound by the FMA-heavy pipe, where the IMAD.WIDE form of this fold costs four cycles per warp.
-// -DP2_FOLD_IMAD restores the one-instruction IMAD.WIDE.U32 form.
-GL_HD u64 fold(u32 c, u64 r) {
-#ifdef P2_FOLD_IMAD
-    return (u64)c * EPS + r;
-#else
-    return r + (u64)(0u - c);
-#endif
-}
-
-// The fold used by the linear layers (wred, add_const) adds the mask 0 / 2^32 - 1 on the ALU pipe: the kernels are bound
-// by the FMA-heavy pipe (an IMAD.WIDE costs ~1.6 plain IMADs there) and the ALU pipe has slack, so the 490 folds per
-// permutation outside the multiplications go there.
-// -DP2_LINEAR_FOLD_IMAD restores the IMAD.WIDE form.
-GL_HD u64 fold_lin(u32 c, u64 r) {
-#ifdef P2_LINEAR_FOLD_IMAD
-    return fold(c, r);
-#else
-    return r + (u64)(0u - c);
-#endif
-}
+// the hash kernels are bound by the FMA-heavy pipe, where the IMAD.WIDE form of this fold costs four cycles per warp
+// (~1.6 plain IMADs), and the ALU pipe has slack.
+GL_HD u64 fold(u32 c, u64 r) { return r + (u64)(0u - c); }
 
 GL_HD u64 canon(u64 x) { return x >= gl::P ? x - gl::P : x; }
 
@@ -102,7 +85,7 @@ GL_HD u64 sqr(u64 a) { return mul(a, a); }
 GL_HD u64 add_const(u64 x, u64 k) {
     u64 r; u32 c;
     addc64(x, k, r, c);
-    return fold_lin(c, r);
+    return fold(c, r);
 }
 
 // ---- 96-bit accumulators -------------------------------------------------------------------------
@@ -130,7 +113,7 @@ GL_HD W wsum(u64 a, u64 b) {
 // w - x for wide w >= x (the caller adds a multiple of p to w beforehand)
 GL_HD void wsub(W& w, W x) {
 #ifdef __CUDA_ARCH__
-    u64 lo; u32 hi;     // the asm template of the first generation's wsub
+    u64 lo; u32 hi;
     asm("sub.cc.u64 %0, %2, %3;\n\tsubc.u32 %1, %4, %5;" : "=l"(lo), "=r"(hi) : "l"(w.lo), "l"(x.lo), "r"(w.hi), "r"(x.hi));
     w.lo = lo; w.hi = hi;
 #else
@@ -143,7 +126,7 @@ GL_HD W wtriple(u64 x) { W w = wshl(x, 1); wadd(w, x); return w; }
 GL_HD u64 wred(W w) {
     u64 r; u32 c;
     addc64(w.lo, mul_eps(w.hi), r, c);
-    return fold_lin(c, r);
+    return fold(c, r);
 }
 static constexpr u64 P8_LO = 0xFFFFFFF800000008ull;   // 8p = 2^67 - 2^35 + 8
 static constexpr u32 P8_HI = 7u;
@@ -236,32 +219,6 @@ GL_HD void external_layer(u64* s) {
     }
 }
 
-// s_i <- d_i s_i + sum,  d = [-2, 1, 2, 1/2, 3, 4, -1/2, -3, -4, 1/4, -1/4, 1/8]
-GL_HD void internal_layer(u64* s) {
-    W sum = glf::wsum(s[0], s[1]);
-#pragma unroll
-    for (int i = 2; i < 12; i++) glf::wadd(sum, s[i]);
-    W sump = sum;                                   // sum + 8p: what the negative entries subtract from
-    { W p8; p8.lo = glf::P8_LO; p8.hi = glf::P8_HI; glf::wadd(sump, p8); }
-    W o;
-    u64 h3 = glf::half(s[3]), h6 = glf::half(s[6]);
-    u64 q9 = glf::div2k<2>(s[9]), q10 = glf::div2k<2>(s[10]);
-    u64 e11 = glf::div2k<3>(s[11]);
-    W t4 = glf::wtriple(s[4]), t7 = glf::wtriple(s[7]);
-    o = sump; glf::wsub(o, glf::wshl(s[0], 1)); s[0] = glf::wred(o);
-    o = sum; glf::wadd(o, s[1]); s[1] = glf::wred(o);
-    o = sum; glf::wadd(o, glf::wshl(s[2], 1)); s[2] = glf::wred(o);
-    o = sum; glf::wadd(o, h3); s[3] = glf::wred(o);
-    o = sum; glf::wadd(o, t4); s[4] = glf::wred(o);
-    o = sum; glf::wadd(o, glf::wshl(s[5], 2)); s[5] = glf::wred(o);
-    o = sump; glf::wsub(o, glf::wide(h6)); s[6] = glf::wred(o);
-    o = sump; glf::wsub(o, t7); s[7] = glf::wred(o);
-    o = sump; glf::wsub(o, glf::wshl(s[8], 2)); s[8] = glf::wred(o);
-    o = sum; glf::wadd(o, q9); s[9] = glf::wred(o);
-    o = sump; glf::wsub(o, glf::wide(q10)); s[10] = glf::wred(o);
-    o = sum; glf::wadd(o, e11); s[11] = glf::wred(o);
-}
-
 // The 22 internal rounds with lanes 1..11 kept as UNREDUCED 96-bit values (VERDICT r1 #7): only lane 0 enters an S-box, so only
 // lane 0 is reduced every round; the other lanes are reduced after every block of 8 rounds (8 + 8 + 6).  Bounds, with M_j the
 // bound of the lanes entering round j of a block (M_0 = 2^64): sum_j < 2^64 + 11 M_j, the subtracting lanes use
@@ -269,7 +226,6 @@ GL_HD void internal_layer(u64* s) {
 // 2^83.7, 2^87.6, 2^91.5, 2^95.5 < 2^96 (tests/cpp/test_arith_v2.cpp recomputes the table and tracks the largest value seen).
 // Per round this removes 11 of the 12 reductions (one IMAD.WIDE + five ALU instructions each) for one extra register per lane:
 // fewer SASS instructions and IMAD.WIDE per round (the FMA-heavy pipe is the binding one).
-// -DP2_EAGER_INTERNAL restores the round-by-round reduction.
 #define P2F_OFF_LO {0xfffffffb00000005ull, 0xffffffbb00000045ull, 0xfffffbfb00000405ull, 0xffffc3bb00003c45ull, \
                     0xfffc77fb00038805ull, 0xffcb07bb0034f845ull, 0xfce573fb031a8c05ull, 0xd171cbbb2e8e3445ull}
 #define P2F_OFF_HI {0x4u, 0x44u, 0x404u, 0x3c44u, 0x38804u, 0x34f844u, 0x31a8c04u, 0x2e8e3444u}
@@ -337,7 +293,7 @@ GL_HD void internal_rounds_lazy(u64* s, const u64* rc) {
 #define P2F_RC_INTERNAL p2::P2_RC_INTERNAL
 #endif
 
-// The 22 internal rounds stay a rolled loop (~26 KB of code; the first generation's fully unrolled 93 KB stalled on
+// The 22 internal rounds stay a rolled loop (~26 KB of code; a fully unrolled permutation, 93 KB, stalled on
 // instruction fetch).
 // Output words are arbitrary representatives; canonicalise with glf::canon before storing.
 GL_HD void permute(u64* s) {
@@ -351,17 +307,7 @@ GL_HD void permute(u64* s) {
             for (int i = 0; i < 12; i++) s[i] = sbox(glf::add_const(s[i], rc[12 * r + i]));
             external_layer(s);
         }
-        if (phase == 0) {
-#ifndef P2_EAGER_INTERNAL      // lazy: fewer IMAD.WIDE on the binding pipe, identical proof bytes
-            internal_rounds_lazy(s, P2F_RC_INTERNAL);
-#else
-#pragma unroll 1
-            for (int r = 0; r < 22; r++) {
-                s[0] = sbox(glf::add_const(s[0], P2F_RC_INTERNAL[r]));
-                internal_layer(s);
-            }
-#endif
-        }
+        if (phase == 0) internal_rounds_lazy(s, P2F_RC_INTERNAL);
     }
 }
 

@@ -2126,14 +2126,7 @@ long long mdn_get_info(mdn_session* s, mdn_info what, uint64_t* out, size_t cap)
             { size_t cap = 0; for (auto& sl : s->arena.slabs) cap += sl.size; v.push_back(cap); v.push_back(s->arena.slabs.size()); v.push_back(s->arena.grow_events); v.push_back(s->arena.live); }
             break;
         }
-        case MDN_INFO_BUILD: {
-#ifdef MDN_GEN1
-            v.push_back(1); v.push_back(1);
-#else
-            v.push_back(2); v.push_back(2);
-#endif
-            break;
-        }
+        case MDN_INFO_BUILD: v = {2, 2}; break;
         default: return -1;
     }
     if (out) for (size_t i = 0; i < v.size() && i < cap; i++) out[i] = v[i];

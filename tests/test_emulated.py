@@ -6,8 +6,7 @@ is host memory.  The same launch geometry, shared-memory tiles, barriers and hos
 these tests cover what the oracle tests cannot reach without a device: session.cu (phases, arena, tables, openings,
 staged API, error paths) and the index arithmetic of every kernel, against the oracle, bit for bit.  What they cannot
 show is listed in tests/emu/cuda_runtime.h (PTX carry primitives, hardware limits, races, speed); the real parity
-gate stays `-m gpu` on an H100.  The emulator builds the product's default (second-generation) kernels; the first-generation
-arithmetic of libmiden_b200_gen1.so is PTX-only and cannot be emulated.  binding.py refuses the emulator library unless MDN_ALLOW_EMULATOR=1."""
+gate stays `-m gpu` on an H100.  binding.py refuses the emulator library unless MDN_ALLOW_EMULATOR=1."""
 import os
 import subprocess
 import sys
@@ -21,8 +20,8 @@ EMU = os.path.join(ROOT, "tests", "emu")
 SKIP = "not 2_20 and not 2_21 and not 2_22 and not full_size and not sharded and not split_proof and not jit" + ("" if os.environ.get("MDN_EMU_FULL") else " and not 2_16")
 
 
-def _build(gen):
-    subprocess.check_call(["make", "-s", "-C", EMU, f"GEN={gen}"])
+def _build():
+    subprocess.check_call(["make", "-s", "-C", EMU])
     return os.path.join(EMU, "libmiden_b200_emu.so")
 
 
@@ -40,7 +39,7 @@ _jobs = {}
 
 def _suite(name):
     if not _jobs:
-        lib = _build("")
+        lib = _build()
         env = dict(os.environ, MDN_LIB_PATH=lib, MDN_ALLOW_EMULATOR="1")
         for key, (file, expr, tmo) in _SUITES.items():
             _jobs[key] = subprocess.Popen([sys.executable, "-m", "pytest", os.path.join(ROOT, "tests", file), "-q", "-m", "gpu", "-k", expr,
@@ -50,7 +49,7 @@ def _suite(name):
 
 
 def test_binding_refuses_the_emulator_without_opt_in():
-    lib = _build("")
+    lib = _build()
     env = dict(os.environ, MDN_LIB_PATH=lib)
     env.pop("MDN_ALLOW_EMULATOR", None)
     code = ("import sys; sys.path.insert(0, %r); import pkgload; B = pkgload.load_pkg().binding\n"
@@ -92,7 +91,7 @@ def test_one_proof_split_over_ranks_on_the_emulator(world, min_log):
     test_split_proof_matches_single_gpu).  min_log = 2 keeps even tiny FRI layers split, so the rank-local folds, the
     split FRI trees and the first-replicated-layer store are exercised at every round of a small proof; the stage
     outputs (roots, quotient accumulator, DEEP evaluations, FRI roots, query indices) are compared as well."""
-    lib = _build("")
+    lib = _build()
     env = dict(os.environ, MDN_LIB_PATH=lib, MDN_ALLOW_EMULATOR="1", MDN_EMU_SHM="1", SHARD_LOG_H="9", OMP_NUM_THREADS="1")
     env.pop("SHARD_BENCH", None)
     if min_log is not None:
@@ -110,7 +109,7 @@ def test_cpp_host_layer_prove_verify_tamper_on_the_emulator():
     """miden-vm_b200/host/miden_prover.hpp (the reference's prover interface restated in C++ above the C ABI) through its
     parity program tests/cpp/test_host_api.cpp, linked against the emulator: StarkConfig / ProverStatement /
     Preprocessed / ProverInstance::prove, verified by the oracle, tampered proofs rejected."""
-    _build("")
+    _build()
     cpp = os.path.join(ROOT, "tests", "cpp")
     subprocess.check_call(["make", "-s", "-C", os.path.join(ROOT, "oracle")])
     subprocess.check_call(["make", "-s", "-C", cpp, "test_host_api_emu"])
@@ -120,7 +119,7 @@ def test_cpp_host_layer_prove_verify_tamper_on_the_emulator():
 
 def test_graft_entry_smoke_on_the_emulator():
     """__graft_entry__.smoke() (one small proof through the C ABI, checked against the oracle) runs unchanged."""
-    lib = _build("")
+    lib = _build()
     env = dict(os.environ, MDN_LIB_PATH=lib, MDN_ALLOW_EMULATOR="1")
     r = subprocess.run([sys.executable, "-c", "import __graft_entry__ as g; g.smoke()"], env=env, capture_output=True, text=True, timeout=600, cwd=ROOT)
     assert r.returncode == 0 and "smoke ok" in r.stdout, r.stdout[-1500:] + r.stderr[-1500:]

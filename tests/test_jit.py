@@ -34,16 +34,6 @@ def test_jit_chunks_large_programs():
     _check(test_airs.big_program_workload(5, n_terms=60).programs[0])
 
 
-def test_jit_second_generation_multiplication_compiles(monkeypatch):
-    """MDN_JIT_ARITH=2 swaps the generated kernels' field multiplication for the second-generation one (one 128-bit
-    product; needs NVRTC's --device-int128).  Opt-in until it has been measured; this keeps it compiling."""
-    monkeypatch.setenv("MDN_JIT_ARITH", "2")
-    wl, _ = test_airs.logup_workload(5)
-    _check(wl.programs[0])
-    _check(wl._lookups[0][1])
-    _check(test_airs.big_program_workload(5, n_terms=60).programs[0])
-
-
 def test_jit_rejects_malformed_programs():
     good = test_airs.periodic_workload(5).programs[0]
     bad = good.copy(); bad[0] ^= 1
