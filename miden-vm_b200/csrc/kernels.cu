@@ -936,25 +936,9 @@ void launch_pow_bitrev(E2 y, u32 n, u64* wvec, u64* scratch, size_t p0, size_t c
     COUNT_LAUNCH(); COUNT_LAUNCH();
 }
 
-// 160-bit accumulator of unreduced 64 x 64 -> 128-bit products
-struct Acc160 { u64 lo, mid; u32 hi; };
-__device__ __forceinline__ void acc_mul(Acc160& A, u64 x, u64 y) {
-    unsigned __int128 q = (unsigned __int128)x * y;
-    u64 ql = (u64)q, qh = (u64)(q >> 64);
-#if defined(__CUDA_ARCH__)
-    asm("add.cc.u64 %0, %0, %3;\n\taddc.cc.u64 %1, %1, %4;\n\taddc.u32 %2, %2, 0;" : "+l"(A.lo), "+l"(A.mid), "+r"(A.hi) : "l"(ql), "l"(qh));
-#else
-    unsigned __int128 s0 = (unsigned __int128)A.lo + ql;
-    unsigned __int128 s1 = (unsigned __int128)A.mid + qh + (u64)(s0 >> 64);
-    A.lo = (u64)s0; A.mid = (u64)s1; A.hi += (u32)(s1 >> 64);
-#endif
-}
-// lo + mid * 2^64 + hi * 2^128 mod p, canonical.  2^64 = 2^32 - 1 and 2^96 = -1, so 2^128 = -2^32: the first two words go
-// through the ordinary 128-bit reduction, and hi * 2^32 (< p for every hi < 2^32) is subtracted.
-__device__ __forceinline__ u64 acc_reduce(const Acc160& A) {
-    u64 r = glf::canon_cc(glf::red128(A.lo, A.mid));
-    return glf::csub(r, (u64)A.hi << 32);
-}
+using glf::Acc160;      // 160-bit accumulator of unreduced products (poseidon2_fast2.cuh)
+using glf::acc_mul;
+using glf::acc_reduce;
 // Column dot products with the two weight vectors of an opening point pair: like k_deep, the 128-bit products are accumulated
 // unreduced (a thread adds chunk / 256 of them per accumulator) and reduced once; 2 columns x 4 weight coordinates per thread
 // (8 accumulators of five registers, 72 registers for sm_90a): one reduction per accumulator instead of one per product.

@@ -174,6 +174,26 @@ GL_HD W wdiv2k(W w) {
     return wshr96(w, K);
 }
 
+// ---- 160-bit accumulator of unreduced 64 x 64 -> 128-bit products (OOD dot products, DEEP quotient) ----------------
+struct Acc160 { u64 lo, mid; u32 hi; };
+GL_HD void acc_mul(Acc160& A, u64 x, u64 y) {
+    u128 q = (u128)x * y;
+    u64 ql = (u64)q, qh = (u64)(q >> 64);
+#if defined(__CUDA_ARCH__)
+    asm("add.cc.u64 %0, %0, %3;\n\taddc.cc.u64 %1, %1, %4;\n\taddc.u32 %2, %2, 0;" : "+l"(A.lo), "+l"(A.mid), "+r"(A.hi) : "l"(ql), "l"(qh));
+#else
+    u128 s0 = (u128)A.lo + ql;
+    u128 s1 = (u128)A.mid + qh + (u64)(s0 >> 64);
+    A.lo = (u64)s0; A.mid = (u64)s1; A.hi += (u32)(s1 >> 64);
+#endif
+}
+// lo + mid * 2^64 + hi * 2^128 mod p, canonical.  2^64 = 2^32 - 1 and 2^96 = -1, so 2^128 = -2^32: the first two words go
+// through the ordinary 128-bit reduction, and hi * 2^32 (< p for every hi < 2^32) is subtracted.
+GL_HD u64 acc_reduce(const Acc160& A) {
+    u64 r = canon_cc(red128(A.lo, A.mid));
+    return csub(r, (u64)A.hi << 32);
+}
+
 }  // namespace glf
 
 namespace p2f {
