@@ -146,9 +146,10 @@ void launch_transpose_slice_push(const u64* src_slice, const PeerPtrs& dst_cm, c
 //                  ->  natural k = k1*N2 + k2
 // =============================================================================================
 static constexpr int NTT_THREADS = 256;
-// one radix-8 group per thread when possible
-static inline unsigned ntt_threads(u32 m, u32 log_cols) {
-    u32 g = (m + log_cols >= 3) ? (1u << (m + log_cols - 3)) : 1u;
+// One group of the widest register round per thread when possible: 2^log_elems words (radix 8 in the run-time schedules,
+// ntt2::sched_log_elems in the compile-time ones, so that no thread idles in the round that holds the most registers).
+static inline unsigned ntt_threads(u32 m, u32 log_cols, u32 log_elems) {
+    u32 g = (m + log_cols >= log_elems) ? (1u << (m + log_cols - log_elems)) : 1u;
     if (g < 32) g = 32;
     if (g > 256) g = 256;
     return g;
@@ -188,14 +189,15 @@ __global__ void NTT_BOUNDS k_fwd_strided(const FwdItem* __restrict__ items, NttT
 template <int N1C, int N2C>
 static void launch_intt_t(u64* cols, size_t col_stride, u32 n_cols, const NttTables& T, u32 log_c, cudaStream_t st) {
     u32 N1 = 1u << T.n1, N2 = 1u << T.n2, C = 1u << log_c;
+    constexpr u32 LOG_E1 = N1C >= 0 ? ntt2::sched_log_elems(N1C) : 3, LOG_E2 = N2C >= 0 ? ntt2::sched_log_elems(N2C) : 3;
     if (T.n1 > 0) {
         size_t smem = ntt2::smem_words_strided(T.n1, log_c) * sizeof(u64);
         cudaFuncSetAttribute(k_intt_strided<N1C, N2C>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        k_intt_strided<N1C, N2C><<<dim3(N2 / C, n_cols), ntt_threads(T.n1, log_c), smem, st>>>(cols, col_stride, T, log_c);
+        k_intt_strided<N1C, N2C><<<dim3(N2 / C, n_cols), ntt_threads(T.n1, log_c, LOG_E1), smem, st>>>(cols, col_stride, T, log_c);
         COUNT_LAUNCH();
     }
     size_t smem = ntt2::smem_words_contig_inv(T.n2) * sizeof(u64);
-    k_intt_contig<N2C><<<dim3(N1, n_cols), ntt_threads(T.n2, 0), smem, st>>>(cols, col_stride, T);
+    k_intt_contig<N2C><<<dim3(N1, n_cols), ntt_threads(T.n2, 0, LOG_E2), smem, st>>>(cols, col_stride, T);
     COUNT_LAUNCH();
 }
 void launch_intt(u64* cols, size_t col_stride, u32 n_cols, const NttTables& T, cudaStream_t st) {
@@ -208,13 +210,14 @@ void launch_intt(u64* cols, size_t col_stride, u32 n_cols, const NttTables& T, c
 template <int N1C, int N2C>
 static void launch_fwd_t(const FwdItem* d_items, u32 n_items, const NttTables& T, const PremulTables& Pm, u32 log_c, cudaStream_t st) {
     u32 N1 = 1u << T.n1, N2 = 1u << T.n2, C = 1u << log_c;
+    constexpr u32 LOG_E1 = N1C >= 0 ? ntt2::sched_log_elems(N1C) : 3, LOG_E2 = N2C >= 0 ? ntt2::sched_log_elems(N2C) : 3;
     size_t smem = ntt2::smem_words_contig_fwd(T.n2) * sizeof(u64);
-    k_fwd_contig<N1C, N2C><<<dim3(N1, n_items), ntt_threads(T.n2, 0), smem, st>>>(d_items, T, Pm);
+    k_fwd_contig<N1C, N2C><<<dim3(N1, n_items), ntt_threads(T.n2, 0, LOG_E2), smem, st>>>(d_items, T, Pm);
     COUNT_LAUNCH();
     if (T.n1 > 0) {
         size_t smem2 = ntt2::smem_words_strided(T.n1, log_c) * sizeof(u64);
         cudaFuncSetAttribute(k_fwd_strided<N1C, N2C>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem2);
-        k_fwd_strided<N1C, N2C><<<dim3(N2 / C, n_items), ntt_threads(T.n1, log_c), smem2, st>>>(d_items, T, log_c);
+        k_fwd_strided<N1C, N2C><<<dim3(N2 / C, n_items), ntt_threads(T.n1, log_c, LOG_E1), smem2, st>>>(d_items, T, log_c);
         COUNT_LAUNCH();
     }
 }
