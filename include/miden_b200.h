@@ -6,7 +6,8 @@
  * (crates/lifted-stark/src/prover/mod.rs:139,157,230-578).  The Rust host keeps trace generation,
  * the AIR (lowered once to an op-list, see mdn_air.program), the LogUp aux-trace builder
  * (a callback) and wincode serialisation of the returned streams.  INTEGRATION.md shows the
- * Rust `extern "C"` binding.
+ * Rust `extern "C"` binding.  Beside the proof, mdn_check_constraints restates `debug::check_constraints`
+ * (crates/lifted-stark/src/debug.rs:70-214): every constraint on every trace row, no proof.
  *
  * Conventions
  *   - every field element is a canonical Goldilocks u64 (< 2^64 - 2^32 + 1); quadratic-extension
@@ -262,6 +263,41 @@ int mdn_prove_commit_aux(mdn_session* s, const mdn_matrix* aux /* instance order
                          const uint64_t* const* aux_values /* per instance, 2*num_aux_values */,
                          uint64_t aux_root[4]);
 int mdn_prove_finish(mdn_session* s, mdn_proof* out);
+
+/* ---- check every constraint on every row, without proving: debug::check_constraints ----------------------------
+ * (crates/lifted-stark/src/debug.rs:70-214; ExecutionTrace::check_constraints, processor/src/trace/mod.rs:251-278).
+ *   1. challenges: the caller's challenger (or the installed hash challenger for Blake3 / Keccak, as in mdn_prove)
+ *      observes observe_felts, the instance count and the log heights in instance order -- and NO commitment (neither
+ *      the preprocessed one nor any root) -- then max num_randomness EF challenges are sampled into randomness_out.
+ *      ExecutionTrace::check_constraints passes `config.challenger()` WITHOUT observe_protocol_params: the caller
+ *      chooses the seed, and the challenges need not equal those of a proof.
+ *   2. aux traces with those challenges: a lowered mdn_air.lookup is built on the device; otherwise `build_aux` is
+ *      called (host-resident traces only, as in mdn_prove); a NULL builder means all-zero aux traces and values.
+ *   3. the session's mdn_external_check, before the row checks (debug.rs:108-118): a non-zero assertion k makes
+ *      the report kind 2; the row checks still run so that failing_rows is filled.  A callback returning < 0
+ *      (ReductionError) makes the call return MDN_ERR_EXTERNAL_ASSERTION.
+ *   4. for every instance (instance order), row r < N and constraint k (emission order): next row (r + 1) mod N,
+ *      is_first = [r == 0], is_last = [r == N-1], is_transition = [r != N-1] exactly, periodic values = row
+ *      r mod 2^log_max_period of periodic_values, PREPROCESSED = rows r and next of `preprocessed`.  A constraint
+ *      fails when it is non-zero (in either coordinate); the first failure is the least (instance, row, k).
+ * Returns MDN_OK whenever the check ran, whatever it found; malformed input gets mdn_prove's statuses and messages.
+ * Refused before any device work: a call between mdn_prove_begin and mdn_prove_finish (MDN_ERR_INVALID_ARG) and a
+ * session split over ranks (MDN_ERR_UNSUPPORTED).  The check uses the proof arena and releases it; it changes nothing
+ * mdn_get_info / mdn_get_timings report about the last proof, and proofs after it are unchanged. */
+typedef struct {
+    uint32_t holds;          /* 1: every constraint is zero on every row and every external assertion is zero */
+    uint32_t kind;           /* 0 none, 1 AIR constraint, 2 external assertion: the failure the reference panics on first */
+    uint32_t instance;       /* kind 1: AIR index in INSTANCE order (statement order, not proof/height order) */
+    uint32_t constraint;     /* kind 1: emission index in the AIR's program; kind 2: assertion index */
+    uint64_t row;            /* kind 1 */
+    uint64_t value[2];       /* kind 1: EF value (c0, c1) of that constraint at that row; c1 = 0 for base constraints */
+    uint64_t failing_rows;   /* (instance, row) pairs, over all AIRs, where at least one constraint is non-zero */
+} mdn_constraint_report;
+int mdn_check_constraints(mdn_session* s, const mdn_statement* st, const mdn_matrix* traces,
+                          const mdn_matrix* preprocessed /* instance order, HOST, width 0 where none; NULL if no AIR declares any */,
+                          const mdn_challenger* challenger, mdn_aux_builder build_aux, void* aux_ctx,
+                          uint32_t flags, uint64_t* randomness_out /* 2*max num_randomness, may be NULL */,
+                          mdn_constraint_report* out);
 
 /* wincode/bincode-default layout of StarkProofData (prover/src/lib.rs:347-354): u64-LE length +
  * height bytes; u64-LE length + u64-LE felts; u64-LE length + 32-byte commitments.  Returns the

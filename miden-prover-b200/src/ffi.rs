@@ -143,6 +143,24 @@ pub type MdnExternalCheck = Option<
     ) -> c_int,
 >;
 
+/// `mdn_constraint_report`: the outcome of `mdn_check_constraints` (48 bytes).
+#[repr(C)]
+#[derive(Clone, Copy, Debug, Default)]
+pub struct MdnConstraintReport {
+    /// 1: every constraint is zero on every row and every external assertion is zero
+    pub holds: u32,
+    /// 0 none, 1 AIR constraint, 2 external assertion
+    pub kind: u32,
+    /// kind 1: AIR index in instance order
+    pub instance: u32,
+    /// kind 1: emission index in the AIR's program; kind 2: assertion index
+    pub constraint: u32,
+    pub row: u64,
+    /// kind 1: (c0, c1) of that constraint at that row
+    pub value: [u64; 2],
+    pub failing_rows: u64,
+}
+
 pub enum MdnSession {}
 
 /// `mdn_hash_kind` (include/miden_b200.h): which `miden_air::config` constructor the session follows.
@@ -197,6 +215,18 @@ unsafe extern "C" {
         aux_root: *mut u64,
     ) -> c_int;
     pub fn mdn_prove_finish(s: *mut MdnSession, out: *mut MdnProof) -> c_int;
+    pub fn mdn_check_constraints(
+        s: *mut MdnSession,
+        st: *const MdnStatement,
+        traces: *const MdnMatrix,
+        preprocessed: *const MdnMatrix,
+        challenger: *const MdnChallenger,
+        build_aux: MdnAuxBuilder,
+        aux_ctx: *mut c_void,
+        flags: u32,
+        randomness_out: *mut u64,
+        out: *mut MdnConstraintReport,
+    ) -> c_int;
     pub fn mdn_session_set_preprocessed(
         s: *mut MdnSession,
         st: *const MdnStatement,

@@ -334,6 +334,84 @@ impl<'s> GpuStarkProver<'s> {
             .collect();
         Ok(RawProof { log_trace_heights, fields, commitments })
     }
+
+    /// `debug::check_constraints(&statement, challenger)` (crates/lifted-stark/src/debug.rs:70-214) on the device: every
+    /// constraint of every AIR on every trace row, without proving.  Mirrors `ExecutionTrace::check_constraints`
+    /// (processor/src/trace/mod.rs:251-278), which passes `config.challenger()` WITHOUT `observe_protocol_params`; pass
+    /// the same here.  Panics with the reference's texts on the first failure.
+    pub fn check_constraints<MA, P>(&mut self, statement: &ProverStatement<Felt, QuadFelt, MA>, challenger: &DuplexChallenger<Felt, P, 12, 8>)
+    where
+        MA: MultiAir<Felt, QuadFelt>,
+    {
+        let traces: &[RowMajorMatrix<Felt>] = statement.traces();
+        let st = statement.statement();
+        let log_heights: Vec<u8> = traces.iter().map(|t| t.height().trailing_zeros() as u8).collect();
+        let lookup_structs: Vec<Option<MdnLookup>> = self
+            .lookups
+            .iter()
+            .map(|l| l.as_ref().map(|(n, prog)| MdnLookup { num_columns: *n, program_words: prog.len() as u32, program: prog.as_ptr() }))
+            .collect();
+        let airs: Vec<MdnAir> = self
+            .lowered
+            .iter()
+            .zip(&lookup_structs)
+            .map(|(a, lk)| MdnAir {
+                width: a.width,
+                aux_width: a.aux_width,
+                num_aux_values: a.num_aux_values,
+                num_randomness: a.num_randomness,
+                log_quotient_degree: a.log_quotient_degree,
+                program_words: a.program.len() as u32,
+                program: a.program.as_ptr(),
+                periodic_values: if a.periodic_values.is_empty() { ptr::null() } else { a.periodic_values.as_ptr() },
+                num_periodic_columns: a.num_periodic_columns,
+                log_max_period: a.log_max_period,
+                preprocessed_width: a.preprocessed_width,
+                lookup: lk.as_ref().map_or(ptr::null(), |l| l as *const MdnLookup),
+            })
+            .collect();
+        let mut rec = RecordingObserver::default();
+        st.observe(&mut rec, &log_heights);
+        let observe_felts: Vec<u64> = rec.felts.iter().map(Felt::as_canonical_u64).collect();
+        let public_values: Vec<u64> = st.air_inputs().iter().map(Felt::as_canonical_u64).collect();
+        let mats: Vec<MdnMatrix> = traces
+            .iter()
+            .map(|t| MdnMatrix { values: t.values.as_ptr() as *const u64, log_height: t.height().trailing_zeros(), width: t.width() as u32 })
+            .collect();
+        // BaseAir::preprocessed_trace per AIR, re-materialised as debug.rs does (width 0 where none)
+        let preps: Vec<Option<RowMajorMatrix<Felt>>> = st.airs().iter().map(|a| a.preprocessed_trace()).collect();
+        let prep_mats: Vec<MdnMatrix> = preps
+            .iter()
+            .map(|p| match p {
+                Some(m) => MdnMatrix { values: m.values.as_ptr() as *const u64, log_height: m.height().trailing_zeros(), width: m.width() as u32 },
+                None => MdnMatrix { values: ptr::null(), log_height: 0, width: 0 },
+            })
+            .collect();
+        let prep_ptr = if preps.iter().any(Option::is_some) { prep_mats.as_ptr() } else { ptr::null() };
+        let mdn_st = MdnStatement {
+            airs: airs.as_ptr(),
+            n_airs: traces.len() as u32,
+            public_values: public_values.as_ptr(),
+            n_public_values: public_values.len() as u32,
+            observe_felts: observe_felts.as_ptr(),
+            n_observe_felts: observe_felts.len() as u32,
+        };
+        let ch = challenger_state(challenger);
+        let mut ctx = CallbackCtx { statement };
+        let ctx_ptr = &mut ctx as *mut CallbackCtx<'_, MA> as *mut c_void;
+        unsafe { mdn_session_set_external_check(self.session.raw, Some(external_trampoline::<MA>), ctx_ptr) };
+        let mut rep = MdnConstraintReport::default();
+        let rc = unsafe {
+            mdn_check_constraints(self.session.raw, &mdn_st, mats.as_ptr(), prep_ptr, &ch, Some(aux_trampoline::<MA>), ctx_ptr, 0, ptr::null_mut(), &mut rep)
+        };
+        unsafe { mdn_session_set_external_check(self.session.raw, None, ptr::null_mut()) };
+        assert_eq!(rc, MDN_OK, "check_constraints failed: {}", last_error(self.session.raw));
+        match rep.kind {
+            2 => panic!("external assertion {} is non-zero", rep.constraint),                            // debug.rs:117
+            1 => panic!("constraint not satisfied at instance {}, row {}", rep.instance, rep.row),      // debug.rs:273-281
+            _ => {}
+        }
+    }
 }
 
 /// `StarkProofData`'s three streams as the C ABI returns them; a commitment is four u64 whatever the hash configuration.

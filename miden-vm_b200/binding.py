@@ -67,6 +67,12 @@ class Timings(C.Structure):
                 ("permutations", C.c_ulonglong), ("leaf_hash_bytes", C.c_double), ("ntt_bytes", C.c_double)]
 
 
+class ConstraintReport(C.Structure):
+    """`mdn_constraint_report`: the outcome of mdn_check_constraints (kind 1 = AIR constraint, 2 = external assertion)."""
+    _fields_ = [("holds", C.c_uint32), ("kind", C.c_uint32), ("instance", C.c_uint32), ("constraint", C.c_uint32),
+                ("row", C.c_uint64), ("value", C.c_uint64 * 2), ("failing_rows", C.c_uint64)]
+
+
 AUX_BUILDER = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_uint32, C.POINTER(Matrix), u64p, u64p, u64p)
 ALLGATHER = C.CFUNCTYPE(C.c_int, C.c_void_p, u64p, u64p, C.c_size_t)
 EXTERNAL_CHECK = C.CFUNCTYPE(C.c_int, C.c_void_p, u64p, C.c_uint32, C.POINTER(u64p), u32p, C.POINTER(C.c_uint8), C.c_uint32, u32p)
@@ -80,6 +86,7 @@ EXPORTS = [
     "mdn_challenger_observe", "mdn_challenger_sample", "mdn_set_debug", "mdn_session_set_shard",
     "mdn_session_set_preprocessed", "mdn_session_set_jit", "mdn_jit_compile_check", "mdn_jit_status", "mdn_abi_layout",
     "mdn_session_set_external_check", "mdn_session_set_hash", "mdn_session_set_hash_challenger",
+    "mdn_check_constraints",
 ]
 
 _lib = None
@@ -117,6 +124,9 @@ def lib():
         L.mdn_session_destroy.argtypes = [C.c_void_p]
         L.mdn_prove.argtypes = [C.c_void_p, C.POINTER(Statement), C.POINTER(Matrix), C.POINTER(Challenger),
                                 AUX_BUILDER, C.c_void_p, C.c_uint32, C.POINTER(Proof)]
+        L.mdn_check_constraints.argtypes = [C.c_void_p, C.POINTER(Statement), C.POINTER(Matrix), C.POINTER(Matrix),
+                                            C.POINTER(Challenger), AUX_BUILDER, C.c_void_p, C.c_uint32, u64p,
+                                            C.POINTER(ConstraintReport)]
         L.mdn_prove_begin.argtypes = [C.c_void_p, C.POINTER(Statement), C.POINTER(Matrix), C.POINTER(Challenger),
                                       C.c_uint32, u64p, u64p]
         L.mdn_prove_commit_aux.argtypes = [C.c_void_p, C.POINTER(Matrix), C.POINTER(u64p), u64p]
@@ -245,6 +255,20 @@ class Session:
         self._check(lib().mdn_prove(self._h, C.byref(statement), traces, C.byref(challenger) if challenger is not None else None, cb, None, flags,
                                     C.byref(proof)))
         return proof_to_numpy(proof)
+
+    def check_constraints(self, statement: Statement, traces, challenger: Challenger, aux_builder=None, preprocessed=None,
+                          flags=0):
+        """`debug::check_constraints(prover_statement, challenger)` on the device: every constraint of every AIR on
+        every trace row, without proving.  `preprocessed` = Matrix array in instance order (width 0 = none) or None.
+        Returns (ConstraintReport, randomness u64[2 * max num_randomness])."""
+        rep = ConstraintReport()
+        n_rand = max((statement.airs[i].num_randomness for i in range(statement.n_airs)), default=0)
+        rnd = np.zeros(max(1, 2 * n_rand), dtype=np.uint64)
+        cb = aux_builder if aux_builder is not None else C.cast(None, AUX_BUILDER)
+        self._check(lib().mdn_check_constraints(self._h, C.byref(statement), traces, preprocessed,
+                                                C.byref(challenger) if challenger is not None else None, cb, None, flags,
+                                                ptr(rnd), C.byref(rep)))
+        return rep, rnd[: 2 * n_rand]
 
     def info(self, what: int, cap: int = 0) -> np.ndarray:
         n = lib().mdn_get_info(self._h, what, None, 0)

@@ -838,6 +838,69 @@ int launch_logup_rows(const LogupArgs& a, cudaStream_t st) {
     return 0;
 }
 
+// =============================================================================================
+// Constraint check on the trace domain (debug.rs check_constraints): the constraint program of k_constraints, read
+// on raw rows with exact 0/1 selectors; FOLD k tests constraint k instead of folding it
+// =============================================================================================
+template <int MAXS>
+__global__ void __launch_bounds__(128) k_check_rows(CheckArgs a) {
+    size_t N = (size_t)1 << a.log_n;
+    size_t r = a.row0 + (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= a.row0 + a.n_rows) return;
+    size_t rn = (r + 1) & (N - 1);
+    E2 is_first = gl::e2(r == 0, 0), is_last = gl::e2(r == N - 1, 0), is_trans = gl::e2(r != N - 1, 0);
+    size_t per_row = (r & (((size_t)1 << a.prog.log_max_period) - 1)) * a.prog.n_periodic;
+    E2 slot[MAXS];
+    u32 k = 0, first_k = 0xFFFFFFFFu;
+    const uint4* code = reinterpret_cast<const uint4*>(a.prog.code);
+    for (u32 i = 0; i < a.prog.n_instr; i++) {
+        uint4 ins = code[i];
+        u32 op = ins.x & 0xff, ext = ins.x >> 8, x = ins.z, y = ins.w;
+        E2 v;
+        switch (op) {
+            case 0: v = gl::e2(a.main_cm[(size_t)y * N + (x ? rn : r)], 0); break;
+            case 1: { size_t p = x ? rn : r; v = gl::e2(a.aux_cm[(size_t)(2 * y) * N + p], a.aux_cm[(size_t)(2 * y + 1) * N + p]); break; }
+            case 2: v = gl::e2(a.publics[x], 0); break;
+            case 3: v = gl::e2(a.challenges[2 * x], a.challenges[2 * x + 1]); break;
+            case 4: v = gl::e2(a.aux_values[2 * x], a.aux_values[2 * x + 1]); break;
+            case 5: v = is_first; break;
+            case 6: v = is_last; break;
+            case 7: v = is_trans; break;
+            case 8: v = gl::e2(a.prog.consts[x], 0); break;
+            case 9: v = gl::e2(a.prog.consts[x], a.prog.consts[x + 1]); break;
+            case 10: v = ext ? gl::e2_add(slot[x], slot[y]) : gl::e2(gl::add(slot[x].a, slot[y].a), 0); break;
+            case 11: v = ext ? gl::e2_sub(slot[x], slot[y]) : gl::e2(gl::sub(slot[x].a, slot[y].a), 0); break;
+            case 12: v = ext ? gl::e2_mul(slot[x], slot[y]) : gl::e2(gl::mul(slot[x].a, slot[y].a), 0); break;
+            case 13: v = ext ? gl::e2_neg(slot[x]) : gl::e2(gl::neg(slot[x].a), 0); break;
+            case 14: v = gl::e2(a.prog.periodic[per_row + x], 0); break;
+            case 16: v = gl::e2(a.prep_cm[(size_t)y * N + (x ? rn : r)], 0); break;
+            default: {   // 15: the compiler places the k-th FOLD for constraint k (emission order)
+                E2 c = slot[x];
+                if (a.probe_value && k == a.probe_k) { a.probe_value[0] = c.a; a.probe_value[1] = c.b; }
+                if ((c.a | c.b) != 0 && first_k == 0xFFFFFFFFu) first_k = k;
+                k++;
+                continue;
+            }
+        }
+        slot[ins.y] = v;
+    }
+    if (first_k != 0xFFFFFFFFu) {
+        atomicMin(a.first, (unsigned long long)(((u64)r << 32) | first_k));
+        atomicAdd(a.failing_rows, 1ull);
+    }
+}
+int launch_check_rows(const CheckArgs& a, cudaStream_t st) {
+    if (a.n_rows == 0) return 0;
+    unsigned blocks = (unsigned)((a.n_rows + 127) / 128);
+    if (a.prog.n_slots <= 16) k_check_rows<16><<<blocks, 128, 0, st>>>(a);
+    else if (a.prog.n_slots <= 64) k_check_rows<64><<<blocks, 128, 0, st>>>(a);
+    else if (a.prog.n_slots <= 256) k_check_rows<256><<<blocks, 128, 0, st>>>(a);
+    else if (a.prog.n_slots <= 1024) k_check_rows<1024><<<blocks, 128, 0, st>>>(a);
+    else return -1;
+    COUNT_LAUNCH();
+    return 0;
+}
+
 // three-phase scan, 2048 rows per block (8 per thread): block totals -> serial scan of the (<= 2048) block
 // totals by one block -> per-block exclusive prefix with the block offset
 static constexpr int SCAN_T = 256, SCAN_E = 8, SCAN_B = SCAN_T * SCAN_E;

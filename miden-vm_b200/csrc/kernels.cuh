@@ -178,6 +178,28 @@ void launch_ef_exclusive_scan(const u64* totals, size_t n, u64* acc0, u64* acc1,
 static constexpr u32 LOGUP_MAX_COLS = 16;
 
 // ---------------------------------------------------------------------------------------------
+// Constraint check without proving (mdn_check_constraints; reference crates/lifted-stark/src/debug.rs:70-214)
+// ---------------------------------------------------------------------------------------------
+// The compiled constraint program evaluated on the TRACE domain, one thread per row r of [row0, row0 + n_rows):
+// MAIN / AUX / PREPROCESSED read rows r and (r + 1) mod N of the raw column-major buffers, PERIODIC reads row
+// r mod max_period of the raw periodic matrix, the selectors are exactly 0 or 1.  FOLD k (op 15) tests constraint k
+// instead of folding it: a row where some constraint is non-zero does atomicMin(first, row << 32 | k) with its lowest
+// such k and atomicAdd(failing_rows, 1).  With probe_value set, the thread of a row stores constraint probe_k's value.
+struct CheckArgs {
+    const u64* main_cm;      // raw main trace, column-major [col][row]
+    const u64* aux_cm;       // aux trace, column-major planes [2c + coord][row], or NULL (aux_width 0)
+    const u64* prep_cm;      // raw preprocessed trace, column-major, or NULL
+    u32 log_n;
+    AirDev prog;             // periodic = RAW periodic matrix, row-major (max_period x n_periodic)
+    const u64* publics; const u64* challenges; const u64* aux_values;   // device; EF pairs for the last two
+    size_t row0, n_rows;
+    unsigned long long* first;          // init ~0
+    unsigned long long* failing_rows;   // init 0
+    u32 probe_k; u64* probe_value;      // EF pair, or NULL
+};
+int launch_check_rows(const CheckArgs& a, cudaStream_t st);   // 0, or -1 when the program needs too many slots
+
+// ---------------------------------------------------------------------------------------------
 // DEEP / FRI / misc
 // ---------------------------------------------------------------------------------------------
 // wvec[i] = y^(bitrev_n(p0 + i)) for i < cnt  (EF interleaved; p0 = 0, cnt = 2^n: the whole vector);

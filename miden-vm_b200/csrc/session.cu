@@ -297,7 +297,7 @@ struct mdn_session {
     void build_tree(Committed& c);
     void lde_matrix(CommittedMat& m);
     void keep_raw_main(u32 j);
-    void build_logup_aux(u32 j, u64* aux_cm, u64 final_out[2]);
+    void build_logup_aux(u32 j, const u64* main_cm, u64* aux_cm, u64 final_out[2]);
     void lde_and_commit(Committed& c, float* t_lde, float* t_hash, bool lde_done = false);
     cudaStream_t copy_stream = nullptr;
     cudaEvent_t copy_ev[8];
@@ -307,6 +307,14 @@ struct mdn_session {
     void host_to_device(u64* dst, const u64* src, size_t n);
     void upload_matrix(const mdn_matrix& m, bool on_device, u64* dst_cm);
     void prove_begin(const mdn_statement* st, const mdn_matrix* traces, const mdn_challenger* ch, u32 flags);
+    void validate_statement(const mdn_statement* st, const mdn_matrix* traces, const mdn_challenger* ch);
+    void bind_airs(const mdn_statement* st, const mdn_matrix* traces, bool jit);
+    void bind_order(const mdn_statement* st, bool tables);
+    void bind_challenger(const mdn_challenger* ch);
+    void upload_and_commit_main(const mdn_matrix* traces, bool on_device);
+    int eval_external(u32* failed);
+    void check_constraints(const mdn_statement* st, const mdn_matrix* traces, const mdn_matrix* prep, const mdn_challenger* ch,
+                           mdn_aux_builder build_aux, void* aux_ctx, u32 flags, mdn_constraint_report* out);
     void commit_aux(const mdn_matrix* aux, const u64* const* aux_values, bool zero_aux);
     void finish();
     u64 grind(u32 bits);
@@ -863,16 +871,9 @@ void mdn_session::prove_begin(const mdn_statement* st, const mdn_matrix* traces,
     mk::reset_launch_count();
     prof.st = stream; prof.reset(); leaf_bytes = ntt_bytes = 0; perms = 0;
     if (!d_flag.p) { ArenaScope persistent(nullptr); d_flag.alloc(1, stream); CUDA_OK(cudaMemsetAsync(d_flag.p, 0, 8, stream)); }
-    if (!st || !traces || (!chal && !byte_hash())) fail(MDN_ERR_INVALID_ARG, "null argument");
-    if (st->n_airs == 0 || st->n_airs > 256) fail(MDN_ERR_INVALID_ARG, "AIR count must be in 1..=256");
-    if (params.log_folding_arity < 1 || params.log_folding_arity > 3) fail(MDN_ERR_INVALID_ARG, "invalid folding arity: log_arity %u (must be 1, 2, or 3)", params.log_folding_arity);
-    u32 lb = params.log_blowup;
-    if (lb == 0 || lb > 4) fail(MDN_ERR_UNSUPPORTED, "log_blowup must be in 1..=4");
-    if (st->n_public_values && !st->public_values) fail(MDN_ERR_INVALID_ARG, "public_values is NULL");
-    if (st->n_observe_felts && !st->observe_felts) fail(MDN_ERR_INVALID_ARG, "observe_felts is NULL");
-    for (u32 i = 0; i < st->n_public_values; i++) if (st->public_values[i] >= gl::P) fail(MDN_ERR_INVALID_ARG, "public value %u is not a canonical field element (>= p)", i);
-    for (u32 i = 0; i < st->n_observe_felts; i++) if (st->observe_felts[i] >= gl::P) fail(MDN_ERR_INVALID_ARG, "observed statement felt %u is not a canonical field element (>= p)", i);
+    validate_statement(st, traces, chal);
     bool on_device = (flags & MDN_FLAG_DEVICE_TRACES) != 0;
+    u32 lb = params.log_blowup;
     if (shard_world > 1) {
         if (!use_arena) fail(MDN_ERR_UNSUPPORTED, "a proof split over several ranks needs the proof arena (unset MDN_NO_ARENA)");
         if (lb < shard_log_g) fail(MDN_ERR_UNSUPPORTED, "a proof can be split over at most 2^log_blowup = %u ranks (one LDE coset each)", 1u << lb);
@@ -882,6 +883,55 @@ void mdn_session::prove_begin(const mdn_statement* st, const mdn_matrix* traces,
     CUDA_OK(cudaEventRecord(ev[0], stream));
 
     u32 k = st->n_airs;
+    bind_airs(st, traces, true);
+    // preprocessed presence / shape parity (ProverInstance::new, prover/mod.rs:139-153; validate_preprocessed,
+    // preprocessed.rs:147-260): a bundle must be installed exactly when some AIR declares preprocessed columns,
+    // and each committed trace must have its AIR's declared width and its main trace's height
+    {
+        bool expected = false;
+        for (u32 i = 0; i < k; i++) expected |= st->airs[i].preprocessed_width > 0;
+        if (expected != has_prep) fail(MDN_ERR_INVALID_ARG, "preprocessed presence mismatch: AIRs %s preprocessed columns but %s bundle is installed", expected ? "declare" : "declare no", has_prep ? "a" : "no");
+        if (has_prep) {
+            std::vector<int> idx(k, -1);
+            for (size_t q = 0; q < prep_air.size(); q++) { if (prep_air[q] >= k) fail(MDN_ERR_INVALID_ARG, "preprocessed bundle was built for a different AIR list"); idx[prep_air[q]] = (int)q; }
+            for (u32 i = 0; i < k; i++) {
+                bool want = st->airs[i].preprocessed_width > 0;
+                if (want != (idx[i] >= 0)) fail(MDN_ERR_INVALID_ARG, "AIR %u: preprocessed trace presence mismatch", i);
+                if (!want) continue;
+                if (prep_c.mats[idx[i]].width != st->airs[i].preprocessed_width) fail(MDN_ERR_INVALID_ARG, "AIR %u: preprocessed width %u does not match the declared %u", i, prep_c.mats[idx[i]].width, st->airs[i].preprocessed_width);
+                if (prep_log_h[idx[i]] != traces[i].log_height) fail(MDN_ERR_INVALID_ARG, "AIR %u: preprocessed height 2^%u differs from the main trace height 2^%u", i, prep_log_h[idx[i]], traces[i].log_height);
+            }
+        }
+    }
+    bind_order(st, true);
+
+    // challenger: caller's pre-bound state, then Statement::observe + observe_shape (mod.rs:290-291)
+    bind_challenger(chal);
+    Duplex& ch = tr.ch;
+    if (has_prep) ch.observe_digest(prep_c.root);   // preprocessed commitment first (mod.rs:282-286)
+    for (u32 i = 0; i < st->n_observe_felts; i++) ch.observe(st->observe_felts[i]);
+    ch.observe(k);
+    for (u32 i = 0; i < k; i++) ch.observe(log_heights[i]);
+    upload_and_commit_main(traces, on_device);
+}
+
+// argument checks of prove_begin, shared with check_constraints
+void mdn_session::validate_statement(const mdn_statement* st, const mdn_matrix* traces, const mdn_challenger* chal) {
+    if (!st || !traces || (!chal && !byte_hash())) fail(MDN_ERR_INVALID_ARG, "null argument");
+    if (st->n_airs == 0 || st->n_airs > 256) fail(MDN_ERR_INVALID_ARG, "AIR count must be in 1..=256");
+    if (params.log_folding_arity < 1 || params.log_folding_arity > 3) fail(MDN_ERR_INVALID_ARG, "invalid folding arity: log_arity %u (must be 1, 2, or 3)", params.log_folding_arity);
+    u32 lb = params.log_blowup;
+    if (lb == 0 || lb > 4) fail(MDN_ERR_UNSUPPORTED, "log_blowup must be in 1..=4");
+    if (st->n_public_values && !st->public_values) fail(MDN_ERR_INVALID_ARG, "public_values is NULL");
+    if (st->n_observe_felts && !st->observe_felts) fail(MDN_ERR_INVALID_ARG, "observe_felts is NULL");
+    for (u32 i = 0; i < st->n_public_values; i++) if (st->public_values[i] >= gl::P) fail(MDN_ERR_INVALID_ARG, "public value %u is not a canonical field element (>= p)", i);
+    for (u32 i = 0; i < st->n_observe_felts; i++) if (st->observe_felts[i] >= gl::P) fail(MDN_ERR_INVALID_ARG, "observed statement felt %u is not a canonical field element (>= p)", i);
+}
+
+// per-AIR shape checks, constraint program compilation and upload, lowered lookup programs.  `jit`: also load the
+// NVRTC kernels of large programs (the proof's constraint evaluation; a constraint check runs the interpreter only)
+void mdn_session::bind_airs(const mdn_statement* st, const mdn_matrix* traces, bool jit) {
+    u32 k = st->n_airs, lb = params.log_blowup;
     airs.resize(k); log_heights.resize(k);
     for (u32 i = 0; i < k; i++) {
         const mdn_air& a = st->airs[i];
@@ -945,7 +995,7 @@ void mdn_session::prove_begin(const mdn_statement* st, const mdn_matrix* traces,
         h.dev.log_max_period = a.log_max_period; h.dev.n_periodic = a.num_periodic_columns;
         // large programs: straight-line kernel compiled once per AIR (jit.hpp); the interpreter stays the fallback
         h.jit.reset(); h.n_constraints = a.program[3];
-        if (jit_min_nodes && a.program[2] >= jit_min_nodes) {
+        if (jit && jit_min_nodes && a.program[2] >= jit_min_nodes) {
             try {
                 u64 key = jit::fnv1a(a.program, a.program_words) ^ ((u64)a.program_words << 40);
                 auto it = jit_kernels.find(key);
@@ -980,7 +1030,7 @@ void mdn_session::prove_begin(const mdn_statement* st, const mdn_matrix* traces,
             h.lookup_dev.n_instr = (u32)(lc.code.size() / 4); h.lookup_dev.n_slots = std::max(1u, lc.n_slots);
             h.lookup_dev.log_max_period = a.log_max_period; h.lookup_dev.n_periodic = a.num_periodic_columns;
             h.lookup_jit.reset();
-            if (jit_min_nodes && lk.program[2] >= jit_min_nodes) {
+            if (jit && jit_min_nodes && lk.program[2] >= jit_min_nodes) {
                 try {
                     u64 key = jit::fnv1a(lk.program, lk.program_words) ^ ((u64)lk.program_words << 40) ^ 0x4C4B5550ull;
                     auto it = jit_kernels.find(key);
@@ -995,34 +1045,25 @@ void mdn_session::prove_begin(const mdn_statement* st, const mdn_matrix* traces,
             }
         }
     }
-    // preprocessed presence / shape parity (ProverInstance::new, prover/mod.rs:139-153; validate_preprocessed,
-    // preprocessed.rs:147-260): a bundle must be installed exactly when some AIR declares preprocessed columns,
-    // and each committed trace must have its AIR's declared width and its main trace's height
-    {
-        bool expected = false;
-        for (u32 i = 0; i < k; i++) expected |= st->airs[i].preprocessed_width > 0;
-        if (expected != has_prep) fail(MDN_ERR_INVALID_ARG, "preprocessed presence mismatch: AIRs %s preprocessed columns but %s bundle is installed", expected ? "declare" : "declare no", has_prep ? "a" : "no");
-        if (has_prep) {
-            std::vector<int> idx(k, -1);
-            for (size_t q = 0; q < prep_air.size(); q++) { if (prep_air[q] >= k) fail(MDN_ERR_INVALID_ARG, "preprocessed bundle was built for a different AIR list"); idx[prep_air[q]] = (int)q; }
-            for (u32 i = 0; i < k; i++) {
-                bool want = st->airs[i].preprocessed_width > 0;
-                if (want != (idx[i] >= 0)) fail(MDN_ERR_INVALID_ARG, "AIR %u: preprocessed trace presence mismatch", i);
-                if (!want) continue;
-                if (prep_c.mats[idx[i]].width != st->airs[i].preprocessed_width) fail(MDN_ERR_INVALID_ARG, "AIR %u: preprocessed width %u does not match the declared %u", i, prep_c.mats[idx[i]].width, st->airs[i].preprocessed_width);
-                if (prep_log_h[idx[i]] != traces[i].log_height) fail(MDN_ERR_INVALID_ARG, "AIR %u: preprocessed height 2^%u differs from the main trace height 2^%u", i, prep_log_h[idx[i]], traces[i].log_height);
-            }
-        }
-    }
+}
+
+// public values, TraceOrder and the NTT tables of every height (`tables` false: the height limit only, for a check)
+void mdn_session::bind_order(const mdn_statement* st, bool tables) {
+    u32 k = st->n_airs;
     publics.assign(st->public_values, st->public_values + st->n_public_values);
     // TraceOrder: stable sort on (log_height, instance)  (order.rs)
     order.resize(k);
     for (u32 i = 0; i < k; i++) order[i] = i;
     std::stable_sort(order.begin(), order.end(), [&](u32 a, u32 b) { return log_heights[a] < log_heights[b]; });
     log_max_n = log_heights[order.back()];
-    for (u32 i = 0; i < k; i++) ntt(log_heights[i]);   // validates the supported range early
+    for (u32 i = 0; i < k; i++) {
+        if (tables) ntt(log_heights[i]);   // validates the supported range early
+        else if (log_heights[i] > 22) fail(MDN_ERR_UNSUPPORTED, "trace height 2^%u exceeds the supported 2^22", log_heights[i]);
+    }
+}
 
-    // challenger: caller's pre-bound state, then Statement::observe + observe_shape (mod.rs:290-291)
+// the transcript starts from the caller's pre-bound challenger (duplex) or the installed hash challenger
+void mdn_session::bind_challenger(const mdn_challenger* chal) {
     Duplex& ch = tr.ch;
     ch.perm = perm();
     if (byte_hash()) {
@@ -1035,11 +1076,11 @@ void mdn_session::prove_begin(const mdn_statement* st, const mdn_matrix* traces,
         for (u32 i = 0; i < chal->input_len; i++) ch.in[i] = chal->input_buffer[i];
         ch.in_len = chal->input_len; ch.out_len = chal->output_len;
     }
-    if (has_prep) ch.observe_digest(prep_c.root);   // preprocessed commitment first (mod.rs:282-286)
-    for (u32 i = 0; i < st->n_observe_felts; i++) ch.observe(st->observe_felts[i]);
-    ch.observe(k);
-    for (u32 i = 0; i < k; i++) ch.observe(log_heights[i]);
+}
 
+// the rest of prove_begin: main traces committed, randomness sampled
+void mdn_session::upload_and_commit_main(const mdn_matrix* traces, bool on_device) {
+    u32 k = (u32)airs.size(), lb = params.log_blowup;
     // 1. upload + transpose main traces (proof order), LDE, LMCS  (mod.rs:326-341)
     size_t coef_total = 0, lde_total = 0;
     for (u32 j = 0; j < k; j++) {
@@ -1186,14 +1227,14 @@ void mdn_session::keep_raw_main(u32 j) {
 
 // build_logup_aux_trace (air/src/lookup/aux_builder.rs:49-97) for proof position j: fraction collection and
 // per-row sums on the trace domain, exclusive EF prefix sum into column 0, committed final = the grand total.
-void mdn_session::build_logup_aux(u32 j, u64* aux_cm, u64 final_out[2]) {
+void mdn_session::build_logup_aux(u32 j, const u64* main_cm, u64* aux_cm, u64 final_out[2]) {
     AirHost& h = airs[order[j]];
     u32 ln = log_heights[order[j]];
     size_t N = (size_t)1 << ln;
     DevBuf totals, scratch, fin;
     totals.alloc(2 * N, stream); scratch.alloc(2 * ((N + 2047) / 2048) + 2, stream); fin.alloc(2, stream);
     mk::LogupArgs la;
-    la.main_cm = h.raw_main.p; la.log_n = ln; la.n_cols = h.desc.aux_width; la.prog = h.lookup_dev;
+    la.main_cm = main_cm; la.log_n = ln; la.n_cols = h.desc.aux_width; la.prog = h.lookup_dev;
     la.publics = d_publics.p; la.challenges = d_randomness.p; la.aux_cm = aux_cm; la.totals = totals.p; la.bad_flag = (u32*)d_flag.p;
     {
         ProfScope ps(prof, PC_CONSTRAINTS);
@@ -1246,6 +1287,184 @@ void mdn_session::build_logup_aux(u32 j, u64* aux_cm, u64 final_out[2]) {
     }
 }
 
+// Statement::eval_external (statement.rs:94-110) on the current aux values, instance order: 0 when every assertion is
+// zero or no callback is installed, > 0 with *failed = the non-zero assertion, < 0 for a ReductionError
+int mdn_session::eval_external(u32* failed) {
+    if (!external_check) return 0;
+    u32 k = (u32)airs.size();
+    std::vector<std::vector<u64>> by_inst(k);
+    for (u32 j = 0; j < k; j++) by_inst[order[j]] = aux_values_p[j];
+    std::vector<const u64*> vp(k); std::vector<u32> vn(k); std::vector<uint8_t> lh(k);
+    for (u32 i = 0; i < k; i++) { vp[i] = by_inst[i].data(); vn[i] = (u32)by_inst[i].size() / 2; lh[i] = (uint8_t)log_heights[i]; }
+    return external_check(external_ctx, (const u64*)randomness.data(), (u32)randomness.size(), vp.data(), vn.data(), lh.data(), k, failed);
+}
+
+// ---------------------------------------------------------------------------------------------
+// check_constraints: every constraint of every AIR on every trace row, without a proof  (debug.rs:70-214)
+// ---------------------------------------------------------------------------------------------
+// The validation, program compilation and main-trace upload of prove_begin; challenges from the statement felts and
+// the instance shape only (no commitment is observed); aux traces from the device LogUp build, the host callback or
+// zeros; the session's external check; then k_check_rows per AIR in instance order.  Nothing of the last proof's
+// outputs, timings or introspection is touched; the caller releases the proof arena afterwards.
+void mdn_session::check_constraints(const mdn_statement* st, const mdn_matrix* traces, const mdn_matrix* prep, const mdn_challenger* chal,
+                                    mdn_aux_builder build_aux, void* aux_ctx, u32 flags, mdn_constraint_report* out) {
+    reset_proof();
+    prof.st = stream; prof.reset();
+    if (!d_flag.p) { ArenaScope persistent(nullptr); d_flag.alloc(1, stream); CUDA_OK(cudaMemsetAsync(d_flag.p, 0, 8, stream)); }
+    if (!out) fail(MDN_ERR_INVALID_ARG, "null argument");
+    validate_statement(st, traces, chal);
+    const bool on_device = (flags & MDN_FLAG_DEVICE_TRACES) != 0;
+    const u32 k = st->n_airs;
+    bind_airs(st, traces, false);
+    // the preprocessed traces come with the call (debug.rs re-materialises BaseAir::preprocessed_trace), not from the
+    // session's committed bundle
+    bool expected = false;
+    for (u32 i = 0; i < k; i++) expected |= st->airs[i].preprocessed_width > 0;
+    if (expected && !prep) fail(MDN_ERR_INVALID_ARG, "preprocessed presence mismatch: AIRs declare preprocessed columns but no preprocessed traces are given");
+    if (prep) for (u32 i = 0; i < k; i++) {
+        if (prep[i].width != st->airs[i].preprocessed_width) fail(MDN_ERR_INVALID_ARG, "AIR %u: preprocessed width %u does not match the declared %u", i, prep[i].width, st->airs[i].preprocessed_width);
+        if (!prep[i].width) continue;
+        if (!prep[i].values) fail(MDN_ERR_INVALID_ARG, "AIR %u: preprocessed matrix is NULL", i);
+        if (prep[i].log_height != traces[i].log_height) fail(MDN_ERR_INVALID_ARG, "AIR %u: preprocessed height 2^%u differs from the main trace height 2^%u", i, prep[i].log_height, traces[i].log_height);
+    }
+    if (build_aux && on_device) fail(MDN_ERR_UNSUPPORTED, "an aux builder needs host-resident main traces");
+    bind_order(st, false);
+
+    // challenges: Statement::observe + observe_shape, no commitment (debug.rs:87-97)
+    bind_challenger(chal);
+    for (u32 i = 0; i < st->n_observe_felts; i++) tr.ch.observe(st->observe_felts[i]);
+    tr.ch.observe(k);
+    for (u32 i = 0; i < k; i++) tr.ch.observe(log_heights[i]);
+    u32 max_rand = 0;
+    for (auto& a : airs) max_rand = std::max(max_rand, a.desc.num_randomness);
+    for (u32 i = 0; i < max_rand; i++) randomness.push_back(tr.ch.sample_ext());
+
+    // raw main traces, column-major, proof order (the layout build_logup_aux reads)
+    std::vector<u32> pos(k);
+    size_t main_total = 0, aux_total = 0;
+    for (u32 j = 0; j < k; j++) {
+        u32 inst = order[j];
+        pos[inst] = j;
+        size_t N = (size_t)1 << log_heights[inst];
+        main_total += N * airs[inst].desc.width; aux_total += N * 2 * airs[inst].desc.aux_width;
+    }
+    main_c.coef_buf.alloc(main_total, stream);
+    aux_c.coef_buf.alloc(aux_total, stream);
+    size_t co = 0, ao = 0;
+    for (u32 j = 0; j < k; j++) {
+        u32 inst = order[j];
+        size_t N = (size_t)1 << log_heights[inst];
+        main_c.mats.push_back(CommittedMat{nullptr, main_c.coef_buf.p + co, log_heights[inst], airs[inst].desc.width});
+        aux_c.mats.push_back(CommittedMat{nullptr, aux_c.coef_buf.p + ao, log_heights[inst], 2 * airs[inst].desc.aux_width});
+        co += N * airs[inst].desc.width; ao += N * 2 * airs[inst].desc.aux_width;
+    }
+    for (u32 j = 0; j < k; j++) upload_matrix(traces[order[j]], on_device, main_c.mats[j].coef);
+    check_input_flag("a main trace");
+    std::vector<DevBuf> prep_cm(k), periodic(k);
+    if (prep) {
+        for (u32 i = 0; i < k; i++) if (prep[i].width) {
+            prep_cm[i].alloc(((size_t)1 << prep[i].log_height) * prep[i].width, stream);
+            upload_matrix(prep[i], false, prep_cm[i].p);
+        }
+        check_input_flag("a preprocessed trace");
+    }
+    for (u32 i = 0; i < k; i++) {
+        const mdn_air& a = st->airs[i];
+        if (!a.num_periodic_columns) continue;
+        size_t n = ((size_t)1 << a.log_max_period) * a.num_periodic_columns;   // canonical: checked by bind_airs
+        periodic[i].alloc(n, stream);
+        CUDA_OK(cudaMemcpyAsync(periodic[i].p, a.periodic_values, n * sizeof(u64), cudaMemcpyHostToDevice, stream));
+    }
+
+    // aux traces built with those challenges (debug.rs:99-106), as mdn_prove builds them
+    std::vector<std::vector<u64>> aux_host(k), val_host(k);
+    if (build_aux) for (u32 i = 0; i < k; i++) {
+        const mdn_air& a = st->airs[i];
+        if (a.lookup) continue;   // built on the device
+        aux_host[i].assign(((size_t)1 << traces[i].log_height) * 2 * a.aux_width, 0);
+        val_host[i].assign(2 * (size_t)a.num_aux_values + 1, 0);
+        std::vector<u64> r;
+        for (u32 q = 0; q < a.num_randomness; q++) { r.push_back(randomness[q].a); r.push_back(randomness[q].b); }
+        r.push_back(0);
+        if (build_aux(aux_ctx, i, &traces[i], r.data(), aux_host[i].data(), val_host[i].data()) != 0)
+            fail(MDN_ERR_AUX_BUILDER, "aux builder failed for instance %u", i);
+    }
+    d_publics.alloc(std::max<size_t>(1, publics.size()), stream);
+    if (!publics.empty()) CUDA_OK(cudaMemcpyAsync(d_publics.p, publics.data(), publics.size() * sizeof(u64), cudaMemcpyHostToDevice, stream));
+    d_randomness.alloc(std::max<size_t>(1, 2 * randomness.size()), stream);
+    if (!randomness.empty()) CUDA_OK(cudaMemcpyAsync(d_randomness.p, randomness.data(), randomness.size() * sizeof(E2), cudaMemcpyHostToDevice, stream));
+    std::vector<u64> flat_values;
+    aux_values_p.assign(k, {}); aux_values_off.assign(k, 0);
+    for (u32 j = 0; j < k; j++) {
+        u32 inst = order[j];
+        AirHost& h = airs[inst];
+        u32 w = 2 * h.desc.aux_width;
+        size_t N = (size_t)1 << log_heights[inst];
+        u64 logup_final[2] = {0, 0};
+        if (h.has_lookup) build_logup_aux(j, main_c.mats[j].coef, aux_c.mats[j].coef, logup_final);   // no LDE: the buffer is raw
+        else if (w && build_aux) upload_matrix(mdn_matrix{aux_host[inst].data(), log_heights[inst], w}, false, aux_c.mats[j].coef);
+        else if (w) CUDA_OK(cudaMemsetAsync(aux_c.mats[j].coef, 0, N * w * sizeof(u64), stream));
+        aux_values_off[j] = flat_values.size();
+        for (u32 v = 0; v < 2 * h.desc.num_aux_values; v++) {
+            u64 x = h.has_lookup ? logup_final[v] : (build_aux ? val_host[inst][v] : 0);
+            if (x >= gl::P) fail(MDN_ERR_INVALID_ARG, "non-canonical aux value");
+            aux_values_p[j].push_back(x); flat_values.push_back(x);
+        }
+    }
+    if (build_aux) check_input_flag("an aux trace");
+    d_aux_values.alloc(std::max<size_t>(1, flat_values.size()), stream);
+    if (!flat_values.empty()) CUDA_OK(cudaMemcpyAsync(d_aux_values.p, flat_values.data(), flat_values.size() * sizeof(u64), cudaMemcpyHostToDevice, stream));
+
+    // external assertions before the row checks (debug.rs:108-118); a failing one is reported, the rows still run
+    u32 ext_failed = 0;
+    int ext_rc = eval_external(&ext_failed);
+    if (ext_rc < 0) fail(MDN_ERR_EXTERNAL_ASSERTION, "eval_external reported a reduction error");
+
+    // row checks (debug.rs:120-214): per AIR the lowest (row, constraint) that is non-zero and the failing-row count
+    DevBuf res; res.alloc(2 * (size_t)k + 4, stream);
+    std::vector<u64> host_res(2 * (size_t)k + 4, 0);
+    for (u32 i = 0; i < k; i++) host_res[2 * i] = ~0ull;
+    CUDA_OK(cudaMemcpyAsync(res.p, host_res.data(), host_res.size() * sizeof(u64), cudaMemcpyHostToDevice, stream));
+    std::vector<mk::CheckArgs> ca(k);
+    for (u32 i = 0; i < k; i++) {
+        u32 j = pos[i];
+        AirHost& h = airs[i];
+        mk::CheckArgs& c = ca[i];
+        c = mk::CheckArgs{};
+        c.main_cm = main_c.mats[j].coef;
+        c.aux_cm = h.desc.aux_width ? aux_c.mats[j].coef : nullptr;
+        c.prep_cm = prep_cm[i].p;
+        c.log_n = log_heights[i];
+        c.prog = h.dev;
+        c.prog.periodic = periodic[i].p;
+        c.publics = d_publics.p; c.challenges = d_randomness.p; c.aux_values = d_aux_values.p + aux_values_off[j];
+        c.row0 = 0; c.n_rows = (size_t)1 << log_heights[i];
+        c.first = (unsigned long long*)(res.p + 2 * i); c.failing_rows = (unsigned long long*)(res.p + 2 * i + 1);
+        if (mk::launch_check_rows(c, stream) != 0) fail(MDN_ERR_UNSUPPORTED, "AIR %u: constraint program too large for the interpreter", i);
+    }
+    CUDA_OK(cudaMemcpyAsync(host_res.data(), res.p, 2 * (size_t)k * sizeof(u64), cudaMemcpyDeviceToHost, stream));
+    CUDA_OK(cudaStreamSynchronize(stream));
+    CUDA_OK(cudaGetLastError());
+
+    memset(out, 0, sizeof *out);
+    for (u32 i = 0; i < k; i++) out->failing_rows += host_res[2 * i + 1];
+    if (ext_rc > 0) { out->kind = 2; out->constraint = ext_failed; }
+    else for (u32 i = 0; i < k; i++) {
+        u64 f = host_res[2 * i];
+        if (f == ~0ull) continue;
+        out->kind = 1; out->instance = i; out->row = f >> 32; out->constraint = (u32)f;
+        // the value: the same kernel on that one row, recording constraint K (its own atomics go to scratch words)
+        mk::CheckArgs c = ca[i];
+        c.row0 = out->row; c.n_rows = 1; c.probe_k = out->constraint; c.probe_value = res.p + 2 * (size_t)k;
+        c.first = (unsigned long long*)(res.p + 2 * (size_t)k + 2); c.failing_rows = (unsigned long long*)(res.p + 2 * (size_t)k + 3);
+        if (mk::launch_check_rows(c, stream) != 0) fail(MDN_ERR_UNSUPPORTED, "AIR %u: constraint program too large for the interpreter", i);
+        CUDA_OK(cudaMemcpyAsync(out->value, res.p + 2 * (size_t)k, 2 * sizeof(u64), cudaMemcpyDeviceToHost, stream));
+        CUDA_OK(cudaStreamSynchronize(stream));
+        break;
+    }
+    out->holds = ext_rc == 0 && out->failing_rows == 0;
+}
+
 // aux traces (instance order, EF flattened to base), aux values; commit + observe (mod.rs:397-422)
 void mdn_session::commit_aux(const mdn_matrix* aux, const u64* const* aux_values, bool zero_aux) {
     if (!in_proof) fail(MDN_ERR_INVALID_ARG, "commit_aux called outside a proof");
@@ -1275,7 +1494,7 @@ void mdn_session::commit_aux(const mdn_matrix* aux, const u64* const* aux_values
         aux_c.mats.push_back(CommittedMat{aux_c.lde_buf.p + lo, aux_c.coef_buf.p + co, log_heights[inst], w});
         u64 logup_final[2] = {0, 0};
         const bool dev_aux = airs[inst].has_lookup;
-        if (dev_aux) build_logup_aux(j, aux_c.coef_buf.p + co, logup_final);
+        if (dev_aux) build_logup_aux(j, airs[inst].raw_main.p, aux_c.coef_buf.p + co, logup_final);
         else if (w) {
             if (zero_aux) CUDA_OK(cudaMemsetAsync(aux_c.coef_buf.p + co, 0, N * w * sizeof(u64), stream));
             else {
@@ -1297,13 +1516,9 @@ void mdn_session::commit_aux(const mdn_matrix* aux, const u64* const* aux_values
     if (!zero_aux) check_input_flag("an aux trace");
     // Statement::eval_external on the aux values in instance order -- including the finals of aux traces built on the
     // device -- before anything is committed (prover/mod.rs:383-395, ProverError::ExternalAssertionFailed)
-    if (external_check) {
-        std::vector<std::vector<u64>> by_inst(k);
-        for (u32 j = 0; j < k; j++) by_inst[order[j]] = aux_values_p[j];
-        std::vector<const u64*> vp(k); std::vector<u32> vn(k); std::vector<uint8_t> lh(k);
-        for (u32 i = 0; i < k; i++) { vp[i] = by_inst[i].data(); vn[i] = (u32)by_inst[i].size() / 2; lh[i] = (uint8_t)log_heights[i]; }
+    {
         u32 failed = 0;
-        int rc = external_check(external_ctx, (const u64*)randomness.data(), (u32)randomness.size(), vp.data(), vn.data(), lh.data(), k, &failed);
+        int rc = eval_external(&failed);
         if (rc > 0) fail(MDN_ERR_EXTERNAL_ASSERTION, "external assertion %u failed", failed);
         if (rc < 0) fail(MDN_ERR_EXTERNAL_ASSERTION, "eval_external reported a reduction error");
     }
@@ -2002,6 +2217,24 @@ int mdn_prove(mdn_session* s, const mdn_statement* st, const mdn_matrix* traces,
     s->finish();
     fill_proof(s, out);
     s->release_proof_memory();
+    API_CATCH(s)
+}
+
+int mdn_check_constraints(mdn_session* s, const mdn_statement* st, const mdn_matrix* traces, const mdn_matrix* preprocessed,
+                          const mdn_challenger* challenger, mdn_aux_builder build_aux, void* aux_ctx, uint32_t flags,
+                          uint64_t* randomness_out, mdn_constraint_report* out) {
+    if (!s) return MDN_ERR_INVALID_ARG;
+    // refused before any device work, so that a staged proof in progress stays intact
+    if (s->in_proof) { s->error = "mdn_check_constraints called inside a proof (between mdn_prove_begin and mdn_prove_finish)"; return MDN_ERR_INVALID_ARG; }
+    if (s->shard_world > 1) { s->error = "mdn_check_constraints does not run on a session split over ranks (mdn_session_set_shard world > 1)"; return MDN_ERR_UNSUPPORTED; }
+    API_TRY(s)
+    {
+        ArenaScope proof_memory(s->use_arena ? &s->arena : nullptr);
+        CUDA_OK(cudaSetDevice(s->device));
+        s->check_constraints(st, traces, preprocessed, challenger, build_aux, aux_ctx, flags, out);
+        if (randomness_out) for (size_t i = 0; i < s->randomness.size(); i++) { randomness_out[2 * i] = s->randomness[i].a; randomness_out[2 * i + 1] = s->randomness[i].b; }
+    }
+    s->reset_proof();
     API_CATCH(s)
 }
 

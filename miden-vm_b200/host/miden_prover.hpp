@@ -14,6 +14,8 @@
 //   ProverInstance::new(&config, &prover_statement, preprocessed) miden::ProverInstance
 //   ProverInstance::prove(challenger) -> StarkOutput              ProverInstance::prove(challenger) -> StarkOutput
 //   StarkProofData { log_trace_heights, transcript }              miden::StarkProofData
+//   debug::check_constraints(&prover_statement, challenger)       miden::check_constraints(config, statement, challenger)
+//     (debug.rs:70-214; panics -> ConstraintViolation)             (every constraint on every row, on the device, no proof)
 //   ProverError::{Instance, Domain, ..}  prover/mod.rs:582-596    miden::ProverError { kind, what() }
 //   HashFunction::{Blake3_256, Keccak, Rpo256, Poseidon2, Rpx256} -> the config constructor (prover/src/lib.rs:245-301)
 //                                                                 miden::HashFunction + StarkConfig::with_hash
@@ -223,7 +225,56 @@ struct Lowered {                                   // C structs pointing into a 
 inline void check(const StarkConfig& c, int rc) {
     if (rc != MDN_OK) throw ProverError(ProverError::from_status(rc), mdn_last_error(c.session()));
 }
+// the mdn_aux_builder seam over an AuxBuilder
+struct AuxCall {
+    const ProverStatement* ps; const AuxBuilder* aux;
+    static int call(void* ctx, uint32_t instance, const mdn_matrix* main, const uint64_t* randomness, uint64_t* aux_out, uint64_t* aux_values) {
+        const AuxCall* self = (const AuxCall*)ctx;
+        try {
+            const Air& a = self->ps->statement.airs[instance];
+            std::vector<QuadFelt> ch(a.num_randomness);
+            for (uint32_t i = 0; i < a.num_randomness; i++) ch[i] = {randomness[2 * i], randomness[2 * i + 1]};
+            std::vector<Felt> flat((size_t(1) << main->log_height) * 2 * a.aux_width, 0);
+            std::vector<QuadFelt> vals(a.num_aux_values, QuadFelt{0, 0});
+            (*self->aux)(instance, self->ps->traces[instance], ch, flat, vals);
+            for (size_t i = 0; i < flat.size(); i++) aux_out[i] = flat[i];
+            for (size_t i = 0; i < vals.size(); i++) { aux_values[2 * i] = vals[i][0]; aux_values[2 * i + 1] = vals[i][1]; }
+            return 0;
+        } catch (...) { return -1; }
+    }
+};
 }  // namespace detail
+
+// The panic of debug::check_constraints as an exception, with the report of mdn_check_constraints
+struct ConstraintViolation : std::runtime_error {
+    mdn_constraint_report report;
+    explicit ConstraintViolation(const mdn_constraint_report& r) : std::runtime_error(message(r)), report(r) {}
+    static std::string message(const mdn_constraint_report& r) {
+        if (r.kind == 2) return "external assertion " + std::to_string(r.constraint) + " is non-zero";              // debug.rs:117
+        return "constraint not satisfied at instance " + std::to_string(r.instance) + ", row " + std::to_string(r.row);   // debug.rs:273-281
+    }
+};
+
+// debug::check_constraints(&prover_statement, challenger) (crates/lifted-stark/src/debug.rs:70-214): every constraint of every
+// AIR on every trace row, on the device, without proving.  Throws ConstraintViolation for the first failure the reference
+// panics on; ExecutionTrace::check_constraints passes config.challenger() without observe_protocol_params, so the caller
+// chooses the seed.  The preprocessed traces are the AIRs' own (Air::preprocessed_trace).
+inline void check_constraints(const StarkConfig& config, const ProverStatement& ps, Challenger challenger, AuxBuilder aux = nullptr) {
+    detail::Lowered low(ps.statement);
+    std::vector<mdn_matrix> mats, prep;
+    bool any_prep = false;
+    for (const RowMajorMatrix& t : ps.traces) mats.push_back(t.raw());
+    for (const Air& a : ps.statement.airs) {
+        prep.push_back(a.preprocessed_width ? a.preprocessed_trace.raw() : mdn_matrix{nullptr, 0, 0});
+        any_prep |= a.preprocessed_width > 0;
+    }
+    detail::AuxCall ctx{&ps, &aux};
+    mdn_constraint_report rep{};
+    detail::check(config, mdn_check_constraints(config.session(), &low.st, mats.data(), any_prep ? prep.data() : nullptr,
+                                                config.hash_challenger() ? nullptr : &challenger.raw, aux ? &detail::AuxCall::call : nullptr,
+                                                &ctx, 0, nullptr, &rep));
+    if (!rep.holds) throw ConstraintViolation(rep);
+}
 
 // Preprocessed::build(&statement, &config): the LDE tree lives on the device inside the config's session
 class Preprocessed {
@@ -266,8 +317,9 @@ public:
         std::vector<mdn_matrix> mats;
         for (const RowMajorMatrix& t : ps_.traces) mats.push_back(t.raw());
         mdn_proof proof{};
-        int rc = mdn_prove(config_.session(), &low.st, mats.data(), config_.hash_challenger() ? nullptr : &challenger.raw, aux_ ? &ProverInstance::trampoline : nullptr,
-                           (void*)this, 0, &proof);
+        detail::AuxCall ctx{&ps_, &aux_};
+        int rc = mdn_prove(config_.session(), &low.st, mats.data(), config_.hash_challenger() ? nullptr : &challenger.raw, aux_ ? &detail::AuxCall::call : nullptr,
+                           &ctx, 0, &proof);
         detail::check(config_, rc);
         StarkOutput out;
         out.proof.log_trace_heights.assign(proof.log_trace_heights, proof.log_trace_heights + proof.n_heights);
@@ -277,20 +329,6 @@ public:
         return out;
     }
 private:
-    static int trampoline(void* ctx, uint32_t instance, const mdn_matrix* main, const uint64_t* randomness, uint64_t* aux_out, uint64_t* aux_values) {
-        const ProverInstance* self = (const ProverInstance*)ctx;
-        try {
-            const Air& a = self->ps_.statement.airs[instance];
-            std::vector<QuadFelt> ch(a.num_randomness);
-            for (uint32_t i = 0; i < a.num_randomness; i++) ch[i] = {randomness[2 * i], randomness[2 * i + 1]};
-            std::vector<Felt> flat((size_t(1) << main->log_height) * 2 * a.aux_width, 0);
-            std::vector<QuadFelt> vals(a.num_aux_values, QuadFelt{0, 0});
-            self->aux_(instance, self->ps_.traces[instance], ch, flat, vals);
-            for (size_t i = 0; i < flat.size(); i++) aux_out[i] = flat[i];
-            for (size_t i = 0; i < vals.size(); i++) { aux_values[2 * i] = vals[i][0]; aux_values[2 * i + 1] = vals[i][1]; }
-            return 0;
-        } catch (...) { return -1; }
-    }
     const StarkConfig& config_; const ProverStatement& ps_; AuxBuilder aux_;
 };
 
