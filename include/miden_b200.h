@@ -14,7 +14,7 @@
  *     elements are two consecutive u64 (c0, c1), u^2 = 7 -- the layout of the reference's
  *     `Felt` / `QuadFelt` (crates/field/src/native/mod.rs:58, flatten_to_base order).
  *   - matrices are row-major exactly like p3 `RowMajorMatrix<Felt>`; the library transposes on
- *     the device.
+ *     the device.  Traces already on the device may also be column-major (MDN_FLAG_COLUMN_MAJOR).
  *   - functions return 0 on success and a negative mdn_status otherwise; the message is
  *     available through mdn_last_error().  Errors mirror `ProverError` / `ExecutionError::
  *     ProvingError(String)` (prover/mod.rs:582-596, prover/src/lib.rs:336-345).
@@ -161,7 +161,35 @@ typedef struct {
 
 enum {
     MDN_FLAG_DEVICE_TRACES = 1u,    /* trace matrices already resident in device memory */
+    MDN_FLAG_COLUMN_MAJOR = 2u,     /* with MDN_FLAG_DEVICE_TRACES only: the device matrices are column-major (below) */
 };
+
+/* ---- traces that already live on the GPU, column-major (MDN_FLAG_DEVICE_TRACES | MDN_FLAG_COLUMN_MAJOR) ----------
+ * Accepted by mdn_prove, mdn_prove_begin and mdn_check_constraints.  Each mdn_matrix.values is then a device pointer on
+ * the session's device, 16-byte aligned, and entry (row r, column c) is at values[(size_t)c << log_height | r] -- the
+ * layout a trace builder on the GPU writes naturally.  The library copies it into its coefficient buffer (no transpose;
+ * the per-kernel class 0 "transpose" of mdn_timings covers this ingest), a LogUp build (mdn_air.lookup) and the row
+ * checks of mdn_check_constraints read it in place, and nothing ever writes to it.  Lifetime: the buffers must stay
+ * valid and unchanged until mdn_prove / mdn_check_constraints returns; in the staged API until mdn_prove_commit_aux
+ * returns.  There, the `aux` matrices of mdn_prove_commit_aux are column-major device matrices too (aux_values stay on
+ * the host).  MDN_FLAG_COLUMN_MAJOR without MDN_FLAG_DEVICE_TRACES, or a misaligned pointer: MDN_ERR_INVALID_ARG.
+ * The preprocessed traces (mdn_session_set_preprocessed, mdn_check_constraints) stay host row-major.
+ *
+ * Aux traces of such calls come from the session's device aux builder, called in instance order for every AIR without
+ * mdn_air.lookup, after the randomness is sampled:
+ *   main       : the AIR's trace as passed (device, column-major)
+ *   randomness : host, 2 * num_randomness u64
+ *   aux_out    : device, column-major, 2 * aux_width columns of 2^log_height rows (EF flattened to base) -- the aux
+ *                coefficient slot of that AIR itself, NULL when aux_width is 0
+ *   aux_values : host, 2 * num_aux_values u64
+ *   stream     : the session's cudaStream_t.  The builder enqueues its work on it or finishes it before returning; the
+ *                library does not synchronise in between.  What it wrote is checked to be canonical.
+ * Return 0 on success; otherwise the call fails with MDN_ERR_AUX_BUILDER.  The `build_aux` argument of those calls
+ * must be NULL (MDN_ERR_INVALID_ARG otherwise).  With no device builder installed the aux traces and values are zero.
+ * Calls without MDN_FLAG_COLUMN_MAJOR never consult it.  fn = NULL removes it. */
+typedef int (*mdn_aux_builder_device)(void* ctx, uint32_t instance, const mdn_matrix* main, const uint64_t* randomness,
+                                      uint64_t* aux_out, uint64_t* aux_values, void* stream);
+int mdn_session_set_device_aux_builder(mdn_session* s, mdn_aux_builder_device fn, void* ctx);
 
 /* ---- session ------------------------------------------------------------------------------ */
 int mdn_session_create(const mdn_pcs_params* params, int cuda_device, mdn_session** out);
@@ -272,7 +300,9 @@ int mdn_prove_finish(mdn_session* s, mdn_proof* out);
  *      ExecutionTrace::check_constraints passes `config.challenger()` WITHOUT observe_protocol_params: the caller
  *      chooses the seed, and the challenges need not equal those of a proof.
  *   2. aux traces with those challenges: a lowered mdn_air.lookup is built on the device; otherwise `build_aux` is
- *      called (host-resident traces only, as in mdn_prove); a NULL builder means all-zero aux traces and values.
+ *      called (host-resident traces only, as in mdn_prove), or with MDN_FLAG_COLUMN_MAJOR the session's device aux
+ *      builder; no builder means all-zero aux traces and values.  Column-major device traces are checked and read in
+ *      place: nothing of them is uploaded or copied.
  *   3. the session's mdn_external_check, before the row checks (debug.rs:108-118): a non-zero assertion k makes
  *      the report kind 2; the row checks still run so that failing_rows is filled.  A callback returning < 0
  *      (ReductionError) makes the call return MDN_ERR_EXTERNAL_ASSERTION.
@@ -364,7 +394,7 @@ typedef struct {
     float h2d_transpose, commit_main, commit_aux, evaluate_constraints, commit_quotient, open, total;
     float lde_main, hash_main;          /* inside commit_main */
     /* per kernel class, summed over the last prove's launches (CUDA events on the session stream):
-     * 0 transpose, 1 NTT/LDE, 2 leaf sponge, 3 Merkle compress, 4 constraints, 5 OOD dot products,
+     * 0 transpose (or the ingest of column-major device traces), 1 NTT/LDE, 2 leaf sponge, 3 Merkle compress, 4 constraints, 5 OOD dot products,
      * 6 DEEP quotient, 7 FRI (leaf+compress+fold), 8 PoW grind, 9 opening gather */
     float kernel_ms[10];
     unsigned kernel_regions[10];        /* timed regions per class */

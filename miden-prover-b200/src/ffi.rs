@@ -18,6 +18,8 @@ pub const MDN_ERR_AUX_BUILDER: c_int = -5;
 pub const MDN_ERR_NO_DEVICE: c_int = -6;
 pub const MDN_ERR_EXTERNAL_ASSERTION: c_int = -7;
 pub const MDN_FLAG_DEVICE_TRACES: u32 = 1;
+/// With `MDN_FLAG_DEVICE_TRACES` only: the device matrices are column-major, entry (r, c) at `values[(c << log_height) | r]`.
+pub const MDN_FLAG_COLUMN_MAJOR: u32 = 2;
 
 #[repr(C)]
 #[derive(Clone, Copy, Debug)]
@@ -124,6 +126,19 @@ pub type MdnAuxBuilder = Option<
         randomness: *const u64,
         aux_out: *mut u64,
         aux_values: *mut u64,
+    ) -> c_int,
+>;
+/// `mdn_aux_builder_device`: the aux trace of a column-major device-trace call, written into `aux_out` (device,
+/// column-major) with work enqueued on `stream` (the session's `cudaStream_t`).
+pub type MdnAuxBuilderDevice = Option<
+    unsafe extern "C" fn(
+        ctx: *mut c_void,
+        instance: u32,
+        main: *const MdnMatrix,
+        randomness: *const u64,
+        aux_out: *mut u64,
+        aux_values: *mut u64,
+        stream: *mut c_void,
     ) -> c_int,
 >;
 /// Bootstrap transport of a proof split over several GPUs (`mdn_allgather_fn`).
@@ -235,6 +250,7 @@ unsafe extern "C" {
     ) -> c_int;
     pub fn mdn_session_set_shard(s: *mut MdnSession, rank: u32, world: u32, f: MdnAllgather, ctx: *mut c_void) -> c_int;
     pub fn mdn_session_set_external_check(s: *mut MdnSession, f: MdnExternalCheck, ctx: *mut c_void) -> c_int;
+    pub fn mdn_session_set_device_aux_builder(s: *mut MdnSession, f: MdnAuxBuilderDevice, ctx: *mut c_void) -> c_int;
     pub fn mdn_session_set_hash(s: *mut MdnSession, kind: c_int) -> c_int;
     pub fn mdn_session_set_hash_challenger(s: *mut MdnSession, c: *const MdnHashChallenger) -> c_int;
     pub fn mdn_session_set_jit(s: *mut MdnSession, min_nodes: u32) -> c_int;

@@ -76,7 +76,9 @@ class ConstraintReport(C.Structure):
 AUX_BUILDER = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_uint32, C.POINTER(Matrix), u64p, u64p, u64p)
 ALLGATHER = C.CFUNCTYPE(C.c_int, C.c_void_p, u64p, u64p, C.c_size_t)
 EXTERNAL_CHECK = C.CFUNCTYPE(C.c_int, C.c_void_p, u64p, C.c_uint32, C.POINTER(u64p), u32p, C.POINTER(C.c_uint8), C.c_uint32, u32p)
+DEVICE_AUX_BUILDER = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_uint32, C.POINTER(Matrix), u64p, C.c_void_p, u64p, C.c_void_p)
 FLAG_DEVICE_TRACES = 1
+FLAG_COLUMN_MAJOR = 2     # with FLAG_DEVICE_TRACES: device matrices are column-major, column c at values + (c << log_height)
 
 # Every symbol include/miden_b200.h declares (checked by tests/test_abi.py).
 EXPORTS = [
@@ -86,7 +88,7 @@ EXPORTS = [
     "mdn_challenger_observe", "mdn_challenger_sample", "mdn_set_debug", "mdn_session_set_shard",
     "mdn_session_set_preprocessed", "mdn_session_set_jit", "mdn_jit_compile_check", "mdn_jit_status", "mdn_abi_layout",
     "mdn_session_set_external_check", "mdn_session_set_hash", "mdn_session_set_hash_challenger",
-    "mdn_check_constraints",
+    "mdn_check_constraints", "mdn_session_set_device_aux_builder",
 ]
 
 _lib = None
@@ -143,6 +145,7 @@ def lib():
         L.mdn_session_set_hash.argtypes = [C.c_void_p, C.c_int]
         L.mdn_session_set_hash_challenger.argtypes = [C.c_void_p, C.POINTER(HashChallenger)]
         L.mdn_session_set_external_check.argtypes = [C.c_void_p, EXTERNAL_CHECK, C.c_void_p]
+        L.mdn_session_set_device_aux_builder.argtypes = [C.c_void_p, DEVICE_AUX_BUILDER, C.c_void_p]
         L.mdn_session_set_preprocessed.argtypes = [C.c_void_p, C.POINTER(Statement), C.POINTER(Matrix), u64p]
         L.mdn_abi_layout.restype = C.c_size_t
         L.mdn_abi_layout.argtypes = [u32p, C.c_size_t]
@@ -223,6 +226,28 @@ class Session:
             self._ext_cb = EXTERNAL_CHECK(tramp)
         self._check(lib().mdn_session_set_external_check(self._h, self._ext_cb, None))
 
+    def set_device_aux_builder(self, fn):
+        """Aux traces of FLAG_DEVICE_TRACES | FLAG_COLUMN_MAJOR calls (mdn_session_set_device_aux_builder):
+        fn(instance, main Matrix, randomness (u64 pointer, 2 * num_randomness words), aux_out device address (int, None
+        when aux_width is 0), stream handle (int)) -> the aux values, a sequence of 2 * num_aux_values ints.  aux_out
+        holds 2 * aux_width columns of 2^log_height rows, column-major; fn enqueues its writes on `stream` or finishes
+        them before returning.  None removes the builder."""
+        if fn is None:
+            self._dev_aux_cb = C.cast(None, DEVICE_AUX_BUILDER)
+        else:
+            def tramp(ctx, instance, main, randomness, aux_out, aux_values, stream):
+                try:
+                    vals = fn(instance, main.contents, randomness, aux_out, stream or 0)
+                    for i, v in enumerate(vals if vals is not None else ()):
+                        aux_values[i] = int(v)
+                    return 0
+                except Exception:
+                    import traceback
+                    traceback.print_exc()
+                    return -1
+            self._dev_aux_cb = DEVICE_AUX_BUILDER(tramp)
+        self._check(lib().mdn_session_set_device_aux_builder(self._h, self._dev_aux_cb, None))
+
     def set_hash(self, kind: int, challenger_input: bytes = b"", challenger_output: bytes = b""):
         """`blake3_256_config` / `keccak_config` instead of `poseidon2_config` (mdn_session_set_hash) + the pre-bound HashChallenger state."""
         self._check(lib().mdn_session_set_hash(self._h, kind))
@@ -283,6 +308,22 @@ class Session:
         t = Timings()
         self._check(lib().mdn_get_timings(self._h, C.byref(t)))
         return t
+
+
+def device_matrices(tensors):
+    """mdn_matrix array (instance order) over CUDA tensors of shape (width, N), 64-bit, contiguous: column-major
+    device traces for FLAG_DEVICE_TRACES | FLAG_COLUMN_MAJOR.  The tensors must outlive every call that uses the array
+    (the array keeps references to them)."""
+    mats = (Matrix * len(tensors))()
+    for i, t in enumerate(tensors):
+        if not t.is_cuda or t.dim() != 2 or t.element_size() != 8 or not t.is_contiguous():
+            raise ValueError(f"tensor {i}: need a contiguous 64-bit CUDA tensor of shape (width, N)")
+        width, n = t.shape
+        if n < 1 or n & (n - 1):
+            raise ValueError(f"tensor {i}: the height {n} is not a power of two")
+        mats[i] = Matrix(C.cast(C.c_void_p(t.data_ptr()), u64p), n.bit_length() - 1, width)
+    mats._keep = list(tensors)
+    return mats
 
 
 def proof_to_numpy(proof: Proof):

@@ -140,6 +140,45 @@ void launch_transpose_slice_push(const u64* src_slice, const PeerPtrs& dst_cm, c
 }
 
 // =============================================================================================
+// column-major ingest: a caller's device matrix (column c at c*N) -> its slot of a coefficient buffer
+// =============================================================================================
+// The layouts already agree, so this is a copy with the canonical check of k_transpose.  src == dst only checks (the
+// columns a device aux builder wrote into their slot) and stores nothing.  The caller's base pointer is 16-byte aligned;
+// a slot that follows a one-row matrix of odd width is not, and takes the scalar loop.
+__global__ void __launch_bounds__(256) k_ingest_cm(const u64* __restrict__ src, u64* __restrict__ dst, size_t n, u32* bad) {
+    const bool store = src != dst;
+    size_t stride = (size_t)gridDim.x * blockDim.x, i0 = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    bool any_bad = false;
+    if (((((size_t)src) | ((size_t)dst)) & 15) == 0) {
+        const ulonglong2* s2 = reinterpret_cast<const ulonglong2*>(src);
+        ulonglong2* d2 = reinterpret_cast<ulonglong2*>(dst);
+        for (size_t i = i0; i < n / 2; i += stride) {
+            ulonglong2 v = s2[i];
+            any_bad |= (v.x >= gl::P) | (v.y >= gl::P);
+            if (store) d2[i] = v;
+        }
+        if ((n & 1) && i0 == 0) {          // N = 1 with an odd width
+            u64 v = src[n - 1];
+            any_bad |= v >= gl::P;
+            if (store) dst[n - 1] = v;
+        }
+    } else {
+        for (size_t i = i0; i < n; i += stride) {
+            u64 v = src[i];
+            any_bad |= v >= gl::P;
+            if (store) dst[i] = v;
+        }
+    }
+    if (any_bad) atomicOr(bad, 1u);
+}
+void launch_ingest_cm(const u64* src_cm, u64* dst_cm, size_t n, u32* d_bad_flag, cudaStream_t st) {
+    if (!n) return;
+    unsigned blocks = (unsigned)std::min<size_t>((n / 2 + 255) / 256 + 1, 132 * 8);     // 8 blocks on each of the H100's 132 SMs
+    k_ingest_cm<<<blocks, 256, 0, st>>>(src_cm, dst_cm, n, d_bad_flag);
+    COUNT_LAUNCH();
+}
+
+// =============================================================================================
 // NTT.  N = N1 * N2.  Index conventions (see DESIGN.md "NTT"):
 //   inverse (DIF): natural j = j1*N2 + j2  ->  slot p = bitrev(k1)*N2 + bitrev(k2), k = k1 + N1*k2
 //   forward (DIT): slot p = p_hi*N2 + p_lo holds c[j], j = bitrev(p_lo)*N1 + bitrev(p_hi)

@@ -73,6 +73,9 @@ void launch_transpose_rm_to_cm(const u64* src_rm, u64* dst_cm, u32 n_rows, u32 w
 // rank (dst_cm.p[g], columns of height n_rows_total); a non-canonical value raises bit 0 of every rank's bad.p[g].
 void launch_transpose_slice_push(const u64* src_slice, const PeerPtrs& dst_cm, const PeerPtrs& bad, u32 world, u32 row0, u32 n_rows_slice,
                                  u32 n_rows_total, u32 width, cudaStream_t st);
+// n words of a column-major device matrix -> the same words of dst_cm, with 16-byte accesses where both pointers allow;
+// a non-canonical value raises bit 0 of *d_bad_flag.  src_cm == dst_cm: check only, nothing is stored.
+void launch_ingest_cm(const u64* src_cm, u64* dst_cm, size_t n, u32* d_bad_flag, cudaStream_t st);
 
 // In-place inverse NTT of `n_cols` columns (stride col_stride): natural evaluations over H ->
 // coefficients (unscaled by 1/N; the forward premul tables carry it), stored bit-reversed.

@@ -42,6 +42,19 @@ struct MdnError : std::runtime_error {
 }
 #define CUDA_OK(expr) do { cudaError_t e_ = (expr); if (e_ != cudaSuccess) fail(MDN_ERR_CUDA, "%s: %s (%s:%d)", #expr, cudaGetErrorString(e_), __FILE__, __LINE__); } while (0)
 
+// MDN_FLAG_COLUMN_MAJOR is set; it is only valid together with MDN_FLAG_DEVICE_TRACES
+bool column_major(uint32_t flags) {
+    if (!(flags & MDN_FLAG_COLUMN_MAJOR)) return false;
+    if (!(flags & MDN_FLAG_DEVICE_TRACES)) fail(MDN_ERR_INVALID_ARG, "MDN_FLAG_COLUMN_MAJOR is only valid together with MDN_FLAG_DEVICE_TRACES");
+    return true;
+}
+// a column-major device matrix with cells has a 16-byte aligned base pointer (the ingest reads it in 16-byte words)
+void check_column_major(const mdn_matrix& m, const char* what, uint32_t i) {
+    if (!m.width) return;
+    if (!m.values) fail(MDN_ERR_INVALID_ARG, "%s %u is NULL", what, i);
+    if ((uintptr_t)m.values & 15) fail(MDN_ERR_INVALID_ARG, "%s %u: a column-major device matrix must be 16-byte aligned", what, i);
+}
+
 std::string g_create_error;
 
 // Proof-lifetime device memory.  Every buffer a proof allocates is gone when the proof ends, and a prover proves
@@ -166,9 +179,11 @@ struct AirHost {
     DevBuf program;   // nodes | constraints | consts(lo,hi pairs as u64)
     mk::AirDev dev;
     // lowered LookupAir (mdn_air.lookup): compiled program, raw periodic matrix, and the raw column-major main
-    // trace kept from before the in-place inverse NTT (the LogUp fractions are evaluated on the trace domain)
+    // trace kept from before the in-place inverse NTT (the LogUp fractions are evaluated on the trace domain):
+    // raw_main_cm points at the copy in raw_main, or at the caller's column-major device trace (MDN_FLAG_COLUMN_MAJOR)
     bool has_lookup = false;
     DevBuf lookup_program, raw_main;
+    const u64* raw_main_cm = nullptr;
     mk::AirDev lookup_dev;
     // NVRTC-specialised constraint kernel (jit.hpp) for large programs; NULL = interpreter
     std::shared_ptr<jit::Kernel> jit, lookup_jit;
@@ -235,6 +250,7 @@ struct mdn_session {
         else mk::launch_compress_layer(children, parents, n, stream, perm());
     }
     mdn_external_check external_check = nullptr; void* external_ctx = nullptr;   // Statement::eval_external (mdn_session_set_external_check)
+    mdn_aux_builder_device dev_aux = nullptr; void* dev_aux_ctx = nullptr;        // mdn_session_set_device_aux_builder
     void shard_map_slab(char* base, size_t size);
     void shard_unmap_slabs();
     void shard_teardown();
@@ -255,6 +271,7 @@ struct mdn_session {
     bool use_arena = getenv("MDN_NO_ARENA") == nullptr;   // off: every buffer is its own allocation (compute-sanitizer memcheck)
     void release_proof_memory();
     bool in_proof = false;
+    bool col_major = false;                 // the proof's traces (and staged aux matrices) are column-major device buffers
     std::vector<AirHost> airs;              // instance order
     std::vector<u32> log_heights;           // instance order
     std::vector<u32> order;                 // proof position -> instance
@@ -296,7 +313,7 @@ struct mdn_session {
     PremulPlan& premul_quotient(u32 n, u32 log_d);
     void build_tree(Committed& c);
     void lde_matrix(CommittedMat& m);
-    void keep_raw_main(u32 j);
+    void keep_raw_main(u32 j, const u64* caller_cm);
     void build_logup_aux(u32 j, const u64* main_cm, u64* aux_cm, u64 final_out[2]);
     void lde_and_commit(Committed& c, float* t_lde, float* t_hash, bool lde_done = false);
     cudaStream_t copy_stream = nullptr;
@@ -305,7 +322,7 @@ struct mdn_session {
     u64* bounce[2] = {nullptr, nullptr}; cudaEvent_t bounce_ev[2]; bool bounce_busy[2] = {false, false};
     static constexpr size_t BOUNCE_WORDS = (size_t)4 << 20;   // 32 MiB each
     void host_to_device(u64* dst, const u64* src, size_t n);
-    void upload_matrix(const mdn_matrix& m, bool on_device, u64* dst_cm);
+    void upload_matrix(const mdn_matrix& m, bool on_device, u64* dst_cm, bool col_major = false);
     void prove_begin(const mdn_statement* st, const mdn_matrix* traces, const mdn_challenger* ch, u32 flags);
     void validate_statement(const mdn_statement* st, const mdn_matrix* traces, const mdn_challenger* ch);
     void bind_airs(const mdn_statement* st, const mdn_matrix* traces, bool jit);
@@ -315,7 +332,8 @@ struct mdn_session {
     int eval_external(u32* failed);
     void check_constraints(const mdn_statement* st, const mdn_matrix* traces, const mdn_matrix* prep, const mdn_challenger* ch,
                            mdn_aux_builder build_aux, void* aux_ctx, u32 flags, mdn_constraint_report* out);
-    void commit_aux(const mdn_matrix* aux, const u64* const* aux_values, bool zero_aux);
+    void commit_aux(const mdn_matrix* aux, const u64* const* aux_values, bool zero_aux, const mdn_matrix* builder_main = nullptr);
+    void call_device_aux_builder(u32 inst, const mdn_matrix& main, u64* aux_slot, std::vector<u64>& values);
     void finish();
     u64 grind(u32 bits);
     void reset_proof();
@@ -392,7 +410,7 @@ PremulPlan& mdn_session::premul_quotient(u32 n, u32 log_d) {
 }
 
 void mdn_session::reset_proof() {
-    in_proof = false; shard_active = false;
+    in_proof = false; shard_active = false; col_major = false;
     log_heights.clear(); order.clear(); publics.clear(); randomness.clear();
     aux_values_p.clear(); aux_values_off.clear();
     tr = Transcript();
@@ -541,10 +559,16 @@ void mdn_session::host_to_device(u64* dst, const u64* src, size_t n) {
     }
 }
 
-// row-major (host or device) -> column-major device
-void mdn_session::upload_matrix(const mdn_matrix& m, bool on_device, u64* dst_cm) {
+// row-major (host or device) or column-major (device) -> column-major device; a column-major matrix whose values are
+// dst_cm already is only checked
+void mdn_session::upload_matrix(const mdn_matrix& m, bool on_device, u64* dst_cm, bool col_major) {
     size_t N = (size_t)1 << m.log_height;
     if (m.width == 0) return;
+    if (col_major) {
+        ProfScope ps(prof, PC_TRANSPOSE);
+        mk::launch_ingest_cm(m.values, dst_cm, N * m.width, (u32*)d_flag.p, stream);
+        return;
+    }
     if (on_device) {
         ProfScope ps(prof, PC_TRANSPOSE);
         mk::launch_transpose_rm_to_cm(m.values, dst_cm, (u32)N, m.width, (u32*)d_flag.p, stream);
@@ -865,6 +889,7 @@ static Compiled compile_oplist(u32 i, const mdn_air& a, u32 n_publics, const u32
 // prove_begin: validation, statement/shape binding, main commit, randomness  (mod.rs:240-349)
 // ---------------------------------------------------------------------------------------------
 void mdn_session::prove_begin(const mdn_statement* st, const mdn_matrix* traces, const mdn_challenger* chal, u32 flags) {
+    const bool cm = column_major(flags);
     reset_proof();
     log_qd = 0;
     memset(&timings, 0, sizeof timings);
@@ -872,6 +897,8 @@ void mdn_session::prove_begin(const mdn_statement* st, const mdn_matrix* traces,
     prof.st = stream; prof.reset(); leaf_bytes = ntt_bytes = 0; perms = 0;
     if (!d_flag.p) { ArenaScope persistent(nullptr); d_flag.alloc(1, stream); CUDA_OK(cudaMemsetAsync(d_flag.p, 0, 8, stream)); }
     validate_statement(st, traces, chal);
+    if (cm) for (u32 i = 0; i < st->n_airs; i++) check_column_major(traces[i], "trace", i);
+    col_major = cm;
     bool on_device = (flags & MDN_FLAG_DEVICE_TRACES) != 0;
     u32 lb = params.log_blowup;
     if (shard_world > 1) {
@@ -1134,7 +1161,7 @@ void mdn_session::upload_and_commit_main(const mdn_matrix* traces, bool on_devic
             }
             shard_barrier();                   // every rank's slice of this matrix has arrived everywhere
             if (q + 1 == k) CUDA_OK(cudaEventRecord(ev[1], stream));
-            keep_raw_main(j);
+            keep_raw_main(j, nullptr);
             lde_matrix(cm);
         }
     } else if (!on_device) {
@@ -1157,13 +1184,15 @@ void mdn_session::upload_and_commit_main(const mdn_matrix* traces, bool on_devic
                 mk::launch_transpose_rm_to_cm(staging[j].p, main_c.mats[j].coef, 1u << main_c.mats[j].log_n, main_c.mats[j].width, (u32*)d_flag.p, stream);
             }
             if (q + 1 == k) CUDA_OK(cudaEventRecord(ev[1], stream));
-            keep_raw_main(j);
+            keep_raw_main(j, nullptr);
             lde_matrix(main_c.mats[j]);   // queued behind the copy of this matrix; overlaps the copy of the next one
         }
     } else {
-        for (u32 j = 0; j < k; j++) upload_matrix(traces[order[j]], true, main_c.mats[j].coef);
+        // device traces: a transpose (row-major) or an ingest (column-major) per matrix; a split proof does the same on
+        // every rank, each from its own whole copy.  A LogUp build reads a column-major trace where the caller keeps it.
+        for (u32 j = 0; j < k; j++) upload_matrix(traces[order[j]], true, main_c.mats[j].coef, col_major);
         CUDA_OK(cudaEventRecord(ev[1], stream));
-        for (u32 j = 0; j < k; j++) { keep_raw_main(j); lde_matrix(main_c.mats[j]); }
+        for (u32 j = 0; j < k; j++) { keep_raw_main(j, col_major ? traces[order[j]].values : nullptr); lde_matrix(main_c.mats[j]); }
     }
     staging.clear();
     check_input_flag("a main trace");
@@ -1216,13 +1245,17 @@ void mdn_session::set_preprocessed(const mdn_statement* st, const mdn_matrix* ma
     has_prep = true;
 }
 
-void mdn_session::keep_raw_main(u32 j) {
+// the raw main trace of a LogUp AIR for its aux build: the caller's column-major device trace when there is one (read in
+// place: the caller keeps it unchanged until the aux commit), otherwise a copy made before the in-place inverse NTT
+void mdn_session::keep_raw_main(u32 j, const u64* caller_cm) {
     AirHost& h = airs[order[j]];
     if (!h.has_lookup) return;
+    if (caller_cm) { h.raw_main_cm = caller_cm; return; }
     CommittedMat& m = main_c.mats[j];
     size_t n = ((size_t)1 << m.log_n) * m.width;
     h.raw_main.alloc(n, stream);
     CUDA_OK(cudaMemcpyAsync(h.raw_main.p, m.coef, n * sizeof(u64), cudaMemcpyDeviceToDevice, stream));
+    h.raw_main_cm = h.raw_main.p;
 }
 
 // build_logup_aux_trace (air/src/lookup/aux_builder.rs:49-97) for proof position j: fraction collection and
@@ -1308,12 +1341,15 @@ int mdn_session::eval_external(u32* failed) {
 // outputs, timings or introspection is touched; the caller releases the proof arena afterwards.
 void mdn_session::check_constraints(const mdn_statement* st, const mdn_matrix* traces, const mdn_matrix* prep, const mdn_challenger* chal,
                                     mdn_aux_builder build_aux, void* aux_ctx, u32 flags, mdn_constraint_report* out) {
+    const bool cm = column_major(flags);
     reset_proof();
     prof.st = stream; prof.reset();
     if (!d_flag.p) { ArenaScope persistent(nullptr); d_flag.alloc(1, stream); CUDA_OK(cudaMemsetAsync(d_flag.p, 0, 8, stream)); }
     if (!out) fail(MDN_ERR_INVALID_ARG, "null argument");
     validate_statement(st, traces, chal);
+    if (cm) for (u32 i = 0; i < st->n_airs; i++) check_column_major(traces[i], "trace", i);
     const bool on_device = (flags & MDN_FLAG_DEVICE_TRACES) != 0;
+    const bool dev_built = cm && dev_aux;   // aux traces from the device aux builder
     const u32 k = st->n_airs;
     bind_airs(st, traces, false);
     // the preprocessed traces come with the call (debug.rs re-materialises BaseAir::preprocessed_trace), not from the
@@ -1327,6 +1363,7 @@ void mdn_session::check_constraints(const mdn_statement* st, const mdn_matrix* t
         if (!prep[i].values) fail(MDN_ERR_INVALID_ARG, "AIR %u: preprocessed matrix is NULL", i);
         if (prep[i].log_height != traces[i].log_height) fail(MDN_ERR_INVALID_ARG, "AIR %u: preprocessed height 2^%u differs from the main trace height 2^%u", i, prep[i].log_height, traces[i].log_height);
     }
+    if (build_aux && cm) fail(MDN_ERR_INVALID_ARG, "with MDN_FLAG_COLUMN_MAJOR the aux traces come from the device aux builder (mdn_session_set_device_aux_builder): build_aux must be NULL");
     if (build_aux && on_device) fail(MDN_ERR_UNSUPPORTED, "an aux builder needs host-resident main traces");
     bind_order(st, false);
 
@@ -1339,7 +1376,8 @@ void mdn_session::check_constraints(const mdn_statement* st, const mdn_matrix* t
     for (auto& a : airs) max_rand = std::max(max_rand, a.desc.num_randomness);
     for (u32 i = 0; i < max_rand; i++) randomness.push_back(tr.ch.sample_ext());
 
-    // raw main traces, column-major, proof order (the layout build_logup_aux reads)
+    // raw main traces, column-major, proof order (the layout build_logup_aux reads); column-major device traces are
+    // read where the caller keeps them (only read: the const_cast feeds the common CommittedMat)
     std::vector<u32> pos(k);
     size_t main_total = 0, aux_total = 0;
     for (u32 j = 0; j < k; j++) {
@@ -1348,17 +1386,18 @@ void mdn_session::check_constraints(const mdn_statement* st, const mdn_matrix* t
         size_t N = (size_t)1 << log_heights[inst];
         main_total += N * airs[inst].desc.width; aux_total += N * 2 * airs[inst].desc.aux_width;
     }
-    main_c.coef_buf.alloc(main_total, stream);
+    if (!cm) main_c.coef_buf.alloc(main_total, stream);
     aux_c.coef_buf.alloc(aux_total, stream);
     size_t co = 0, ao = 0;
     for (u32 j = 0; j < k; j++) {
         u32 inst = order[j];
         size_t N = (size_t)1 << log_heights[inst];
-        main_c.mats.push_back(CommittedMat{nullptr, main_c.coef_buf.p + co, log_heights[inst], airs[inst].desc.width});
+        u64* main_cm = cm ? const_cast<u64*>(traces[inst].values) : main_c.coef_buf.p + co;
+        main_c.mats.push_back(CommittedMat{nullptr, main_cm, log_heights[inst], airs[inst].desc.width});
         aux_c.mats.push_back(CommittedMat{nullptr, aux_c.coef_buf.p + ao, log_heights[inst], 2 * airs[inst].desc.aux_width});
         co += N * airs[inst].desc.width; ao += N * 2 * airs[inst].desc.aux_width;
     }
-    for (u32 j = 0; j < k; j++) upload_matrix(traces[order[j]], on_device, main_c.mats[j].coef);
+    for (u32 j = 0; j < k; j++) upload_matrix(traces[order[j]], on_device, main_c.mats[j].coef, cm);   // column-major: check only
     check_input_flag("a main trace");
     std::vector<DevBuf> prep_cm(k), periodic(k);
     if (prep) {
@@ -1389,6 +1428,8 @@ void mdn_session::check_constraints(const mdn_statement* st, const mdn_matrix* t
         if (build_aux(aux_ctx, i, &traces[i], r.data(), aux_host[i].data(), val_host[i].data()) != 0)
             fail(MDN_ERR_AUX_BUILDER, "aux builder failed for instance %u", i);
     }
+    if (dev_built) for (u32 i = 0; i < k; i++)
+        if (!st->airs[i].lookup) call_device_aux_builder(i, traces[i], aux_c.mats[pos[i]].coef, val_host[i]);
     d_publics.alloc(std::max<size_t>(1, publics.size()), stream);
     if (!publics.empty()) CUDA_OK(cudaMemcpyAsync(d_publics.p, publics.data(), publics.size() * sizeof(u64), cudaMemcpyHostToDevice, stream));
     d_randomness.alloc(std::max<size_t>(1, 2 * randomness.size()), stream);
@@ -1402,16 +1443,17 @@ void mdn_session::check_constraints(const mdn_statement* st, const mdn_matrix* t
         size_t N = (size_t)1 << log_heights[inst];
         u64 logup_final[2] = {0, 0};
         if (h.has_lookup) build_logup_aux(j, main_c.mats[j].coef, aux_c.mats[j].coef, logup_final);   // no LDE: the buffer is raw
+        else if (w && dev_built) upload_matrix(mdn_matrix{aux_c.mats[j].coef, log_heights[inst], w}, true, aux_c.mats[j].coef, true);   // check only
         else if (w && build_aux) upload_matrix(mdn_matrix{aux_host[inst].data(), log_heights[inst], w}, false, aux_c.mats[j].coef);
         else if (w) CUDA_OK(cudaMemsetAsync(aux_c.mats[j].coef, 0, N * w * sizeof(u64), stream));
         aux_values_off[j] = flat_values.size();
         for (u32 v = 0; v < 2 * h.desc.num_aux_values; v++) {
-            u64 x = h.has_lookup ? logup_final[v] : (build_aux ? val_host[inst][v] : 0);
+            u64 x = h.has_lookup ? logup_final[v] : (build_aux || dev_built ? val_host[inst][v] : 0);
             if (x >= gl::P) fail(MDN_ERR_INVALID_ARG, "non-canonical aux value");
             aux_values_p[j].push_back(x); flat_values.push_back(x);
         }
     }
-    if (build_aux) check_input_flag("an aux trace");
+    if (build_aux || dev_built) check_input_flag("an aux trace");
     d_aux_values.alloc(std::max<size_t>(1, flat_values.size()), stream);
     if (!flat_values.empty()) CUDA_OK(cudaMemcpyAsync(d_aux_values.p, flat_values.data(), flat_values.size() * sizeof(u64), cudaMemcpyHostToDevice, stream));
 
@@ -1465,8 +1507,22 @@ void mdn_session::check_constraints(const mdn_statement* st, const mdn_matrix* t
     out->holds = ext_rc == 0 && out->failing_rows == 0;
 }
 
-// aux traces (instance order, EF flattened to base), aux values; commit + observe (mod.rs:397-422)
-void mdn_session::commit_aux(const mdn_matrix* aux, const u64* const* aux_values, bool zero_aux) {
+// mdn_aux_builder_device for instance `inst`: the aux columns go straight into `aux_slot` (column-major, on the session's
+// stream), the aux values into `values`
+void mdn_session::call_device_aux_builder(u32 inst, const mdn_matrix& main, u64* aux_slot, std::vector<u64>& values) {
+    const mdn_air& a = airs[inst].desc;
+    values.assign(2 * (size_t)a.num_aux_values + 1, 0);
+    std::vector<u64> r;
+    for (u32 q = 0; q < a.num_randomness; q++) { r.push_back(randomness[q].a); r.push_back(randomness[q].b); }
+    r.push_back(0);
+    if (dev_aux(dev_aux_ctx, inst, &main, r.data(), a.aux_width ? aux_slot : nullptr, values.data(), (void*)stream) != 0)
+        fail(MDN_ERR_AUX_BUILDER, "device aux builder failed for instance %u", inst);
+}
+
+// aux traces (instance order, EF flattened to base), aux values; commit + observe (mod.rs:397-422).  In a column-major
+// proof `aux` holds device matrices; `builder_main` (the proof's main traces) calls the device aux builder instead,
+// which writes every slot in place, so the ingest only checks them.
+void mdn_session::commit_aux(const mdn_matrix* aux, const u64* const* aux_values, bool zero_aux, const mdn_matrix* builder_main) {
     if (!in_proof) fail(MDN_ERR_INVALID_ARG, "commit_aux called outside a proof");
     u32 k = (u32)airs.size(), lb = params.log_blowup;
     CUDA_OK(cudaEventRecord(ev[3], stream));
@@ -1485,22 +1541,46 @@ void mdn_session::commit_aux(const mdn_matrix* aux, const u64* const* aux_values
     d_randomness.alloc(std::max<size_t>(1, 2 * randomness.size()), stream);
     if (!randomness.empty()) CUDA_OK(cudaMemcpyAsync(d_randomness.p, randomness.data(), randomness.size() * sizeof(E2), cudaMemcpyHostToDevice, stream));
     size_t co = 0, lo = 0;
-    std::vector<u64> flat_values;
-    aux_values_p.assign(k, {}); aux_values_off.assign(k, 0);
+    std::vector<u32> pos(k);
     for (u32 j = 0; j < k; j++) {
         u32 inst = order[j];
         size_t N = (size_t)1 << log_heights[inst];
         u32 w = 2 * airs[inst].desc.aux_width;
         aux_c.mats.push_back(CommittedMat{aux_c.lde_buf.p + lo, aux_c.coef_buf.p + co, log_heights[inst], w});
+        pos[inst] = j;
+        co += N * w; lo += (N << lb) * w;
+    }
+    // the device aux builder, instance order, for the AIRs without a lowered LookupAir
+    std::vector<mdn_matrix> built;
+    std::vector<std::vector<u64>> built_values;
+    std::vector<const u64*> built_ptrs;
+    if (builder_main) {
+        built.resize(k); built_values.resize(k); built_ptrs.assign(k, nullptr);
+        for (u32 i = 0; i < k; i++) {
+            if (airs[i].has_lookup) continue;
+            CommittedMat& m = aux_c.mats[pos[i]];
+            call_device_aux_builder(i, builder_main[i], m.coef, built_values[i]);
+            built[i] = mdn_matrix{m.coef, m.log_n, m.width};
+            built_ptrs[i] = built_values[i].data();
+        }
+        aux = built.data(); aux_values = built_ptrs.data(); zero_aux = false;
+    }
+    std::vector<u64> flat_values;
+    aux_values_p.assign(k, {}); aux_values_off.assign(k, 0);
+    for (u32 j = 0; j < k; j++) {
+        u32 inst = order[j];
+        u32 w = 2 * airs[inst].desc.aux_width;
+        CommittedMat& m = aux_c.mats[j];
         u64 logup_final[2] = {0, 0};
         const bool dev_aux = airs[inst].has_lookup;
-        if (dev_aux) build_logup_aux(j, airs[inst].raw_main.p, aux_c.coef_buf.p + co, logup_final);
+        if (dev_aux) build_logup_aux(j, airs[inst].raw_main_cm, m.coef, logup_final);
         else if (w) {
-            if (zero_aux) CUDA_OK(cudaMemsetAsync(aux_c.coef_buf.p + co, 0, N * w * sizeof(u64), stream));
+            if (zero_aux) CUDA_OK(cudaMemsetAsync(m.coef, 0, ((size_t)1 << m.log_n) * w * sizeof(u64), stream));
             else {
                 if (!aux[inst].values) fail(MDN_ERR_INVALID_ARG, "aux trace %u is NULL", inst);
                 if (aux[inst].width != w || aux[inst].log_height != log_heights[inst]) fail(MDN_ERR_INVALID_ARG, "aux trace %u has the wrong shape", inst);
-                upload_matrix(aux[inst], false, aux_c.coef_buf.p + co);
+                if (col_major && !builder_main) check_column_major(aux[inst], "aux trace", inst);
+                upload_matrix(aux[inst], col_major, m.coef, col_major);   // a builder's slot: check only
             }
         }
         u32 nav = airs[inst].desc.num_aux_values;
@@ -1511,7 +1591,6 @@ void mdn_session::commit_aux(const mdn_matrix* aux, const u64* const* aux_values
             if (x >= gl::P) fail(MDN_ERR_INVALID_ARG, "non-canonical aux value");
             aux_values_p[j].push_back(x); flat_values.push_back(x);
         }
-        co += N * w; lo += (N << lb) * w;
     }
     if (!zero_aux) check_input_flag("an aux trace");
     // Statement::eval_external on the aux values in instance order -- including the finals of aux traces built on the
@@ -2187,10 +2266,14 @@ int mdn_prove(mdn_session* s, const mdn_statement* st, const mdn_matrix* traces,
               mdn_aux_builder build_aux, void* aux_ctx, uint32_t flags, mdn_proof* out) {
     if (!s || !out) return MDN_ERR_INVALID_ARG;
     API_TRY(s)
+    const bool cm = column_major(flags);
+    if (cm && build_aux) fail(MDN_ERR_INVALID_ARG, "with MDN_FLAG_COLUMN_MAJOR the aux traces come from the device aux builder (mdn_session_set_device_aux_builder): build_aux must be NULL");
     ArenaScope proof_memory(s->use_arena ? &s->arena : nullptr);
     CUDA_OK(cudaSetDevice(s->device));
     s->prove_begin(st, traces, challenger, flags);
-    if (!build_aux) {
+    if (cm && s->dev_aux) {
+        s->commit_aux(nullptr, nullptr, false, traces);
+    } else if (!build_aux) {
         s->commit_aux(nullptr, nullptr, true);
     } else {
         if (flags & MDN_FLAG_DEVICE_TRACES) fail(MDN_ERR_UNSUPPORTED, "an aux builder needs host-resident main traces");
@@ -2426,6 +2509,12 @@ int mdn_session_set_hash_challenger(mdn_session* s, const mdn_hash_challenger* c
 int mdn_session_set_external_check(mdn_session* s, mdn_external_check fn, void* ctx) {
     if (!s) return MDN_ERR_INVALID_ARG;
     s->external_check = fn; s->external_ctx = ctx;
+    return MDN_OK;
+}
+
+int mdn_session_set_device_aux_builder(mdn_session* s, mdn_aux_builder_device fn, void* ctx) {
+    if (!s) return MDN_ERR_INVALID_ARG;
+    s->dev_aux = fn; s->dev_aux_ctx = fn ? ctx : nullptr;
     return MDN_OK;
 }
 

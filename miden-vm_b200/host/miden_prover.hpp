@@ -154,6 +154,32 @@ struct ProverStatement {
     }
 };
 
+// A trace that already lives on the GPU, column-major: entry (row r, column c) at values[(c << log_height) | r] on the
+// config's device, 16-byte aligned.  Not owned: it must stay valid and unchanged while a prove / check runs.
+struct ColumnMajorDeviceMatrix {
+    const Felt* values = nullptr;
+    uint32_t log_height = 0, width = 0;
+    size_t height() const { return size_t(1) << log_height; }
+    mdn_matrix raw() const { return {values, log_height, width}; }
+};
+
+// ProverStatement over device-resident column-major traces (MDN_FLAG_DEVICE_TRACES | MDN_FLAG_COLUMN_MAJOR)
+struct DeviceProverStatement {
+    Statement statement;
+    std::vector<ColumnMajorDeviceMatrix> traces;   // instance order
+    DeviceProverStatement(Statement s, std::vector<ColumnMajorDeviceMatrix> t) : statement(std::move(s)), traces(std::move(t)) {
+        if (traces.size() != statement.airs.size()) throw ProverError(ProverError::Instance, "trace count does not match the AIR count");
+        for (size_t i = 0; i < traces.size(); i++)
+            if (traces[i].width != statement.airs[i].width) throw ProverError(ProverError::Instance, "trace width does not match its AIR");
+    }
+};
+
+// LiftedAir::build_aux_trace on the GPU, for the AIRs that do not ship a lowered LookupAir: write the 2*aux_width base
+// columns of `aux_out` (device, column-major, height rows; nullptr when aux_width is 0) with work enqueued on `stream`
+// (the session's cudaStream_t) or finished before returning, and fill `aux_values`.
+using DeviceAuxBuilder = std::function<void(uint32_t instance, const ColumnMajorDeviceMatrix& main, const std::vector<QuadFelt>& challenges,
+                                            Felt* aux_out, std::vector<QuadFelt>& aux_values, void* stream)>;
+
 // GenericStarkConfig: PCS parameters + the pre-bound challenger prototype; owns the device session
 class StarkConfig {
 public:
@@ -243,6 +269,35 @@ struct AuxCall {
         } catch (...) { return -1; }
     }
 };
+// the mdn_aux_builder_device seam over a DeviceAuxBuilder, installed on the session for one call
+struct DeviceAuxCall {
+    const DeviceProverStatement* ps; const DeviceAuxBuilder* aux;
+    static int call(void* ctx, uint32_t instance, const mdn_matrix*, const uint64_t* randomness, uint64_t* aux_out, uint64_t* aux_values, void* stream) {
+        const DeviceAuxCall* self = (const DeviceAuxCall*)ctx;
+        try {
+            const Air& a = self->ps->statement.airs[instance];
+            std::vector<QuadFelt> ch(a.num_randomness);
+            for (uint32_t i = 0; i < a.num_randomness; i++) ch[i] = {randomness[2 * i], randomness[2 * i + 1]};
+            std::vector<QuadFelt> vals(a.num_aux_values, QuadFelt{0, 0});
+            (*self->aux)(instance, self->ps->traces[instance], ch, aux_out, vals, stream);
+            for (size_t i = 0; i < vals.size(); i++) { aux_values[2 * i] = vals[i][0]; aux_values[2 * i + 1] = vals[i][1]; }
+            return 0;
+        } catch (...) { return -1; }
+    }
+    struct Installed {       // the builder is a session setting: removed again when the call returns or throws
+        mdn_session* s;
+        Installed(mdn_session* s_, DeviceAuxCall* c) : s(s_) { if (*c->aux) mdn_session_set_device_aux_builder(s, &DeviceAuxCall::call, c); }
+        ~Installed() { mdn_session_set_device_aux_builder(s, nullptr, nullptr); }
+    };
+};
+inline StarkOutput to_output(const mdn_proof& proof) {
+    StarkOutput out;
+    out.proof.log_trace_heights.assign(proof.log_trace_heights, proof.log_trace_heights + proof.n_heights);
+    out.proof.transcript.fields.assign(proof.fields, proof.fields + proof.n_fields);
+    out.proof.transcript.commitments.resize(proof.n_commitments);
+    for (size_t i = 0; i < proof.n_commitments; i++) for (int k = 0; k < 4; k++) out.proof.transcript.commitments[i][k] = proof.commitments[4 * i + k];
+    return out;
+}
 }  // namespace detail
 
 // The panic of debug::check_constraints as an exception, with the report of mdn_check_constraints
@@ -273,6 +328,25 @@ inline void check_constraints(const StarkConfig& config, const ProverStatement& 
     detail::check(config, mdn_check_constraints(config.session(), &low.st, mats.data(), any_prep ? prep.data() : nullptr,
                                                 config.hash_challenger() ? nullptr : &challenger.raw, aux ? &detail::AuxCall::call : nullptr,
                                                 &ctx, 0, nullptr, &rep));
+    if (!rep.holds) throw ConstraintViolation(rep);
+}
+// The same check on device-resident column-major traces, read in place (nothing is uploaded or copied); the aux traces
+// come from `aux` on the device (none: zero aux traces).
+inline void check_constraints(const StarkConfig& config, const DeviceProverStatement& ps, Challenger challenger, DeviceAuxBuilder aux = nullptr) {
+    detail::Lowered low(ps.statement);
+    std::vector<mdn_matrix> mats, prep;
+    bool any_prep = false;
+    for (const ColumnMajorDeviceMatrix& t : ps.traces) mats.push_back(t.raw());
+    for (const Air& a : ps.statement.airs) {
+        prep.push_back(a.preprocessed_width ? a.preprocessed_trace.raw() : mdn_matrix{nullptr, 0, 0});
+        any_prep |= a.preprocessed_width > 0;
+    }
+    detail::DeviceAuxCall ctx{&ps, &aux};
+    detail::DeviceAuxCall::Installed installed(config.session(), &ctx);
+    mdn_constraint_report rep{};
+    detail::check(config, mdn_check_constraints(config.session(), &low.st, mats.data(), any_prep ? prep.data() : nullptr,
+                                                config.hash_challenger() ? nullptr : &challenger.raw, nullptr, nullptr,
+                                                MDN_FLAG_DEVICE_TRACES | MDN_FLAG_COLUMN_MAJOR, nullptr, &rep));
     if (!rep.holds) throw ConstraintViolation(rep);
 }
 
@@ -307,29 +381,44 @@ class ProverInstance {
 public:
     // `preprocessed` must be non-null exactly when some AIR declares preprocessed columns (PresenceMismatch otherwise)
     ProverInstance(const StarkConfig& config, const ProverStatement& ps, const Preprocessed* preprocessed, AuxBuilder aux = nullptr)
-        : config_(config), ps_(ps), aux_(std::move(aux)) {
-        bool expected = false;
-        for (const Air& a : ps.statement.airs) expected |= a.preprocessed_width > 0;
-        if (expected != (preprocessed != nullptr)) throw ProverError(ProverError::Instance, "preprocessed presence mismatch");
+        : config_(config), ps_(&ps), aux_(std::move(aux)) {
+        check_presence(ps.statement, preprocessed);
+    }
+    // device-resident column-major traces; the aux traces are built on the device by `aux` (none: zero aux traces)
+    ProverInstance(const StarkConfig& config, const DeviceProverStatement& ps, const Preprocessed* preprocessed, DeviceAuxBuilder aux = nullptr)
+        : config_(config), dps_(&ps), dev_aux_(std::move(aux)) {
+        check_presence(ps.statement, preprocessed);
     }
     StarkOutput prove(const Challenger& challenger) const {
-        detail::Lowered low(ps_.statement);
-        std::vector<mdn_matrix> mats;
-        for (const RowMajorMatrix& t : ps_.traces) mats.push_back(t.raw());
         mdn_proof proof{};
-        detail::AuxCall ctx{&ps_, &aux_};
-        int rc = mdn_prove(config_.session(), &low.st, mats.data(), config_.hash_challenger() ? nullptr : &challenger.raw, aux_ ? &detail::AuxCall::call : nullptr,
-                           &ctx, 0, &proof);
+        const mdn_challenger* ch = config_.hash_challenger() ? nullptr : &challenger.raw;
+        if (dps_) {
+            detail::Lowered low(dps_->statement);
+            std::vector<mdn_matrix> mats;
+            for (const ColumnMajorDeviceMatrix& t : dps_->traces) mats.push_back(t.raw());
+            detail::DeviceAuxCall ctx{dps_, &dev_aux_};
+            detail::DeviceAuxCall::Installed installed(config_.session(), &ctx);
+            detail::check(config_, mdn_prove(config_.session(), &low.st, mats.data(), ch, nullptr, nullptr,
+                                             MDN_FLAG_DEVICE_TRACES | MDN_FLAG_COLUMN_MAJOR, &proof));
+            return detail::to_output(proof);
+        }
+        detail::Lowered low(ps_->statement);
+        std::vector<mdn_matrix> mats;
+        for (const RowMajorMatrix& t : ps_->traces) mats.push_back(t.raw());
+        detail::AuxCall ctx{ps_, &aux_};
+        int rc = mdn_prove(config_.session(), &low.st, mats.data(), ch, aux_ ? &detail::AuxCall::call : nullptr, &ctx, 0, &proof);
         detail::check(config_, rc);
-        StarkOutput out;
-        out.proof.log_trace_heights.assign(proof.log_trace_heights, proof.log_trace_heights + proof.n_heights);
-        out.proof.transcript.fields.assign(proof.fields, proof.fields + proof.n_fields);
-        out.proof.transcript.commitments.resize(proof.n_commitments);
-        for (size_t i = 0; i < proof.n_commitments; i++) for (int k = 0; k < 4; k++) out.proof.transcript.commitments[i][k] = proof.commitments[4 * i + k];
-        return out;
+        return detail::to_output(proof);
     }
 private:
-    const StarkConfig& config_; const ProverStatement& ps_; AuxBuilder aux_;
+    static void check_presence(const Statement& s, const Preprocessed* preprocessed) {
+        bool expected = false;
+        for (const Air& a : s.airs) expected |= a.preprocessed_width > 0;
+        if (expected != (preprocessed != nullptr)) throw ProverError(ProverError::Instance, "preprocessed presence mismatch");
+    }
+    const StarkConfig& config_;
+    const ProverStatement* ps_ = nullptr; AuxBuilder aux_;
+    const DeviceProverStatement* dps_ = nullptr; DeviceAuxBuilder dev_aux_;
 };
 
 }  // namespace miden
