@@ -329,6 +329,79 @@ int mdn_check_constraints(mdn_session* s, const mdn_statement* st, const mdn_mat
                           uint32_t flags, uint64_t* randomness_out /* 2*max num_randomness, may be NULL */,
                           mdn_constraint_report* out);
 
+/* ---- find unbalanced LogUp bus messages, without proving: check_trace_balance ----------------------------------
+ * (air/src/lookup/debug/trace/mod.rs:169-309, builder.rs:201-375).  Walks every row of every AIR of the statement that
+ * carries a lowered mdn_air.lookup, keys every active push by its encoded denominator and sums the multiplicities
+ * jointly over those AIRs (Miden's buses close across AIRs; a one-AIR statement gives the reference's per-AIR report).
+ * AIRs without mdn_air.lookup are skipped and counted.  Per push, exactly as the reference's DebugTraceBuilder:
+ * interaction k of the lookup program pushes (multiplicity, denominator) at row r when its flag is non-zero (or it has
+ * none); the multiplicity is recorded as given, not multiplied by the flag; a zero denominator is an ordinary key (the
+ * aux build refuses it); the next row wraps; periodic values are row r mod 2^log_max_period of periodic_values.
+ *   randomness : 2 * max num_randomness u64 (alpha, beta, ...: EF pairs), canonical -- e.g. the randomness_out of
+ *                mdn_check_constraints or mdn_prove_begin.  Nothing is observed; no hash configuration is consulted.
+ *   boundary   : n_boundary triples {denominator c0, c1, multiplicity}, canonical: the output of LookupAir::eval_boundary
+ *                (DebugBoundaryEmitter, builder.rs:401-415).  Emission i is tagged instance 0xFFFFFFFF,
+ *                row UINT64_MAX, column 0xFFFFFFFF, interaction i.
+ *   mutex_sites: NULL, or per AIR (instance order) NULL or one word per interaction of its lookup program: 0xFFFFFFFF
+ *                when the interaction is not in a group_with_cached_encoding, else (g << 16) | site with g the group's
+ *                index within its column (the reference's group_idx) and site one insert / insert_encoded / batch call
+ *                of that group (every interaction of a batch carries the batch's site, so all of them share one flag
+ *                node).  A row violates group g of column c when more than one distinct site of it has a non-zero flag
+ *                (track_mutex, builder.rs:204-208).  At most 1024 annotated interactions per AIR.
+ *   max_contributions : the pushes of the unmatched denominators are listed when there are at most this many.
+ *   flags      : as mdn_check_constraints: host row-major traces, MDN_FLAG_DEVICE_TRACES, | MDN_FLAG_COLUMN_MAJOR (read
+ *                in place).
+ * Orders.  unmatched: ascending denominator (c0, then c1) -- the derived Ord of p3's BinomialExtensionField over
+ * Felt::cmp (crates/field/src/native/mod.rs:681); p3 is not vendored, so this order is not pinned by the reference's own
+ * sources.  contributions: grouped in unmatched order, in emission order (instance, row, interaction) inside a group,
+ * boundary emissions last.  mutex_violations: (instance, row, column, group).  The report does not depend on the order
+ * in which the device's atomics ran.
+ * Returns MDN_OK whenever the check ran, whatever it found.  Refused before any device work: a call between
+ * mdn_prove_begin and mdn_prove_finish (MDN_ERR_INVALID_ARG) and a session split over ranks (MDN_ERR_UNSUPPORTED).
+ * Malformed or non-canonical randomness, boundary triples or annotations: MDN_ERR_INVALID_ARG; a table larger than the
+ * free device memory: MDN_ERR_UNSUPPORTED.  The report's memory is owned by the session and valid until the next call
+ * on it.  Nothing mdn_get_info / mdn_get_timings report about the last proof changes, and later proofs are unchanged. */
+typedef struct {
+    uint64_t denom[2];               /* encoded denominator (c0, c1) */
+    uint64_t net_multiplicity;       /* sum of its multiplicities mod p, non-zero */
+    uint64_t n_pushes;               /* pushes that landed on it */
+    uint64_t first_row;              /* its least push (instance, row, interaction); UINT64_MAX for a boundary emission */
+    uint32_t first_instance;         /* instance order; 0xFFFFFFFF: boundary */
+    uint32_t first_interaction;      /* interaction index in the AIR's lookup program; boundary: index in `boundary` */
+} mdn_unmatched;
+typedef struct {
+    uint64_t row;                    /* UINT64_MAX: boundary */
+    uint64_t multiplicity;           /* as pushed */
+    uint32_t instance;               /* 0xFFFFFFFF: boundary */
+    uint32_t column;                 /* aux column of the interaction; 0xFFFFFFFF: boundary */
+    uint32_t interaction;
+    uint32_t reserved;
+} mdn_balance_push;
+typedef struct {
+    uint64_t row;
+    uint32_t instance, column, group, active_flags;   /* active_flags: distinct sites of the group with a non-zero flag */
+} mdn_mutex_violation;
+typedef struct {
+    uint32_t holds;                  /* 1: nothing unmatched and no mutex violation */
+    uint32_t contributions_complete; /* 1: contributions lists every push of every unmatched denominator */
+    uint64_t n_pushes;               /* active pushes, boundary emissions included */
+    uint64_t n_denominators;         /* distinct denominators pushed */
+    uint64_t n_unmatched;
+    uint64_t n_mutex_violations;
+    uint64_t n_contributions;        /* pushes of the unmatched denominators (= sum of their n_pushes) */
+    uint32_t n_skipped_airs;         /* AIRs without mdn_air.lookup */
+    uint32_t reserved;
+    const mdn_unmatched* unmatched;               /* n_unmatched */
+    const mdn_balance_push* contributions;        /* n_contributions when contributions_complete, else NULL */
+    const mdn_mutex_violation* mutex_violations;  /* the first min(n_mutex_violations, max_contributions) */
+    uint64_t n_mutex_listed;
+} mdn_balance_report;
+int mdn_check_trace_balance(mdn_session* s, const mdn_statement* st, const mdn_matrix* traces /* instance order */,
+                            const uint64_t* randomness /* 2 * max num_randomness: alpha, beta, ... */,
+                            const uint64_t* boundary, size_t n_boundary /* n x {denom c0, denom c1, multiplicity} */,
+                            const uint32_t* const* mutex_sites /* per AIR, NULL or one word per interaction; NULL = none */,
+                            uint64_t max_contributions, uint32_t flags, mdn_balance_report* out);
+
 /* wincode/bincode-default layout of StarkProofData (prover/src/lib.rs:347-354): u64-LE length +
  * height bytes; u64-LE length + u64-LE felts; u64-LE length + 32-byte commitments.  Returns the
  * number of bytes needed; writes only if cap is large enough.  (Layout unpinned in-tree.) */

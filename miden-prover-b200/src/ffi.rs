@@ -176,6 +176,63 @@ pub struct MdnConstraintReport {
     pub failing_rows: u64,
 }
 
+/// `mdn_unmatched` (include/miden_b200.h): a denominator whose multiplicities do not sum to zero, with its least push.
+#[repr(C)]
+#[derive(Clone, Copy, Debug, Default)]
+pub struct MdnUnmatched {
+    pub denom: [u64; 2],
+    pub net_multiplicity: u64,
+    pub n_pushes: u64,
+    /// u64::MAX for a boundary emission
+    pub first_row: u64,
+    /// 0xFFFFFFFF for a boundary emission
+    pub first_instance: u32,
+    /// interaction index in the AIR's lookup program; boundary: index in the boundary list
+    pub first_interaction: u32,
+}
+
+/// `mdn_balance_push`: one push of an unmatched denominator.
+#[repr(C)]
+#[derive(Clone, Copy, Debug, Default)]
+pub struct MdnBalancePush {
+    pub row: u64,
+    pub multiplicity: u64,
+    pub instance: u32,
+    pub column: u32,
+    pub interaction: u32,
+    pub reserved: u32,
+}
+
+/// `mdn_mutex_violation`: more than one site of a cached-encoding group active on one row.
+#[repr(C)]
+#[derive(Clone, Copy, Debug, Default)]
+pub struct MdnMutexViolation {
+    pub row: u64,
+    pub instance: u32,
+    pub column: u32,
+    pub group: u32,
+    pub active_flags: u32,
+}
+
+/// `mdn_balance_report`: the outcome of `mdn_check_trace_balance`; the arrays belong to the session.
+#[repr(C)]
+#[derive(Clone, Copy, Debug)]
+pub struct MdnBalanceReport {
+    pub holds: u32,
+    pub contributions_complete: u32,
+    pub n_pushes: u64,
+    pub n_denominators: u64,
+    pub n_unmatched: u64,
+    pub n_mutex_violations: u64,
+    pub n_contributions: u64,
+    pub n_skipped_airs: u32,
+    pub reserved: u32,
+    pub unmatched: *const MdnUnmatched,
+    pub contributions: *const MdnBalancePush,
+    pub mutex_violations: *const MdnMutexViolation,
+    pub n_mutex_listed: u64,
+}
+
 pub enum MdnSession {}
 
 /// `mdn_hash_kind` (include/miden_b200.h): which `miden_air::config` constructor the session follows.
@@ -241,6 +298,18 @@ unsafe extern "C" {
         flags: u32,
         randomness_out: *mut u64,
         out: *mut MdnConstraintReport,
+    ) -> c_int;
+    pub fn mdn_check_trace_balance(
+        s: *mut MdnSession,
+        st: *const MdnStatement,
+        traces: *const MdnMatrix,
+        randomness: *const u64,
+        boundary: *const u64,
+        n_boundary: usize,
+        mutex_sites: *const *const u32,
+        max_contributions: u64,
+        flags: u32,
+        out: *mut MdnBalanceReport,
     ) -> c_int;
     pub fn mdn_session_set_preprocessed(
         s: *mut MdnSession,

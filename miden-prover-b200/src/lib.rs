@@ -412,6 +412,171 @@ impl<'s> GpuStarkProver<'s> {
             _ => {}
         }
     }
+
+    /// `check_trace_balance(air, main, periodic, publics, var_len_publics, challenges)` (air/src/lookup/debug/trace/mod.rs:169-189)
+    /// on the device, jointly over every AIR with a device lookup (Miden's buses close across AIRs).  `boundary` is what the
+    /// statement's `eval_boundary` emitted into a [`RecordingBoundary`]; `mutex_sites[i]` is AIR i's annotation (one word per
+    /// interaction, include/miden_b200.h) and `site_names[i][k]` the `insert` name of its interaction k, which the report
+    /// uses in place of the reference's `msg_repr`.  Like the rest of this crate, not compiled in this repository.
+    pub fn check_trace_balance<MA>(
+        &mut self,
+        statement: &ProverStatement<Felt, QuadFelt, MA>,
+        challenges: &[QuadFelt],
+        boundary: &RecordingBoundary,
+        mutex_sites: &[Option<Vec<u32>>],
+        site_names: &[Vec<&'static str>],
+        max_contributions: u64,
+    ) -> GpuBalanceReport
+    where
+        MA: MultiAir<Felt, QuadFelt>,
+    {
+        let traces: &[RowMajorMatrix<Felt>] = statement.traces();
+        let st = statement.statement();
+        let lookup_structs: Vec<Option<MdnLookup>> = self
+            .lookups
+            .iter()
+            .map(|l| l.as_ref().map(|(n, prog)| MdnLookup { num_columns: *n, program_words: prog.len() as u32, program: prog.as_ptr() }))
+            .collect();
+        let airs: Vec<MdnAir> = self
+            .lowered
+            .iter()
+            .zip(&lookup_structs)
+            .map(|(a, lk)| MdnAir {
+                width: a.width,
+                aux_width: a.aux_width,
+                num_aux_values: a.num_aux_values,
+                num_randomness: a.num_randomness,
+                log_quotient_degree: a.log_quotient_degree,
+                program_words: a.program.len() as u32,
+                program: a.program.as_ptr(),
+                periodic_values: if a.periodic_values.is_empty() { ptr::null() } else { a.periodic_values.as_ptr() },
+                num_periodic_columns: a.num_periodic_columns,
+                log_max_period: a.log_max_period,
+                preprocessed_width: a.preprocessed_width,
+                lookup: lk.as_ref().map_or(ptr::null(), |l| l as *const MdnLookup),
+            })
+            .collect();
+        let public_values: Vec<u64> = st.air_inputs().iter().map(Felt::as_canonical_u64).collect();
+        let mats: Vec<MdnMatrix> = traces
+            .iter()
+            .map(|t| MdnMatrix { values: t.values.as_ptr() as *const u64, log_height: t.height().trailing_zeros(), width: t.width() as u32 })
+            .collect();
+        let mdn_st = MdnStatement {
+            airs: airs.as_ptr(),
+            n_airs: traces.len() as u32,
+            public_values: public_values.as_ptr(),
+            n_public_values: public_values.len() as u32,
+            observe_felts: ptr::null(),
+            n_observe_felts: 0,
+        };
+        let ef = |q: &QuadFelt| -> [u64; 2] {
+            let c = q.as_basis_coefficients_slice();
+            [c[0].as_canonical_u64(), c[1].as_canonical_u64()]
+        };
+        let rnd: Vec<u64> = challenges.iter().flat_map(|c| ef(c)).collect();
+        let bnd: Vec<u64> = boundary.emissions.iter().flat_map(|(_, d, m)| { let d = ef(d); [d[0], d[1], m.as_canonical_u64()] }).collect();
+        let sites: Vec<*const u32> = (0..traces.len())
+            .map(|i| mutex_sites.get(i).and_then(|m| m.as_ref()).map_or(ptr::null(), |m| m.as_ptr()))
+            .collect();
+        let mut rep = core::mem::MaybeUninit::<MdnBalanceReport>::zeroed();
+        let rc = unsafe {
+            mdn_check_trace_balance(self.session.raw, &mdn_st, mats.as_ptr(), rnd.as_ptr(), bnd.as_ptr(), boundary.emissions.len(),
+                                    sites.as_ptr(), max_contributions, 0, rep.as_mut_ptr())
+        };
+        assert_eq!(rc, MDN_OK, "check_trace_balance failed: {}", last_error(self.session.raw));
+        let rep = unsafe { rep.assume_init() };
+        // interaction index -> insert name; boundary emissions keep their eval_boundary name
+        let name = |inst: u32, k: u32| -> String {
+            if inst == u32::MAX {
+                return format!("[boundary:{}]", boundary.emissions.get(k as usize).map_or("?", |e| e.0));
+            }
+            site_names.get(inst as usize).and_then(|n| n.get(k as usize)).map_or(format!("interaction {k}"), |s| s.to_string())
+        };
+        let unmatched = unsafe { core::slice::from_raw_parts(rep.unmatched, rep.n_unmatched as usize) };
+        let pushes: &[MdnBalancePush] =
+            if rep.contributions_complete != 0 { unsafe { core::slice::from_raw_parts(rep.contributions, rep.n_contributions as usize) } } else { &[] };
+        let mut out = GpuBalanceReport::default();
+        let mut c = 0usize;
+        for u in unmatched {
+            let n = if rep.contributions_complete != 0 { u.n_pushes as usize } else { 0 };
+            let contributions = pushes[c..c + n]
+                .iter()
+                .map(|p| GpuPush { instance: p.instance, row: p.row, column: p.column, interaction: p.interaction, multiplicity: p.multiplicity, site: name(p.instance, p.interaction) })
+                .collect();
+            c += n;
+            out.unmatched.push(GpuUnmatched {
+                denom: u.denom,
+                net_multiplicity: u.net_multiplicity,
+                n_pushes: u.n_pushes,
+                first: GpuPush { instance: u.first_instance, row: u.first_row, column: u32::MAX, interaction: u.first_interaction, multiplicity: 0, site: name(u.first_instance, u.first_interaction) },
+                contributions,
+            });
+        }
+        out.mutex_violations = unsafe { core::slice::from_raw_parts(rep.mutex_violations, rep.n_mutex_listed as usize) }.to_vec();
+        out.n_mutex_violations = rep.n_mutex_violations;
+        out
+    }
+}
+
+/// A `BoundaryBuilder` that records `eval_boundary`'s emissions (name, encoded denominator, multiplicity) for
+/// [`GpuStarkProver::check_trace_balance`], as the reference's `DebugBoundaryEmitter` (builder.rs:382-415) feeds its walk.
+pub struct RecordingBoundary<'a> {
+    pub challenges: &'a miden_air::lookup::Challenges<QuadFelt>,
+    pub public_values: &'a [Felt],
+    pub var_len_public_inputs: &'a [&'a [Felt]],
+    pub emissions: Vec<(&'static str, QuadFelt, Felt)>,
+}
+
+impl<'a> miden_air::lookup::BoundaryBuilder for RecordingBoundary<'a> {
+    type F = Felt;
+    type EF = QuadFelt;
+    fn public_values(&self) -> &[Felt] {
+        self.public_values
+    }
+    fn var_len_public_inputs(&self) -> &[&[Felt]] {
+        self.var_len_public_inputs
+    }
+    fn insert<M>(&mut self, name: &'static str, multiplicity: Felt, msg: M)
+    where
+        M: miden_air::lookup::LookupMessage<Felt, QuadFelt>,
+    {
+        self.emissions.push((name, msg.encode(self.challenges), multiplicity));
+    }
+}
+
+/// One push of an unmatched denominator; `site` names its insert (or `[boundary:<name>]`).
+#[derive(Clone, Debug)]
+pub struct GpuPush {
+    pub instance: u32,
+    pub row: u64,
+    pub column: u32,
+    pub interaction: u32,
+    pub multiplicity: u64,
+    pub site: String,
+}
+
+#[derive(Clone, Debug)]
+pub struct GpuUnmatched {
+    pub denom: [u64; 2],
+    pub net_multiplicity: u64,
+    pub n_pushes: u64,
+    pub first: GpuPush,
+    /// every push in emission order, empty when there were more than `max_contributions` in all
+    pub contributions: Vec<GpuPush>,
+}
+
+/// `BalanceReport` (air/src/lookup/debug/trace/mod.rs:84-95) as the device reports it.
+#[derive(Clone, Debug, Default)]
+pub struct GpuBalanceReport {
+    pub unmatched: Vec<GpuUnmatched>,
+    pub mutex_violations: Vec<MdnMutexViolation>,
+    pub n_mutex_violations: u64,
+}
+
+impl GpuBalanceReport {
+    pub fn is_ok(&self) -> bool {
+        self.unmatched.is_empty() && self.n_mutex_violations == 0
+    }
 }
 
 /// `StarkProofData`'s three streams as the C ABI returns them; a commitment is four u64 whatever the hash configuration.

@@ -95,6 +95,55 @@ class LookupProgramBuilder(ProgramBuilder):
         super().__init__()
         self.num_columns = num_columns
         self.interactions: list[tuple[int, int, int, int]] = []
+        # mutual-exclusion annotation of every interaction (mdn_check_trace_balance): NO_FLAG, or group << 16 | site
+        self.sites: list[int] = []
+        self._groups = [0] * num_columns       # next group index per column (the reference's group_idx)
+        self._group = None                     # (column, group index, cached, next site) of the open group
+        self._batch_site = None
+
+    class _Scope:
+        def __init__(self, enter, leave):
+            self._enter, self._leave = enter, leave
+
+        def __enter__(self):
+            return self._enter()
+
+        def __exit__(self, *exc):
+            self._leave()
+
+    def group(self, column: int, cached: bool = False):
+        """`with b.group(c, cached)`: the inserts inside belong to the next group of column c (`LookupColumn::group`, or
+        `group_with_cached_encoding` when cached: then every insert / batch inside is one mutual-exclusion site)."""
+        def enter():
+            assert self._group is None, "groups do not nest"
+            self._group = [column, self._groups[column], cached, 0]
+            self._groups[column] += 1
+            return self._group[1]
+
+        def leave():
+            self._group = None
+        return self._Scope(enter, leave)
+
+    def batch(self):
+        """`with b.batch()`: the inserts inside are one `LookupGroup::batch` call (they share its flag): one site."""
+        def enter():
+            assert self._group is not None and self._batch_site is None
+            self._batch_site = self._new_site()
+
+        def leave():
+            self._batch_site = None
+        return self._Scope(enter, leave)
+
+    def _new_site(self):
+        g = self._group
+        site = g[3]
+        g[3] += 1
+        return site
+
+    def mutex_sites(self) -> np.ndarray:
+        """One word per interaction for mdn_check_trace_balance: 0xFFFFFFFF outside a cached-encoding group, else
+        (group index within its column) << 16 | site."""
+        return np.array(self.sites, dtype=np.uint32)
 
     def bus_prefix(self, bus: int, max_message_width: int) -> Expr:
         """`Challenges::new`: bus_prefix[i] = alpha + (i + 1) * beta^W (air/src/lookup/challenges.rs)."""
@@ -115,6 +164,13 @@ class LookupProgramBuilder(ProgramBuilder):
 
     def insert(self, column: int, flag, multiplicity: Expr, denominator: Expr):
         self.interactions.append((column, NO_FLAG if flag is None else flag.id, multiplicity.id, denominator.id))
+        g = self._group
+        if g is None or not g[2]:
+            self.sites.append(NO_FLAG)
+            return
+        assert g[0] == column, "an insert belongs to its group's column"
+        site = self._batch_site if self._batch_site is not None else self._new_site()
+        self.sites.append((g[1] << 16) | site)
 
     def assert_zero(self, e):  # pragma: no cover - a lookup description emits no constraints
         raise TypeError("LookupBuilder has no assert_* surface")

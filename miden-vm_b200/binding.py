@@ -73,6 +73,49 @@ class ConstraintReport(C.Structure):
                 ("row", C.c_uint64), ("value", C.c_uint64 * 2), ("failing_rows", C.c_uint64)]
 
 
+class Unmatched(C.Structure):
+    """`mdn_unmatched`: a denominator whose multiplicities do not sum to zero, with its least push."""
+    _fields_ = [("denom", C.c_uint64 * 2), ("net_multiplicity", C.c_uint64), ("n_pushes", C.c_uint64), ("first_row", C.c_uint64),
+                ("first_instance", C.c_uint32), ("first_interaction", C.c_uint32)]
+
+
+class BalancePush(C.Structure):
+    """`mdn_balance_push`: one push of an unmatched denominator (instance / column 0xFFFFFFFF: a boundary emission)."""
+    _fields_ = [("row", C.c_uint64), ("multiplicity", C.c_uint64), ("instance", C.c_uint32), ("column", C.c_uint32),
+                ("interaction", C.c_uint32), ("reserved", C.c_uint32)]
+
+
+class MutexViolation(C.Structure):
+    _fields_ = [("row", C.c_uint64), ("instance", C.c_uint32), ("column", C.c_uint32), ("group", C.c_uint32), ("active_flags", C.c_uint32)]
+
+
+class BalanceReport(C.Structure):
+    """`mdn_balance_report`: the outcome of mdn_check_trace_balance.  Its arrays are owned by the session."""
+    _fields_ = [("holds", C.c_uint32), ("contributions_complete", C.c_uint32), ("n_pushes", C.c_uint64),
+                ("n_denominators", C.c_uint64), ("n_unmatched", C.c_uint64), ("n_mutex_violations", C.c_uint64),
+                ("n_contributions", C.c_uint64), ("n_skipped_airs", C.c_uint32), ("reserved", C.c_uint32),
+                ("unmatched", C.POINTER(Unmatched)), ("contributions", C.POINTER(BalancePush)),
+                ("mutex_violations", C.POINTER(MutexViolation)), ("n_mutex_listed", C.c_uint64)]
+
+
+BOUNDARY = 0xFFFFFFFF     # instance / column of a boundary emission in a balance report (row = 2^64 - 1)
+
+
+def balance_report_dict(rep: BalanceReport) -> dict:
+    """A BalanceReport as plain Python values (copied out of the session's memory): every field, lists of tuples
+    unmatched (denom, net, n_pushes, (first instance, first row, first interaction)), contributions (instance, row,
+    column, interaction, multiplicity) and mutex_violations (instance, row, column, group, active_flags)."""
+    um = [((u.denom[0], u.denom[1]), u.net_multiplicity, u.n_pushes, (u.first_instance, u.first_row, u.first_interaction))
+          for u in (rep.unmatched[i] for i in range(rep.n_unmatched))]
+    co = [(c.instance, c.row, c.column, c.interaction, c.multiplicity)
+          for c in (rep.contributions[i] for i in range(rep.n_contributions if rep.contributions_complete else 0))]
+    mv = [(m.instance, m.row, m.column, m.group, m.active_flags) for m in (rep.mutex_violations[i] for i in range(rep.n_mutex_listed))]
+    return dict(holds=rep.holds, contributions_complete=rep.contributions_complete, n_pushes=rep.n_pushes,
+                n_denominators=rep.n_denominators, n_unmatched=rep.n_unmatched, n_mutex_violations=rep.n_mutex_violations,
+                n_contributions=rep.n_contributions, n_skipped_airs=rep.n_skipped_airs, unmatched=um, contributions=co,
+                mutex_violations=mv)
+
+
 AUX_BUILDER = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_uint32, C.POINTER(Matrix), u64p, u64p, u64p)
 ALLGATHER = C.CFUNCTYPE(C.c_int, C.c_void_p, u64p, u64p, C.c_size_t)
 EXTERNAL_CHECK = C.CFUNCTYPE(C.c_int, C.c_void_p, u64p, C.c_uint32, C.POINTER(u64p), u32p, C.POINTER(C.c_uint8), C.c_uint32, u32p)
@@ -88,7 +131,7 @@ EXPORTS = [
     "mdn_challenger_observe", "mdn_challenger_sample", "mdn_set_debug", "mdn_session_set_shard",
     "mdn_session_set_preprocessed", "mdn_session_set_jit", "mdn_jit_compile_check", "mdn_jit_status", "mdn_abi_layout",
     "mdn_session_set_external_check", "mdn_session_set_hash", "mdn_session_set_hash_challenger",
-    "mdn_check_constraints", "mdn_session_set_device_aux_builder",
+    "mdn_check_constraints", "mdn_session_set_device_aux_builder", "mdn_check_trace_balance",
 ]
 
 _lib = None
@@ -129,6 +172,8 @@ def lib():
         L.mdn_check_constraints.argtypes = [C.c_void_p, C.POINTER(Statement), C.POINTER(Matrix), C.POINTER(Matrix),
                                             C.POINTER(Challenger), AUX_BUILDER, C.c_void_p, C.c_uint32, u64p,
                                             C.POINTER(ConstraintReport)]
+        L.mdn_check_trace_balance.argtypes = [C.c_void_p, C.POINTER(Statement), C.POINTER(Matrix), u64p, u64p, C.c_size_t,
+                                              C.POINTER(u32p), C.c_uint64, C.c_uint32, C.POINTER(BalanceReport)]
         L.mdn_prove_begin.argtypes = [C.c_void_p, C.POINTER(Statement), C.POINTER(Matrix), C.POINTER(Challenger),
                                       C.c_uint32, u64p, u64p]
         L.mdn_prove_commit_aux.argtypes = [C.c_void_p, C.POINTER(Matrix), C.POINTER(u64p), u64p]
@@ -294,6 +339,27 @@ class Session:
                                                 C.byref(challenger) if challenger is not None else None, cb, None, flags,
                                                 ptr(rnd), C.byref(rep)))
         return rep, rnd[: 2 * n_rand]
+
+    def check_trace_balance(self, statement: Statement, traces, randomness, boundary=(), mutex_sites=None,
+                            max_contributions: int = 1 << 16, flags=0) -> dict:
+        """`check_trace_balance` (air/src/lookup/debug/trace/mod.rs:169) on the device, jointly over every AIR of the
+        statement with a lowered lookup program.  randomness: 2 * max num_randomness words (e.g. the randomness of
+        check_constraints); boundary: (c0, c1, multiplicity) triples of eval_boundary; mutex_sites: per AIR None or the
+        annotation array of LookupProgramBuilder.mutex_sites().  Returns balance_report_dict of the report."""
+        rnd = np.ascontiguousarray(np.asarray(randomness, dtype=np.uint64).reshape(-1))
+        bnd = np.ascontiguousarray(np.asarray([[int(x) for x in t] for t in boundary], dtype=np.uint64).reshape(-1))
+        keep, sites = [], None
+        if mutex_sites is not None:
+            sites = (u32p * statement.n_airs)()
+            for i, m in enumerate(mutex_sites):
+                if m is not None:
+                    keep.append(np.ascontiguousarray(m, dtype=np.uint32))
+                    sites[i] = keep[-1].ctypes.data_as(u32p)
+        rep = BalanceReport()
+        self._check(lib().mdn_check_trace_balance(self._h, C.byref(statement), traces, ptr(rnd) if rnd.size else None,
+                                                  ptr(bnd) if bnd.size else None, len(bnd) // 3, sites, max_contributions,
+                                                  flags, C.byref(rep)))
+        return balance_report_dict(rep)
 
     def info(self, what: int, cap: int = 0) -> np.ndarray:
         n = lib().mdn_get_info(self._h, what, None, 0)

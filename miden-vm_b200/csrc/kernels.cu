@@ -940,6 +940,160 @@ int launch_check_rows(const CheckArgs& a, cudaStream_t st) {
     return 0;
 }
 
+// =============================================================================================
+// LogUp bus balance (debug/trace check_trace_balance): the lookup program of k_logup_rows, every active push keyed
+// by its denominator in a device hash table (kernels.cuh BalanceTable)
+// =============================================================================================
+__device__ __forceinline__ u64 balance_hash(u64 c0, u64 c1) {
+    u64 h = c0 * 0x9E3779B97F4A7C15ull ^ (c1 + 0x632BE59BD9B4E019ull) * 0xC2B2AE3D27D4EB4Full;
+    return h ^ (h >> 29) ^ (h >> 47);
+}
+#ifdef MDN_EMULATED
+// tests/emu runs every fiber on one OS thread, so a plain compare-and-swap is atomic there
+static inline ulonglong2 cas128(ulonglong2* p, ulonglong2 cmp, ulonglong2 v) { ulonglong2 o = *p; if (o.x == cmp.x && o.y == cmp.y) *p = v; return o; }
+#else
+__device__ __forceinline__ ulonglong2 cas128(ulonglong2* p, ulonglong2 cmp, ulonglong2 v) { return atomicCAS(p, cmp, v); }   // sm_90: 128-bit CAS
+#endif
+// the slot of key (c0, c1), claimed with a 128-bit compare-and-swap when the key is new.  A plain load first: a key,
+// once written, never changes, and a stale or half-written view (one word still all ones) falls through to the CAS.
+__device__ __forceinline__ u64 balance_insert(const BalanceTable& t, u64 c0, u64 c1) {
+    ulonglong2* keys = reinterpret_cast<ulonglong2*>(t.keys);
+    for (u64 s = balance_hash(c0, c1) & t.mask;; s = (s + 1) & t.mask) {
+        ulonglong2 cur = keys[s];
+        if (cur.x == c0 && cur.y == c1) return s;
+        if (cur.x != ~0ull && cur.y != ~0ull) continue;
+        ulonglong2 old = cas128(&keys[s], make_ulonglong2(~0ull, ~0ull), make_ulonglong2(c0, c1));
+        if ((old.x == ~0ull && old.y == ~0ull) || (old.x == c0 && old.y == c1)) return s;
+    }
+}
+// the slot of a key already inserted (a later kernel: no concurrent writers)
+__device__ __forceinline__ u64 balance_find(const BalanceTable& t, u64 c0, u64 c1) {
+    const ulonglong2* keys = reinterpret_cast<const ulonglong2*>(t.keys);
+    u64 s = balance_hash(c0, c1) & t.mask;
+    for (;; s = (s + 1) & t.mask) { ulonglong2 cur = keys[s]; if (cur.x == c0 && cur.y == c1) return s; }
+}
+// exact and order-independent: the 128-bit integer sum of the canonical multiplicities (a carry into the high word
+// whenever the low word wraps), the push count and the least push key
+__device__ __forceinline__ void balance_add(const BalanceTable& t, u64 s, u64 m, u64 key) {
+    unsigned long long* sum = reinterpret_cast<unsigned long long*>(t.sums) + 2 * s;
+    unsigned long long old = atomicAdd(sum, (unsigned long long)m);
+    if (old + m < old) atomicAdd(sum + 1, 1ull);
+    atomicAdd(t.count + s, 1ull);
+    atomicMin(t.first + s, (unsigned long long)key);
+}
+
+template <int MAXS>
+__global__ void __launch_bounds__(128) k_balance_rows(BalanceArgs a) {
+    size_t N = (size_t)1 << a.log_n;
+    size_t r = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= N) return;
+    size_t rn = (r + 1) & (N - 1);
+    size_t per_row = (r & (((size_t)1 << a.prog.log_max_period) - 1)) * a.prog.n_periodic;
+    E2 slot[MAXS];
+    u64 act[BALANCE_MUTEX_MAX / 64];       // activity of the annotated interactions (bit mutex_pos[k])
+    for (u32 w = 0; w < (a.n_mutex + 63) / 64; w++) act[w] = 0;
+    unsigned long long pushes = 0;
+    const uint4* code = reinterpret_cast<const uint4*>(a.prog.code);
+    for (u32 i = 0; i < a.prog.n_instr; i++) {
+        uint4 ins = code[i];
+        u32 op = ins.x & 0xff, ext = ins.x >> 8, x = ins.z, y = ins.w;
+        E2 v;
+        switch (op) {
+            case 0: v = gl::e2(a.main_cm[(size_t)y * N + (x ? rn : r)], 0); break;
+            case 2: v = gl::e2(a.publics[x], 0); break;
+            case 3: v = gl::e2(a.challenges[2 * x], a.challenges[2 * x + 1]); break;
+            case 8: v = gl::e2(a.prog.consts[x], 0); break;
+            case 9: v = gl::e2(a.prog.consts[x], a.prog.consts[x + 1]); break;
+            case 10: v = ext ? gl::e2_add(slot[x], slot[y]) : gl::e2(gl::add(slot[x].a, slot[y].a), 0); break;
+            case 11: v = ext ? gl::e2_sub(slot[x], slot[y]) : gl::e2(gl::sub(slot[x].a, slot[y].a), 0); break;
+            case 12: v = ext ? gl::e2_mul(slot[x], slot[y]) : gl::e2(gl::mul(slot[x].a, slot[y].a), 0); break;
+            case 13: v = ext ? gl::e2_neg(slot[x]) : gl::e2(gl::neg(slot[x].a), 0); break;
+            case 14: v = gl::e2(a.prog.periodic[per_row + x], 0); break;
+            default: {   // 17 EMIT of interaction k = ext
+                u32 fs = x & 0xffffu, ms = x >> 16, k = ext;
+                if (fs != 0xffffu && slot[fs].a == 0) continue;           // builder.rs:245: a zero flag skips the push
+                if (a.n_mutex) { u32 b = a.mutex_pos[k]; if (b != 0xFFFFFFFFu) act[b >> 6] |= 1ull << (b & 63); }
+                if (a.mode == 0) { pushes++; continue; }
+                E2 d = slot[y];                                            // a zero denominator is an ordinary key
+                u64 m = slot[ms].a, key = balance_key(a.instance, r, k);
+                if (a.mode == 1) { balance_add(a.t, balance_insert(a.t, d.a, d.b), m, key); continue; }
+                u64 s = balance_find(a.t, d.a, d.b);
+                if (a.t.sums[2 * s + 1]) {
+                    unsigned long long p = atomicAdd(a.counters + 2, 1ull);
+                    a.contrib_out[3 * p] = s; a.contrib_out[3 * p + 1] = key; a.contrib_out[3 * p + 2] = m;
+                }
+                continue;
+            }
+        }
+        slot[ins.y] = v;
+    }
+    if (pushes) atomicAdd(a.counters, pushes);
+    if (!a.n_mutex || a.mode == 2) return;
+    // groups in (column, group) order, sites consecutive inside a group: count the distinct sites with an active interaction
+    u32 cur_g = a.mutex_group[0], cur_s = a.mutex_site[0], cnt = 0;
+    bool counted = false;
+    for (u32 b = 0;; b++) {
+        const bool end = b == a.n_mutex;
+        u32 g = end ? 0xFFFFFFFFu : a.mutex_group[b], s = end ? 0xFFFFFFFFu : a.mutex_site[b];
+        if (end || g != cur_g) {
+            if (cnt > 1) {
+                unsigned long long p = atomicAdd(a.counters + 1, 1ull);
+                if (a.mode == 1) {
+                    a.mutex_out[3 * p] = ((u64)a.instance << 32) | r;
+                    a.mutex_out[3 * p + 1] = ((u64)(cur_g >> 16) << 32) | (cur_g & 0xffffu);
+                    a.mutex_out[3 * p + 2] = cnt;
+                }
+            }
+            if (end) break;
+            cur_g = g; cur_s = s; cnt = 0; counted = false;
+        } else if (s != cur_s) { cur_s = s; counted = false; }
+        if (!counted && ((act[b >> 6] >> (b & 63)) & 1)) { cnt++; counted = true; }
+    }
+}
+int launch_balance_rows(const BalanceArgs& a, cudaStream_t st) {
+    size_t N = (size_t)1 << a.log_n;
+    unsigned blocks = (unsigned)((N + 127) / 128);
+    if (a.n_mutex > BALANCE_MUTEX_MAX) return -1;
+    if (a.prog.n_slots <= 16) k_balance_rows<16><<<blocks, 128, 0, st>>>(a);
+    else if (a.prog.n_slots <= 64) k_balance_rows<64><<<blocks, 128, 0, st>>>(a);
+    else if (a.prog.n_slots <= 256) k_balance_rows<256><<<blocks, 128, 0, st>>>(a);
+    else if (a.prog.n_slots <= 1024) k_balance_rows<1024><<<blocks, 128, 0, st>>>(a);
+    else return -1;
+    COUNT_LAUNCH();
+    return 0;
+}
+__global__ void __launch_bounds__(128) k_balance_boundary(BalanceTable t, const u64* __restrict__ tr, u32 n) {
+    u32 i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    balance_add(t, balance_insert(t, tr[3 * i], tr[3 * i + 1]), tr[3 * i + 2], balance_key(BALANCE_BOUNDARY, 0, i));
+}
+void launch_balance_boundary(const BalanceTable& t, const u64* triples, u32 n, cudaStream_t st) {
+    if (!n) return;
+    k_balance_boundary<<<(n + 127) / 128, 128, 0, st>>>(t, triples, n);
+    COUNT_LAUNCH();
+}
+__global__ void __launch_bounds__(256) k_balance_finish(BalanceTable t, unsigned long long* counters, u64* out) {
+    size_t s = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (s > t.mask) return;
+    u64 c0 = t.keys[2 * s], c1 = t.keys[2 * s + 1];
+    if (c0 == ~0ull && c1 == ~0ull) return;
+    atomicAdd(counters + 3, 1ull);
+    // hi * 2^64 + lo mod p, with 2^64 = 2^32 - 1 (mod p)
+    u64 lo = t.sums[2 * s], hi = t.sums[2 * s + 1];
+    u64 net = gl::add(gl::mul(hi >= gl::P ? hi - gl::P : hi, 0xFFFFFFFFull), lo >= gl::P ? lo - gl::P : lo);
+    t.sums[2 * s] = net;
+    t.sums[2 * s + 1] = net != 0;
+    if (!net) return;
+    unsigned long long p = atomicAdd(counters + 4, 1ull);
+    u64* o = out + 6 * p;
+    o[0] = c0; o[1] = c1; o[2] = net; o[3] = t.count[s]; o[4] = t.first[s]; o[5] = s;
+}
+void launch_balance_finish(const BalanceTable& t, unsigned long long* counters, u64* out, cudaStream_t st) {
+    size_t slots = (size_t)t.mask + 1;
+    k_balance_finish<<<(unsigned)((slots + 255) / 256), 256, 0, st>>>(t, counters, out);
+    COUNT_LAUNCH();
+}
+
 // three-phase scan, 2048 rows per block (8 per thread): block totals -> serial scan of the (<= 2048) block
 // totals by one block -> per-block exclusive prefix with the block offset
 static constexpr int SCAN_T = 256, SCAN_E = 8, SCAN_B = SCAN_T * SCAN_E;

@@ -203,6 +203,52 @@ struct CheckArgs {
 int launch_check_rows(const CheckArgs& a, cudaStream_t st);   // 0, or -1 when the program needs too many slots
 
 // ---------------------------------------------------------------------------------------------
+// LogUp bus balance without proving (mdn_check_trace_balance; reference air/src/lookup/debug/trace/mod.rs:169-309)
+// ---------------------------------------------------------------------------------------------
+// Open-addressing hash table keyed by the 128-bit encoded denominator (c0, c1), `mask + 1` slots (a power of two, at
+// most half full).  An empty slot's key is all ones (never a canonical pair).  Per slot: the unreduced multiplicity
+// sum as a 128-bit integer (sum[2s] low word, sum[2s + 1] high word), the push count and the least packed push key
+// (balance_key below).  k_balance_finish overwrites sum[2s] with the net multiplicity mod p and sum[2s + 1] with
+// 1 when that net is non-zero (the slot is unmatched), else 0.
+struct BalanceTable {
+    u64* keys;                           // [slots][2], 16-byte aligned
+    u64* sums;                           // [slots][2]
+    unsigned long long* count;           // [slots], init 0
+    unsigned long long* first;           // [slots], init ~0
+    u64 mask;
+};
+// packed (instance, row, interaction) of a push, ordered as the tuple: instance < 2^9 (BALANCE_BOUNDARY for a boundary
+// emission, after every instance), row < 2^24, interaction < 2^24
+static constexpr u32 BALANCE_BOUNDARY = 0x100;
+__host__ __device__ inline u64 balance_key(u32 inst, u64 row, u32 k) { return ((u64)inst << 48) | (row << 24) | k; }
+// One thread per trace row interprets the compiled lookup program (k_logup_rows' instruction set; the EMIT word's bits
+// 8..31 carry the interaction index).  An EMIT whose flag is zero is skipped; otherwise, by mode:
+//   0  count: counters[0] += 1 per push, counters[1] += 1 per mutex violation (no table access)
+//   1  insert: add the multiplicity to the denominator's slot; record each mutex violation into mutex_out
+//   2  collect: every push whose denominator's slot is unmatched -> contrib_out {slot, balance_key, multiplicity}
+// Mutex check (builder.rs:204-208): mutex_pos[k] = bit of interaction k in the row's activity set (~0: not in a
+// cached-encoding group); bits are ordered by (column, group, site); mutex_group[b] = column << 16 | group and
+// mutex_site[b] = site of bit b.  A row violates a group where more than one distinct site has an active interaction.
+static constexpr u32 BALANCE_MUTEX_MAX = 1024;   // annotated interactions per AIR
+struct BalanceArgs {
+    const u64* main_cm; u32 log_n;       // raw main trace, column-major [col][row]
+    AirDev prog;                          // lookup program; periodic = RAW periodic matrix, row-major
+    const u64* publics; const u64* challenges;
+    u32 instance, mode;
+    const u32* mutex_pos; const u32* mutex_group; const u32* mutex_site; u32 n_mutex;   // n_mutex == 0: no annotation
+    BalanceTable t;
+    unsigned long long* counters;        // [0] pushes, [1] mutex violations, [2] contributions
+    u64* mutex_out;                       // 3 u64 per violation: instance << 32 | row, column << 32 | group, active sites
+    u64* contrib_out;                     // 3 u64 per push
+};
+int launch_balance_rows(const BalanceArgs& a, cudaStream_t st);   // 0, or -1 when the program needs too many slots
+// boundary emissions: n triples {c0, c1, multiplicity}; emission i is keyed balance_key(BALANCE_BOUNDARY, 0, i)
+void launch_balance_boundary(const BalanceTable& t, const u64* triples, u32 n, cudaStream_t st);
+// every occupied slot: counters[3] += 1; the net reduced mod p; an unmatched slot s appends
+// {c0, c1, net, count, first, s} to out (6 u64 each) at counters[4]
+void launch_balance_finish(const BalanceTable& t, unsigned long long* counters, u64* out, cudaStream_t st);
+
+// ---------------------------------------------------------------------------------------------
 // DEEP / FRI / misc
 // ---------------------------------------------------------------------------------------------
 // wvec[i] = y^(bitrev_n(p0 + i)) for i < cnt  (EF interleaved; p0 = 0, cnt = 2^n: the whole vector);

@@ -332,6 +332,12 @@ struct mdn_session {
     int eval_external(u32* failed);
     void check_constraints(const mdn_statement* st, const mdn_matrix* traces, const mdn_matrix* prep, const mdn_challenger* ch,
                            mdn_aux_builder build_aux, void* aux_ctx, u32 flags, mdn_constraint_report* out);
+    void check_trace_balance(const mdn_statement* st, const mdn_matrix* traces, const u64* rnd, const u64* boundary, size_t n_boundary,
+                             const uint32_t* const* mutex_sites, u64 max_contrib, u32 flags, mdn_balance_report* out);
+    // the last balance report's lists (mdn_balance_report points into them)
+    std::vector<mdn_unmatched> bal_unmatched;
+    std::vector<mdn_balance_push> bal_contrib;
+    std::vector<mdn_mutex_violation> bal_mutex;
     void commit_aux(const mdn_matrix* aux, const u64* const* aux_values, bool zero_aux, const mdn_matrix* builder_main = nullptr);
     void call_device_aux_builder(u32 inst, const mdn_matrix& main, u64* aux_slot, std::vector<u64>& values);
     void finish();
@@ -848,7 +854,8 @@ static Compiled compile_oplist(u32 i, const mdn_air& a, u32 n_publics, const u32
         if (evs[e].kind) {
             const u32* it = items + 4 * (size_t)evs[e].node;
             u32 fs = it[1] == 0xFFFFFFFFu ? 0xffffu : slot_of[it[1]];
-            code.insert(code.end(), {17u, it[0], fs | (slot_of[it[2]] << 16), slot_of[it[3]]});
+            // bits 8..31: the interaction index (read by the balance check only; it keeps nc below 2^24)
+            code.insert(code.end(), {17u | ((evs[e].node & 0xFFFFFFu) << 8), it[0], fs | (slot_of[it[2]] << 16), slot_of[it[3]]});
             // a node may serve several operands of one interaction: release each distinct node once
             u32 ops3[3] = {it[1], it[2], it[3]};
             for (int q = 0; q < 3; q++) {
@@ -1505,6 +1512,249 @@ void mdn_session::check_constraints(const mdn_statement* st, const mdn_matrix* t
         break;
     }
     out->holds = ext_rc == 0 && out->failing_rows == 0;
+}
+
+// ---------------------------------------------------------------------------------------------
+// check_trace_balance: every active LogUp push keyed by its denominator, without a proof  (debug/trace/mod.rs:169-309)
+// ---------------------------------------------------------------------------------------------
+// The validation, program compilation and main-trace upload of check_constraints; the challenges are an argument.  Per
+// AIR with a lowered lookup program, k_balance_rows counts the pushes (which sizes the table), then inserts them; the
+// boundary triples follow; k_balance_finish reduces every sum and compacts the unmatched denominators; when the report
+// can hold them, a third row pass collects their pushes.  The host sorts what is reported.
+void mdn_session::check_trace_balance(const mdn_statement* st, const mdn_matrix* traces, const u64* rnd, const u64* boundary, size_t n_boundary,
+                                      const uint32_t* const* mutex_sites, u64 max_contrib, u32 flags, mdn_balance_report* out) {
+    const bool cm = column_major(flags);
+    reset_proof();
+    prof.st = stream; prof.reset();
+    if (!d_flag.p) { ArenaScope persistent(nullptr); d_flag.alloc(1, stream); CUDA_OK(cudaMemsetAsync(d_flag.p, 0, 8, stream)); }
+    if (!out) fail(MDN_ERR_INVALID_ARG, "null argument");
+    const mdn_challenger no_challenger{};   // nothing is observed: validate_statement only checks the statement
+    validate_statement(st, traces, &no_challenger);
+    if (cm) for (u32 i = 0; i < st->n_airs; i++) check_column_major(traces[i], "trace", i);
+    const bool on_device = (flags & MDN_FLAG_DEVICE_TRACES) != 0;
+    const u32 k = st->n_airs;
+    bind_airs(st, traces, false);
+    bind_order(st, false);
+
+    // arguments: challenges, boundary emissions, interaction counts, mutex annotations
+    u32 max_rand = 0;
+    for (auto& a : airs) max_rand = std::max(max_rand, a.desc.num_randomness);
+    if (max_rand && !rnd) fail(MDN_ERR_INVALID_ARG, "randomness is NULL");
+    for (u32 i = 0; i < 2 * max_rand; i++) if (rnd[i] >= gl::P) fail(MDN_ERR_INVALID_ARG, "randomness word %u is not a canonical field element (>= p)", i);
+    if (n_boundary && !boundary) fail(MDN_ERR_INVALID_ARG, "boundary is NULL");
+    if (n_boundary >= (1u << 24)) fail(MDN_ERR_UNSUPPORTED, "at most 2^24 - 1 boundary emissions");
+    for (size_t q = 0; q < 3 * n_boundary; q++)
+        if (boundary[q] >= gl::P) fail(MDN_ERR_INVALID_ARG, "boundary emission %zu: %s is not a canonical field element (>= p)", q / 3, q % 3 == 2 ? "the multiplicity" : "the denominator");
+    struct Mutex { std::vector<u32> pos, group, site; };
+    std::vector<Mutex> mx(k);
+    u32 skipped = 0;
+    for (u32 i = 0; i < k; i++) {
+        const uint32_t* ann = mutex_sites ? mutex_sites[i] : nullptr;
+        if (!airs[i].has_lookup) {
+            skipped++;
+            if (ann) fail(MDN_ERR_INVALID_ARG, "AIR %u: mutex sites given for an AIR without a lookup program", i);
+            continue;
+        }
+        const u32* w = st->airs[i].lookup->program;
+        const u32 nn = w[2], nc = w[3];
+        if (nc >= (1u << 24)) fail(MDN_ERR_UNSUPPORTED, "AIR %u: at most 2^24 - 1 lookup interactions", i);
+        if (!ann) continue;
+        const u32* items = w + 5 + 3 * (size_t)nn;   // {column, flag, multiplicity, denominator}
+        std::vector<u32> ids;
+        for (u32 q = 0; q < nc; q++) if (ann[q] != 0xFFFFFFFFu) ids.push_back(q);
+        if (ids.size() > mk::BALANCE_MUTEX_MAX) fail(MDN_ERR_UNSUPPORTED, "AIR %u: %zu interactions in cached-encoding groups (at most %u)", i, ids.size(), mk::BALANCE_MUTEX_MAX);
+        auto group_of = [&](u32 q) { return (items[4 * (size_t)q] << 16) | (ann[q] >> 16); };
+        std::stable_sort(ids.begin(), ids.end(), [&](u32 a, u32 b) {
+            return std::make_pair(group_of(a), ann[a] & 0xFFFFu) < std::make_pair(group_of(b), ann[b] & 0xFFFFu); });
+        Mutex& m = mx[i];
+        m.pos.assign(nc, 0xFFFFFFFFu);
+        for (size_t b = 0; b < ids.size(); b++) {
+            u32 q = ids[b];
+            if (b && group_of(ids[b - 1]) == group_of(q) && (ann[ids[b - 1]] & 0xFFFFu) == (ann[q] & 0xFFFFu) && items[4 * (size_t)ids[b - 1] + 1] != items[4 * (size_t)q + 1])
+                fail(MDN_ERR_INVALID_ARG, "AIR %u: interactions %u and %u share mutex site %u of group %u but not a flag node (one site is one insert or batch call)", i, ids[b - 1], q, ann[q] & 0xFFFFu, ann[q] >> 16);
+            m.pos[q] = (u32)b; m.group.push_back(group_of(q)); m.site.push_back(ann[q] & 0xFFFFu);
+        }
+    }
+
+    // raw main traces of the lookup AIRs, column-major (column-major device traces are read where the caller keeps them)
+    std::vector<const u64*> main_cm(k, nullptr);
+    size_t main_total = 0;
+    for (u32 i = 0; i < k; i++) if (airs[i].has_lookup && !cm) main_total += ((size_t)1 << log_heights[i]) * airs[i].desc.width;
+    if (main_total) main_c.coef_buf.alloc(main_total, stream);
+    size_t co = 0;
+    for (u32 i = 0; i < k; i++) {
+        if (!airs[i].has_lookup) continue;
+        u64* dst = cm ? const_cast<u64*>(traces[i].values) : main_c.coef_buf.p + co;
+        if (!cm) co += ((size_t)1 << log_heights[i]) * airs[i].desc.width;
+        upload_matrix(traces[i], on_device, dst, cm);   // column-major: check only
+        main_cm[i] = dst;
+    }
+    check_input_flag("a main trace");
+    d_publics.alloc(std::max<size_t>(1, publics.size()), stream);
+    if (!publics.empty()) CUDA_OK(cudaMemcpyAsync(d_publics.p, publics.data(), publics.size() * sizeof(u64), cudaMemcpyHostToDevice, stream));
+    d_randomness.alloc(std::max<size_t>(1, 2 * (size_t)max_rand), stream);
+    if (max_rand) CUDA_OK(cudaMemcpyAsync(d_randomness.p, rnd, 2 * (size_t)max_rand * sizeof(u64), cudaMemcpyHostToDevice, stream));
+    std::vector<DevBuf> d_mx(k);
+    for (u32 i = 0; i < k; i++) {
+        const Mutex& m = mx[i];
+        if (m.group.empty()) continue;
+        std::vector<u32> words(m.pos);
+        words.insert(words.end(), m.group.begin(), m.group.end());
+        words.insert(words.end(), m.site.begin(), m.site.end());
+        d_mx[i].alloc((words.size() + 1) / 2, stream);
+        CUDA_OK(cudaMemcpyAsync(d_mx[i].p, words.data(), words.size() * sizeof(u32), cudaMemcpyHostToDevice, stream));
+    }
+    DevBuf ctr; ctr.alloc(5, stream);
+    CUDA_OK(cudaMemsetAsync(ctr.p, 0, 5 * sizeof(u64), stream));
+    unsigned long long* counters = (unsigned long long*)ctr.p;
+    std::vector<mk::BalanceArgs> ba(k);
+    auto run_rows = [&](u32 mode) {
+        for (u32 i = 0; i < k; i++) {
+            if (!airs[i].has_lookup) continue;
+            mk::BalanceArgs& b = ba[i];
+            b.mode = mode;
+            if (mk::launch_balance_rows(b, stream) != 0) fail(MDN_ERR_UNSUPPORTED, "AIR %u: lookup program too large for the interpreter", i);
+        }
+    };
+    for (u32 i = 0; i < k; i++) {
+        if (!airs[i].has_lookup) continue;
+        mk::BalanceArgs& b = ba[i];
+        b = mk::BalanceArgs{};
+        b.main_cm = main_cm[i]; b.log_n = log_heights[i]; b.prog = airs[i].lookup_dev;
+        b.publics = d_publics.p; b.challenges = d_randomness.p; b.instance = i;
+        const u32 nc = st->airs[i].lookup->program[3], na = (u32)mx[i].group.size();
+        if (na) {
+            const u32* w = (const u32*)d_mx[i].p;
+            b.mutex_pos = w; b.mutex_group = w + nc; b.mutex_site = w + nc + na; b.n_mutex = na;
+        }
+        b.counters = counters;
+    }
+
+    // 1. count: the table holds at most every push, so 2x the pushes in slots keeps it at most half full
+    run_rows(0);
+    u64 cnt[5];
+    CUDA_OK(cudaMemcpyAsync(cnt, ctr.p, sizeof cnt, cudaMemcpyDeviceToHost, stream));
+    CUDA_OK(cudaStreamSynchronize(stream));
+    const u64 n_push = cnt[0] + n_boundary, n_mutex = cnt[1];
+    u64 slots = 1024;
+    while (slots < 2 * n_push) slots <<= 1;
+    const size_t need = (size_t)(6 * slots + 6 * std::max<u64>(1, n_push) + 3 * std::max<u64>(1, n_mutex)) * sizeof(u64);
+    auto too_large = [&](const char* what) {
+        fail(MDN_ERR_UNSUPPORTED, "the balance table for %llu pushes needs %.1f GiB of device memory: %s",
+             (unsigned long long)n_push, need / 1073741824.0, what);
+    };
+    size_t arena_b = 0;
+    for (auto& sl : arena.slabs) arena_b += sl.size - sl.used;
+#ifndef MDN_EMULATED   // tests/emu has no device memory of its own: only the failed allocation below is reported there
+    size_t free_b = 0, total_b = 0;
+    CUDA_OK(cudaMemGetInfo(&free_b, &total_b));
+    char msg[64];
+    snprintf(msg, sizeof msg, "%.1f GiB are free", (free_b + arena_b) / 1073741824.0);
+    if (need > free_b + arena_b) too_large(msg);
+#endif
+    DevBuf table, unm, mut;
+    try {
+        table.alloc(6 * slots, stream); unm.alloc(6 * std::max<u64>(1, n_push), stream); mut.alloc(3 * std::max<u64>(1, n_mutex), stream);
+    } catch (const MdnError&) {   // an out-of-memory allocation leaves no error behind; nothing has been launched on the table yet
+        cudaGetLastError();
+        too_large("the allocation failed");
+    }
+    mk::BalanceTable t;
+    t.keys = table.p; t.sums = table.p + 2 * slots;
+    t.count = (unsigned long long*)(table.p + 4 * slots); t.first = (unsigned long long*)(table.p + 5 * slots); t.mask = slots - 1;
+    CUDA_OK(cudaMemsetAsync(t.keys, 0xFF, 2 * slots * sizeof(u64), stream));
+    CUDA_OK(cudaMemsetAsync(t.sums, 0, 3 * slots * sizeof(u64), stream));
+    CUDA_OK(cudaMemsetAsync(t.first, 0xFF, slots * sizeof(u64), stream));
+    CUDA_OK(cudaMemsetAsync(ctr.p, 0, 5 * sizeof(u64), stream));
+
+    // 2. insert, boundary, finish
+    for (auto& b : ba) { b.t = t; b.mutex_out = mut.p; }
+    run_rows(1);
+    DevBuf bnd;
+    if (n_boundary) {
+        bnd.alloc(3 * n_boundary, stream);
+        CUDA_OK(cudaMemcpyAsync(bnd.p, boundary, 3 * n_boundary * sizeof(u64), cudaMemcpyHostToDevice, stream));
+        mk::launch_balance_boundary(t, bnd.p, (u32)n_boundary, stream);
+    }
+    mk::launch_balance_finish(t, counters, unm.p, stream);
+    CUDA_OK(cudaMemcpyAsync(cnt, ctr.p, sizeof cnt, cudaMemcpyDeviceToHost, stream));
+    CUDA_OK(cudaStreamSynchronize(stream));
+    const u64 n_unm = cnt[4], n_distinct = cnt[3];
+    std::vector<u64> uh(6 * n_unm), mh(3 * n_mutex);
+    if (n_unm) CUDA_OK(cudaMemcpyAsync(uh.data(), unm.p, uh.size() * sizeof(u64), cudaMemcpyDeviceToHost, stream));
+    if (n_mutex) CUDA_OK(cudaMemcpyAsync(mh.data(), mut.p, mh.size() * sizeof(u64), cudaMemcpyDeviceToHost, stream));
+    CUDA_OK(cudaStreamSynchronize(stream));
+    CUDA_OK(cudaGetLastError());
+
+    // unmatched, ascending (c0, c1)
+    std::vector<u64> ord(n_unm);
+    for (u64 u = 0; u < n_unm; u++) ord[u] = u;
+    std::sort(ord.begin(), ord.end(), [&](u64 a, u64 b) { return std::make_pair(uh[6 * a], uh[6 * a + 1]) < std::make_pair(uh[6 * b], uh[6 * b + 1]); });
+    auto column_of = [&](u32 inst, u32 q) { return st->airs[inst].lookup->program[5 + 3 * (size_t)st->airs[inst].lookup->program[2] + 4 * (size_t)q]; };
+    bal_unmatched.assign(n_unm, mdn_unmatched{});
+    std::map<u64, u64> rank_of_slot;
+    std::map<std::pair<u64, u64>, u64> rank_of_denom;
+    u64 n_contrib = 0;
+    for (u64 j = 0; j < n_unm; j++) {
+        const u64* e = &uh[6 * ord[j]];
+        mdn_unmatched& m = bal_unmatched[j];
+        m.denom[0] = e[0]; m.denom[1] = e[1]; m.net_multiplicity = e[2]; m.n_pushes = e[3];
+        u32 inst = (u32)(e[4] >> 48), q = (u32)(e[4] & 0xFFFFFFu);
+        m.first_instance = inst == mk::BALANCE_BOUNDARY ? 0xFFFFFFFFu : inst;
+        m.first_row = inst == mk::BALANCE_BOUNDARY ? ~0ull : (e[4] >> 24) & 0xFFFFFFu;
+        m.first_interaction = q;
+        rank_of_slot[e[5]] = j; rank_of_denom[{e[0], e[1]}] = j;
+        n_contrib += e[3];
+    }
+    // 3. the pushes of the unmatched denominators, when the report can hold them
+    bal_contrib.clear();
+    const bool complete = n_contrib <= max_contrib;
+    if (complete && n_contrib) {
+        DevBuf con; con.alloc(3 * n_contrib, stream);
+        CUDA_OK(cudaMemsetAsync(ctr.p, 0, 5 * sizeof(u64), stream));
+        for (auto& b : ba) b.contrib_out = con.p;
+        run_rows(2);
+        CUDA_OK(cudaMemcpyAsync(cnt, ctr.p, sizeof cnt, cudaMemcpyDeviceToHost, stream));
+        CUDA_OK(cudaStreamSynchronize(stream));
+        std::vector<u64> ch(3 * cnt[2]);
+        if (cnt[2]) CUDA_OK(cudaMemcpyAsync(ch.data(), con.p, ch.size() * sizeof(u64), cudaMemcpyDeviceToHost, stream));
+        CUDA_OK(cudaStreamSynchronize(stream));
+        struct Rec { u64 rank, key, m; };
+        std::vector<Rec> recs;
+        for (u64 p = 0; p < cnt[2]; p++) recs.push_back({rank_of_slot.at(ch[3 * p]), ch[3 * p + 1], ch[3 * p + 2]});
+        for (size_t q = 0; q < n_boundary; q++) {
+            auto it = rank_of_denom.find({boundary[3 * q], boundary[3 * q + 1]});
+            if (it != rank_of_denom.end()) recs.push_back({it->second, mk::balance_key(mk::BALANCE_BOUNDARY, 0, (u32)q), boundary[3 * q + 2]});
+        }
+        if (recs.size() != n_contrib) fail(MDN_ERR_CUDA, "balance check: %zu pushes collected, %llu counted", recs.size(), (unsigned long long)n_contrib);
+        std::sort(recs.begin(), recs.end(), [](const Rec& a, const Rec& b) { return std::make_pair(a.rank, a.key) < std::make_pair(b.rank, b.key); });
+        for (const Rec& r : recs) {
+            mdn_balance_push p{};
+            u32 inst = (u32)(r.key >> 48), q = (u32)(r.key & 0xFFFFFFu);
+            p.multiplicity = r.m; p.interaction = q;
+            if (inst == mk::BALANCE_BOUNDARY) { p.instance = 0xFFFFFFFFu; p.row = ~0ull; p.column = 0xFFFFFFFFu; }
+            else { p.instance = inst; p.row = (r.key >> 24) & 0xFFFFFFu; p.column = column_of(inst, q); }
+            bal_contrib.push_back(p);
+        }
+    }
+    // mutex violations, (instance, row, column, group)
+    std::vector<u64> mo(n_mutex);
+    for (u64 v = 0; v < n_mutex; v++) mo[v] = v;
+    std::sort(mo.begin(), mo.end(), [&](u64 a, u64 b) { return std::make_pair(mh[3 * a], mh[3 * a + 1]) < std::make_pair(mh[3 * b], mh[3 * b + 1]); });
+    bal_mutex.clear();
+    for (u64 v = 0; v < n_mutex && v < max_contrib; v++) {
+        const u64* e = &mh[3 * mo[v]];
+        mdn_mutex_violation mv{};
+        mv.instance = (u32)(e[0] >> 32); mv.row = e[0] & 0xFFFFFFFFu; mv.column = (u32)(e[1] >> 32); mv.group = (u32)e[1]; mv.active_flags = (u32)e[2];
+        bal_mutex.push_back(mv);
+    }
+
+    memset(out, 0, sizeof *out);
+    out->n_pushes = n_push; out->n_denominators = n_distinct; out->n_unmatched = n_unm; out->n_mutex_violations = n_mutex;
+    out->n_contributions = n_contrib; out->contributions_complete = complete; out->n_skipped_airs = skipped;
+    out->unmatched = bal_unmatched.data(); out->contributions = complete ? bal_contrib.data() : nullptr;
+    out->mutex_violations = bal_mutex.data(); out->n_mutex_listed = bal_mutex.size();
+    out->holds = n_unm == 0 && n_mutex == 0;
 }
 
 // mdn_aux_builder_device for instance `inst`: the aux columns go straight into `aux_slot` (column-major, on the session's
@@ -2316,6 +2566,23 @@ int mdn_check_constraints(mdn_session* s, const mdn_statement* st, const mdn_mat
         CUDA_OK(cudaSetDevice(s->device));
         s->check_constraints(st, traces, preprocessed, challenger, build_aux, aux_ctx, flags, out);
         if (randomness_out) for (size_t i = 0; i < s->randomness.size(); i++) { randomness_out[2 * i] = s->randomness[i].a; randomness_out[2 * i + 1] = s->randomness[i].b; }
+    }
+    s->reset_proof();
+    API_CATCH(s)
+}
+
+int mdn_check_trace_balance(mdn_session* s, const mdn_statement* st, const mdn_matrix* traces, const uint64_t* randomness,
+                            const uint64_t* boundary, size_t n_boundary, const uint32_t* const* mutex_sites,
+                            uint64_t max_contributions, uint32_t flags, mdn_balance_report* out) {
+    if (!s) return MDN_ERR_INVALID_ARG;
+    // refused before any device work, so that a staged proof in progress stays intact
+    if (s->in_proof) { s->error = "mdn_check_trace_balance called inside a proof (between mdn_prove_begin and mdn_prove_finish)"; return MDN_ERR_INVALID_ARG; }
+    if (s->shard_world > 1) { s->error = "mdn_check_trace_balance does not run on a session split over ranks (mdn_session_set_shard world > 1)"; return MDN_ERR_UNSUPPORTED; }
+    API_TRY(s)
+    {
+        ArenaScope proof_memory(s->use_arena ? &s->arena : nullptr);
+        CUDA_OK(cudaSetDevice(s->device));
+        s->check_trace_balance(st, traces, randomness, boundary, n_boundary, mutex_sites, max_contributions, flags, out);
     }
     s->reset_proof();
     API_CATCH(s)

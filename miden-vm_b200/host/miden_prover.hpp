@@ -16,6 +16,8 @@
 //   StarkProofData { log_trace_heights, transcript }              miden::StarkProofData
 //   debug::check_constraints(&prover_statement, challenger)       miden::check_constraints(config, statement, challenger)
 //     (debug.rs:70-214; panics -> ConstraintViolation)             (every constraint on every row, on the device, no proof)
+//   lookup::debug::check_trace_balance(air, main, .., challenges)  miden::check_trace_balance(config, statement, challenges, ..)
+//     (air/src/lookup/debug/trace/mod.rs:169-309) -> BalanceReport  -> miden::BalanceReport (to_string() = its Display)
 //   ProverError::{Instance, Domain, ..}  prover/mod.rs:582-596    miden::ProverError { kind, what() }
 //   HashFunction::{Blake3_256, Keccak, Rpo256, Poseidon2, Rpx256} -> the config constructor (prover/src/lib.rs:245-301)
 //                                                                 miden::HashFunction + StarkConfig::with_hash
@@ -24,6 +26,7 @@
 // CUDA device throws ProverError{NoDevice}.
 #pragma once
 #include "../../include/miden_b200.h"
+#include <algorithm>
 #include <array>
 #include <cstdint>
 #include <functional>
@@ -348,6 +351,81 @@ inline void check_constraints(const StarkConfig& config, const DeviceProverState
                                                 config.hash_challenger() ? nullptr : &challenger.raw, nullptr, nullptr,
                                                 MDN_FLAG_DEVICE_TRACES | MDN_FLAG_COLUMN_MAJOR, nullptr, &rep));
     if (!rep.holds) throw ConstraintViolation(rep);
+}
+
+// check_trace_balance's BalanceReport (air/src/lookup/debug/trace/mod.rs:44-95), copied out of the session.  A push names its
+// interaction (the index in the AIR's lookup program) where the reference names its group and message; the caller maps
+// the index back to its insert site.  Boundary emissions have instance / column 0xFFFFFFFF and row UINT64_MAX.
+struct BalanceReport {
+    struct Push { uint32_t instance, column, interaction; uint64_t row; Felt multiplicity; };
+    struct Unmatched { QuadFelt denom; Felt net_multiplicity; uint64_t n_pushes; Push first; std::vector<Push> contributions; };
+    struct MutexViolation { uint32_t instance; uint64_t row; uint32_t column, group, active_flags; };
+    std::vector<Unmatched> unmatched;
+    std::vector<MutexViolation> mutex_violations;
+    uint64_t n_pushes = 0, n_denominators = 0, n_mutex_violations = 0;
+    uint32_t n_skipped_airs = 0;
+    bool contributions_complete = true;
+    bool is_ok() const { return unmatched.empty() && n_mutex_violations == 0; }
+    // the reference's Display (mod.rs:97-138): at most four pushes per unmatched denominator
+    std::string to_string() const {
+        if (is_ok()) return "BalanceReport: OK\n";
+        std::string s = "BalanceReport: " + std::to_string(unmatched.size()) + " unmatched, " + std::to_string(n_mutex_violations) + " mutex violations\n";
+        auto ef = [](const QuadFelt& q) { return "(" + std::to_string(q[0]) + ", " + std::to_string(q[1]) + ")"; };
+        for (const Unmatched& u : unmatched) {
+            s += "  denom " + ef(u.denom) + " net multiplicity " + std::to_string(u.net_multiplicity) + "\n";
+            const std::vector<Push>& shown = u.contributions.empty() ? std::vector<Push>{u.first} : u.contributions;
+            for (size_t i = 0; i < shown.size() && i < 4; i++)
+                s += "    row=" + std::to_string(shown[i].row) + " col=" + std::to_string(shown[i].column) + " interaction=" + std::to_string(shown[i].interaction) +
+                     " mult=" + std::to_string(shown[i].multiplicity) + (shown[i].instance == 0xFFFFFFFFu ? " [boundary]" : " instance=" + std::to_string(shown[i].instance)) + "\n";
+            if (u.n_pushes > std::min<uint64_t>(shown.size(), 4)) s += "    \xE2\x80\xA6 " + std::to_string(u.n_pushes - std::min<uint64_t>(shown.size(), 4)) + " more contributions\n";
+        }
+        for (const MutexViolation& m : mutex_violations)
+            s += "  mutex violation at row " + std::to_string(m.row) + " col " + std::to_string(m.column) + " group " + std::to_string(m.group) + ": " +
+                 std::to_string(m.active_flags) + " active flags\n";
+        return s;
+    }
+};
+
+// check_trace_balance(air, main_trace, .., challenges) (air/src/lookup/debug/trace/mod.rs:169-189), jointly over every AIR of the
+// statement with a lowered lookup program, on the device.  `challenges` = the randomness (alpha, beta, ...) the caller chose
+// (e.g. what mdn_prove_begin sampled); `boundary` = the (denominator, multiplicity) pairs eval_boundary emits; `mutex_sites` =
+// per AIR, empty or one word per interaction (include/miden_b200.h).  Throws ProverError on malformed input only.
+inline BalanceReport check_trace_balance(const StarkConfig& config, const ProverStatement& ps, const std::vector<QuadFelt>& challenges,
+                                         const std::vector<std::pair<QuadFelt, Felt>>& boundary = {},
+                                         const std::vector<std::vector<uint32_t>>& mutex_sites = {}, uint64_t max_contributions = 1u << 16) {
+    detail::Lowered low(ps.statement);
+    std::vector<mdn_matrix> mats;
+    for (const RowMajorMatrix& t : ps.traces) mats.push_back(t.raw());
+    std::vector<Felt> rnd, bnd;
+    for (const QuadFelt& c : challenges) { rnd.push_back(c[0]); rnd.push_back(c[1]); }
+    for (const auto& b : boundary) { bnd.push_back(b.first[0]); bnd.push_back(b.first[1]); bnd.push_back(b.second); }
+    std::vector<const uint32_t*> sites(ps.statement.airs.size(), nullptr);
+    for (size_t i = 0; i < mutex_sites.size() && i < sites.size(); i++) if (!mutex_sites[i].empty()) sites[i] = mutex_sites[i].data();
+    mdn_balance_report r{};
+    detail::check(config, mdn_check_trace_balance(config.session(), &low.st, mats.data(), rnd.empty() ? nullptr : rnd.data(),
+                                                   bnd.empty() ? nullptr : bnd.data(), boundary.size(), mutex_sites.empty() ? nullptr : sites.data(),
+                                                   max_contributions, 0, &r));
+    BalanceReport out;
+    out.n_pushes = r.n_pushes; out.n_denominators = r.n_denominators; out.n_mutex_violations = r.n_mutex_violations;
+    out.n_skipped_airs = r.n_skipped_airs; out.contributions_complete = r.contributions_complete != 0;
+    size_t c = 0;
+    for (uint64_t j = 0; j < r.n_unmatched; j++) {
+        const mdn_unmatched& u = r.unmatched[j];
+        BalanceReport::Unmatched e{{u.denom[0], u.denom[1]}, u.net_multiplicity, u.n_pushes,
+                                   {u.first_instance, 0xFFFFFFFFu, u.first_interaction, u.first_row, 0}, {}};
+        if (r.contributions_complete)
+            for (uint64_t q = 0; q < u.n_pushes; q++, c++) {
+                const mdn_balance_push& p = r.contributions[c];
+                e.contributions.push_back({p.instance, p.column, p.interaction, p.row, p.multiplicity});
+            }
+        if (!e.contributions.empty()) e.first = e.contributions.front();
+        out.unmatched.push_back(std::move(e));
+    }
+    for (uint64_t j = 0; j < r.n_mutex_listed; j++) {
+        const mdn_mutex_violation& m = r.mutex_violations[j];
+        out.mutex_violations.push_back({m.instance, m.row, m.column, m.group, m.active_flags});
+    }
+    return out;
 }
 
 // Preprocessed::build(&statement, &config): the LDE tree lives on the device inside the config's session
