@@ -174,6 +174,10 @@ enum {
  * returns.  There, the `aux` matrices of mdn_prove_commit_aux are column-major device matrices too (aux_values stay on
  * the host).  MDN_FLAG_COLUMN_MAJOR without MDN_FLAG_DEVICE_TRACES, or a misaligned pointer: MDN_ERR_INVALID_ARG.
  * The preprocessed traces (mdn_session_set_preprocessed, mdn_check_constraints) stay host row-major.
+ * mdn_check_lookup_folds takes its `aux` matrices in the same layout (width 2 * aux_width: coordinate k of aux column c
+ * is column 2c + k) and reads them in place; its `folds_out` buffers are then device buffers of 4 * num_columns columns
+ * of 2^log_height rows, column 4c + w holding word w of (V c0, V c1, U c0, U c1) of aux column c:
+ * folds_out[i][(size_t)(4 * c + w) << log_height | r].
  *
  * Aux traces of such calls come from the session's device aux builder, called in instance order for every AIR without
  * mdn_air.lookup, after the randomness is sampled:
@@ -401,6 +405,79 @@ int mdn_check_trace_balance(mdn_session* s, const mdn_statement* st, const mdn_m
                             const uint64_t* boundary, size_t n_boundary /* n x {denom c0, denom c1, multiplicity} */,
                             const uint32_t* const* mutex_sites /* per AIR, NULL or one word per interaction; NULL = none */,
                             uint64_t max_contributions, uint32_t flags, mdn_balance_report* out);
+
+/* ---- cross-check a LogUp aux trace against the constraint path, without proving: collect_column_oracle_folds -----
+ * (air/src/lookup/debug/trace/mod.rs:191-207 with run_trace_walk :220-282, filled by DebugTraceBuilder,
+ * debug/trace/builder.rs:114-149,234-372; compared as assert_prover_matches_oracle does,
+ * processor/src/trace/tests/lookup.rs:185-265).  For every row r of every AIR that carries a lowered mdn_air.lookup and
+ * every aux column c it computes the constraint-path fold (V_c(r), U_c(r)), starting from (0, 1) each row, and checks
+ * the aux trace against it:
+ *   aux[r][c]               == V_c(r) / U_c(r)            for c >= 1           (kind 1 otherwise)
+ *   aux[r+1][0] - aux[r][0] == sum over c of V_c(r)/U_c(r)                     (kind 2 otherwise)
+ *   U_c(r) != 0                                                                (kind 3 otherwise: reported, not divided)
+ * A column whose U is zero is left out of the kind 1 comparison, and a row with any zero U out of the kind 2 comparison.
+ * Rows, the next-row wrap, periodic values, flags and the "multiplicity as given" rule are those of
+ * mdn_check_trace_balance; nothing is observed and no hash configuration is consulted.  Boundary emissions do not enter
+ * the folds (mod.rs:194-195).  AIRs without mdn_air.lookup are skipped and counted.
+ * The fold is the builder's, which (V, U) is compared with as a pair, not "sum m/d, then split":
+ *   batch  : (N, D) <- (N * d + D * m, D * d) per interaction, from (0, 1)              (builder.rs:353-355,369-371)
+ *   group  : (V_g, U_g) <- (V_g + N * flag, U_g + (D - 1) * flag) per insert / insert_encoded / batch call, from (0, 1),
+ *            a single insert being the batch of its one interaction; the flag enters as a field element (an
+ *            interaction without a flag node has flag 1) and a zero flag adds nothing   (builder.rs:245-252,278-279)
+ *   column : (V, U) <- (V * U_g + V_g * U, U * U_g) per group, from (0, 1)              (builder.rs:144-146)
+ * Of a group_with_cached_encoding only the canonical closure is folded, which is the one the lowered program carries
+ * (builder.rs:177-181).  With boolean flags of which at most one is set per group this equals the prover path
+ * (k_logup_rows: one rational per column over the active pushes); where a flag is not boolean or two flags of a group
+ * are set together the two paths differ, and this call says where.
+ * The lowered mdn_lookup program carries column, flag, multiplicity and denominator per interaction but not where a
+ * group or a batch begins, so that comes as an optional per-interaction argument (as mutex_sites does for
+ * mdn_check_trace_balance; mdn_lookup is unchanged):
+ *   fold_marks : NULL, or per AIR (instance order) NULL or one word per interaction of its lookup program, emission
+ *                order: 3 = the interaction opens a new group (and the first insert / batch call of it), 1 = it opens a
+ *                new insert / insert_encoded / batch call in the open group, 0 = it continues the batch of the previous
+ *                interaction.  Interaction 0 and every interaction whose column differs from its predecessor's carry
+ *                3; an interaction marked 0 shares its predecessor's flag node.  NULL: every interaction is a group of
+ *                its own, i.e. (V, U) <- (V * (1 + (d - 1) * flag) + m * flag * U, U * (1 + (d - 1) * flag)).
+ *   randomness : as mdn_check_trace_balance (2 * max num_randomness u64, canonical).
+ *   aux        : NULL, or per AIR (instance order; entries of AIRs without mdn_air.lookup are ignored) the aux trace
+ *                in this library's layout: 2^log_height rows (the reference's (n+1)-row `accumulate` output without
+ *                its last row, aux_builder.rs:49-97), base-flattened EF, width 2 * aux_width, canonical; host row-major,
+ *                or on the device as the traces are (MDN_FLAG_DEVICE_TRACES, | MDN_FLAG_COLUMN_MAJOR: read in place).
+ *                NULL: the call first runs the device LogUp build (k_logup_rows + k_scan_*) on the same traces and
+ *                challenges and checks that -- the prover path against the constraint path.  That build refuses a zero
+ *                denominator (MDN_ERR_INVALID_ARG), so a kind 3 report needs an explicit aux.
+ *   aux_finals : with aux, per AIR 2 u64 (host, canonical): the value aux[n][0] would hold (aux value 0), which closes
+ *                the last row's delta: aux_finals[i] - aux[n-1][0].  Must be NULL when aux is NULL.
+ *   folds_out  : NULL, or per AIR NULL or a buffer of rows x num_columns x 4 u64, entry (r, c) = (V c0, V c1, U c0, U c1)
+ *                at folds_out[i][4 * (r * num_columns + c)]: host memory, device memory with MDN_FLAG_DEVICE_TRACES
+ *                (16-byte aligned), column-major planes with | MDN_FLAG_COLUMN_MAJOR (layout above).
+ * First failure: the least (instance, row, column) in instance order; failing_rows and zero_u count over all AIRs.
+ * Returns MDN_OK whenever the check ran, whatever it found.  Refusals and statuses as mdn_check_trace_balance: malformed
+ * or non-canonical randomness, aux, finals or marks MDN_ERR_INVALID_ARG; a call between mdn_prove_begin and
+ * mdn_prove_finish MDN_ERR_INVALID_ARG and a session split over ranks MDN_ERR_UNSUPPORTED, both before any device work;
+ * a host folds_out whose device staging is larger than the free device memory MDN_ERR_UNSUPPORTED.  Nothing
+ * mdn_get_info / mdn_get_timings report about the last proof changes, and later proofs are unchanged. */
+typedef struct {
+    uint32_t holds;            /* 1: every checked (row, column) agrees and no U is zero */
+    uint32_t kind;             /* 0 none, 1 fraction column mismatch (c >= 1), 2 accumulator mismatch (c = 0), 3 zero U */
+    uint32_t instance;         /* first failure: least (instance, row, column), instance order */
+    uint32_t column;
+    uint64_t row;
+    uint64_t fold[4];          /* (V c0,c1, U c0,c1) of that (row, column) */
+    uint64_t expected[2];      /* kind 1: V/U; kind 2: sum_c V_c/U_c; kind 3: 0 (c >= 1) or the sum over the non-zero U (c = 0) */
+    uint64_t actual[2];        /* kind 1, 3 (c >= 1): aux[r][c]; kind 2, 3 (c = 0): aux[r+1][0] - aux[r][0] */
+    uint64_t failing_rows;     /* (instance, row) pairs with at least one disagreement or zero U, over all AIRs */
+    uint64_t zero_u;           /* (instance, row, column) triples with U == 0 */
+    uint32_t n_skipped_airs;   /* AIRs without mdn_air.lookup */
+    uint32_t reserved;
+} mdn_fold_report;
+int mdn_check_lookup_folds(mdn_session* s, const mdn_statement* st, const mdn_matrix* traces /* instance order */,
+                           const uint64_t* randomness /* 2 * max num_randomness: alpha, beta, ... */,
+                           const uint32_t* const* fold_marks /* per AIR, NULL or one word per interaction; NULL = none */,
+                           const mdn_matrix* aux /* instance order, width 2 * aux_width; NULL: the device LogUp build */,
+                           const uint64_t* const* aux_finals /* per AIR 2 u64; NULL with aux == NULL */,
+                           uint64_t* const* folds_out /* NULL, or per AIR NULL or rows x num_columns x 4 u64 */,
+                           uint32_t flags, mdn_fold_report* out);
 
 /* wincode/bincode-default layout of StarkProofData (prover/src/lib.rs:347-354): u64-LE length +
  * height bytes; u64-LE length + u64-LE felts; u64-LE length + 32-byte commitments.  Returns the

@@ -233,6 +233,24 @@ pub struct MdnBalanceReport {
     pub n_mutex_listed: u64,
 }
 
+/// `mdn_fold_report`: the outcome of `mdn_check_lookup_folds` (kind 1 fraction column, 2 accumulator, 3 zero U).
+#[repr(C)]
+#[derive(Clone, Copy, Debug, Default)]
+pub struct MdnFoldReport {
+    pub holds: u32,
+    pub kind: u32,
+    pub instance: u32,
+    pub column: u32,
+    pub row: u64,
+    pub fold: [u64; 4],
+    pub expected: [u64; 2],
+    pub actual: [u64; 2],
+    pub failing_rows: u64,
+    pub zero_u: u64,
+    pub n_skipped_airs: u32,
+    pub reserved: u32,
+}
+
 pub enum MdnSession {}
 
 /// `mdn_hash_kind` (include/miden_b200.h): which `miden_air::config` constructor the session follows.
@@ -310,6 +328,18 @@ unsafe extern "C" {
         max_contributions: u64,
         flags: u32,
         out: *mut MdnBalanceReport,
+    ) -> c_int;
+    pub fn mdn_check_lookup_folds(
+        s: *mut MdnSession,
+        st: *const MdnStatement,
+        traces: *const MdnMatrix,
+        randomness: *const u64,
+        fold_marks: *const *const u32,
+        aux: *const MdnMatrix,
+        aux_finals: *const *const u64,
+        folds_out: *const *mut u64,
+        flags: u32,
+        out: *mut MdnFoldReport,
     ) -> c_int;
     pub fn mdn_session_set_preprocessed(
         s: *mut MdnSession,

@@ -100,6 +100,9 @@ class LookupProgramBuilder(ProgramBuilder):
         self._groups = [0] * num_columns       # next group index per column (the reference's group_idx)
         self._group = None                     # (column, group index, cached, next site) of the open group
         self._batch_site = None
+        # fold annotation of every interaction (mdn_check_lookup_folds): 3 opens a group, 1 an insert / batch, 0 continues a batch
+        self.marks: list[int] = []
+        self._opens = 3                        # what the next insert opens
 
     class _Scope:
         def __init__(self, enter, leave):
@@ -118,10 +121,12 @@ class LookupProgramBuilder(ProgramBuilder):
             assert self._group is None, "groups do not nest"
             self._group = [column, self._groups[column], cached, 0]
             self._groups[column] += 1
+            self._opens = 3
             return self._group[1]
 
         def leave():
             self._group = None
+            self._opens = 3
         return self._Scope(enter, leave)
 
     def batch(self):
@@ -129,9 +134,11 @@ class LookupProgramBuilder(ProgramBuilder):
         def enter():
             assert self._group is not None and self._batch_site is None
             self._batch_site = self._new_site()
+            self._opens |= 1
 
         def leave():
             self._batch_site = None
+            self._opens |= 1
         return self._Scope(enter, leave)
 
     def _new_site(self):
@@ -144,6 +151,11 @@ class LookupProgramBuilder(ProgramBuilder):
         """One word per interaction for mdn_check_trace_balance: 0xFFFFFFFF outside a cached-encoding group, else
         (group index within its column) << 16 | site."""
         return np.array(self.sites, dtype=np.uint32)
+
+    def fold_marks(self) -> np.ndarray:
+        """One word per interaction for mdn_check_lookup_folds: 3 when it opens a group (an insert outside `group` is a
+        group of its own), 1 when it opens an insert or batch in the open group, 0 when it continues the open batch."""
+        return np.array(self.marks, dtype=np.uint32)
 
     def bus_prefix(self, bus: int, max_message_width: int) -> Expr:
         """`Challenges::new`: bus_prefix[i] = alpha + (i + 1) * beta^W (air/src/lookup/challenges.rs)."""
@@ -165,6 +177,8 @@ class LookupProgramBuilder(ProgramBuilder):
     def insert(self, column: int, flag, multiplicity: Expr, denominator: Expr):
         self.interactions.append((column, NO_FLAG if flag is None else flag.id, multiplicity.id, denominator.id))
         g = self._group
+        self.marks.append(self._opens)
+        self._opens = 3 if g is None else (0 if self._batch_site is not None else 1)
         if g is None or not g[2]:
             self.sites.append(NO_FLAG)
             return

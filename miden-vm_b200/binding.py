@@ -98,6 +98,20 @@ class BalanceReport(C.Structure):
                 ("mutex_violations", C.POINTER(MutexViolation)), ("n_mutex_listed", C.c_uint64)]
 
 
+class FoldReport(C.Structure):
+    """`mdn_fold_report`: the outcome of mdn_check_lookup_folds (kind 1 = fraction column, 2 = accumulator, 3 = zero U)."""
+    _fields_ = [("holds", C.c_uint32), ("kind", C.c_uint32), ("instance", C.c_uint32), ("column", C.c_uint32),
+                ("row", C.c_uint64), ("fold", C.c_uint64 * 4), ("expected", C.c_uint64 * 2), ("actual", C.c_uint64 * 2),
+                ("failing_rows", C.c_uint64), ("zero_u", C.c_uint64), ("n_skipped_airs", C.c_uint32), ("reserved", C.c_uint32)]
+
+
+def fold_report_dict(rep: FoldReport) -> dict:
+    """A FoldReport as plain Python values."""
+    return dict(holds=rep.holds, kind=rep.kind, instance=rep.instance, column=rep.column, row=rep.row, fold=tuple(rep.fold),
+                expected=tuple(rep.expected), actual=tuple(rep.actual), failing_rows=rep.failing_rows, zero_u=rep.zero_u,
+                n_skipped_airs=rep.n_skipped_airs)
+
+
 BOUNDARY = 0xFFFFFFFF     # instance / column of a boundary emission in a balance report (row = 2^64 - 1)
 
 
@@ -132,6 +146,7 @@ EXPORTS = [
     "mdn_session_set_preprocessed", "mdn_session_set_jit", "mdn_jit_compile_check", "mdn_jit_status", "mdn_abi_layout",
     "mdn_session_set_external_check", "mdn_session_set_hash", "mdn_session_set_hash_challenger",
     "mdn_check_constraints", "mdn_session_set_device_aux_builder", "mdn_check_trace_balance",
+    "mdn_check_lookup_folds",
 ]
 
 _lib = None
@@ -174,6 +189,9 @@ def lib():
                                             C.POINTER(ConstraintReport)]
         L.mdn_check_trace_balance.argtypes = [C.c_void_p, C.POINTER(Statement), C.POINTER(Matrix), u64p, u64p, C.c_size_t,
                                               C.POINTER(u32p), C.c_uint64, C.c_uint32, C.POINTER(BalanceReport)]
+        L.mdn_check_lookup_folds.argtypes = [C.c_void_p, C.POINTER(Statement), C.POINTER(Matrix), u64p, C.POINTER(u32p),
+                                             C.POINTER(Matrix), C.POINTER(u64p), C.POINTER(u64p), C.c_uint32,
+                                             C.POINTER(FoldReport)]
         L.mdn_prove_begin.argtypes = [C.c_void_p, C.POINTER(Statement), C.POINTER(Matrix), C.POINTER(Challenger),
                                       C.c_uint32, u64p, u64p]
         L.mdn_prove_commit_aux.argtypes = [C.c_void_p, C.POINTER(Matrix), C.POINTER(u64p), u64p]
@@ -360,6 +378,38 @@ class Session:
                                                   ptr(bnd) if bnd.size else None, len(bnd) // 3, sites, max_contributions,
                                                   flags, C.byref(rep)))
         return balance_report_dict(rep)
+
+    def check_lookup_folds(self, statement: Statement, traces, randomness, fold_marks=None, aux=None, aux_finals=None,
+                           folds_out=None, flags=0) -> dict:
+        """`collect_column_oracle_folds` (air/src/lookup/debug/trace/mod.rs:196) on the device, compared with an aux trace
+        as `assert_prover_matches_oracle` compares them.  fold_marks: per AIR None or LookupProgramBuilder.fold_marks();
+        aux: Matrix array in instance order (host row-major, or device as `flags` say) with aux_finals, per AIR None or
+        (c0, c1) -- or None for the device LogUp build of the same call; folds_out: per AIR None, a uint64 numpy array of
+        rows * num_columns * 4 words to fill, or a device address (int) with FLAG_DEVICE_TRACES.  Returns fold_report_dict."""
+        rnd = np.ascontiguousarray(np.asarray(randomness, dtype=np.uint64).reshape(-1))
+        n, keep = statement.n_airs, []
+        marks = fins = outs = None
+        if fold_marks is not None:
+            marks = (u32p * n)()
+            for i, m in enumerate(fold_marks):
+                if m is not None:
+                    keep.append(np.ascontiguousarray(m, dtype=np.uint32))
+                    marks[i] = keep[-1].ctypes.data_as(u32p)
+        if aux_finals is not None:
+            fins = (u64p * n)()
+            for i, f in enumerate(aux_finals):
+                if f is not None:
+                    keep.append(np.array([int(f[0]), int(f[1])], dtype=np.uint64))
+                    fins[i] = ptr(keep[-1])
+        if folds_out is not None:
+            outs = (u64p * n)()
+            for i, o in enumerate(folds_out):
+                if o is not None:
+                    outs[i] = ptr(o) if isinstance(o, np.ndarray) else C.cast(C.c_void_p(int(o)), u64p)
+        rep = FoldReport()
+        self._check(lib().mdn_check_lookup_folds(self._h, C.byref(statement), traces, ptr(rnd) if rnd.size else None, marks,
+                                                 aux, fins, outs, flags, C.byref(rep)))
+        return fold_report_dict(rep)
 
     def info(self, what: int, cap: int = 0) -> np.ndarray:
         n = lib().mdn_get_info(self._h, what, None, 0)

@@ -816,6 +816,20 @@ int launch_constraints(const ConstraintArgs& a, cudaStream_t st) {
 // =============================================================================================
 // LogUp aux trace (trace-domain interpreter + EF scan)
 // =============================================================================================
+// one instruction of a compiled lookup program that is not an EMIT: the leaves a LookupBuilder exposes and the arithmetic
+// ops, at trace row r (rn = the next row, wrapping).  Shared by the kernels that interpret lookup programs.
+#define LOOKUP_NODE_CASES(a, N, r, rn, per_row, slot, x, y, ext, v)                                                     \
+    case 0: v = gl::e2((a).main_cm[(size_t)(y) * (N) + ((x) ? (rn) : (r))], 0); break;                                  \
+    case 2: v = gl::e2((a).publics[x], 0); break;                                                                       \
+    case 3: v = gl::e2((a).challenges[2 * (x)], (a).challenges[2 * (x) + 1]); break;                                    \
+    case 8: v = gl::e2((a).prog.consts[x], 0); break;                                                                   \
+    case 9: v = gl::e2((a).prog.consts[x], (a).prog.consts[(x) + 1]); break;                                            \
+    case 10: v = (ext) ? gl::e2_add(slot[x], slot[y]) : gl::e2(gl::add(slot[x].a, slot[y].a), 0); break;                \
+    case 11: v = (ext) ? gl::e2_sub(slot[x], slot[y]) : gl::e2(gl::sub(slot[x].a, slot[y].a), 0); break;                \
+    case 12: v = (ext) ? gl::e2_mul(slot[x], slot[y]) : gl::e2(gl::mul(slot[x].a, slot[y].a), 0); break;                \
+    case 13: v = (ext) ? gl::e2_neg(slot[x]) : gl::e2(gl::neg(slot[x].a), 0); break;                                    \
+    case 14: v = gl::e2((a).prog.periodic[(per_row) + (x)], 0); break;
+
 template <int MAXS>
 __global__ void __launch_bounds__(128) k_logup_rows(LogupArgs a) {
     size_t N = (size_t)1 << a.log_n;
@@ -832,16 +846,7 @@ __global__ void __launch_bounds__(128) k_logup_rows(LogupArgs a) {
         u32 op = ins.x & 0xff, ext = ins.x >> 8, x = ins.z, y = ins.w;
         E2 v;
         switch (op) {
-            case 0: v = gl::e2(a.main_cm[(size_t)y * N + (x ? rn : r)], 0); break;
-            case 2: v = gl::e2(a.publics[x], 0); break;
-            case 3: v = gl::e2(a.challenges[2 * x], a.challenges[2 * x + 1]); break;
-            case 8: v = gl::e2(a.prog.consts[x], 0); break;
-            case 9: v = gl::e2(a.prog.consts[x], a.prog.consts[x + 1]); break;
-            case 10: v = ext ? gl::e2_add(slot[x], slot[y]) : gl::e2(gl::add(slot[x].a, slot[y].a), 0); break;
-            case 11: v = ext ? gl::e2_sub(slot[x], slot[y]) : gl::e2(gl::sub(slot[x].a, slot[y].a), 0); break;
-            case 12: v = ext ? gl::e2_mul(slot[x], slot[y]) : gl::e2(gl::mul(slot[x].a, slot[y].a), 0); break;
-            case 13: v = ext ? gl::e2_neg(slot[x]) : gl::e2(gl::neg(slot[x].a), 0); break;
-            case 14: v = gl::e2(a.prog.periodic[per_row + x], 0); break;
+            LOOKUP_NODE_CASES(a, N, r, rn, per_row, slot, x, y, ext, v)
             default: {   // 17 EMIT
                 u32 c = ins.y, fs = x & 0xffffu, ms = x >> 16;
                 if (fs != 0xffffu && slot[fs].a == 0) continue;          // prover.rs:357: flag == 0 skips the push
@@ -999,16 +1004,7 @@ __global__ void __launch_bounds__(128) k_balance_rows(BalanceArgs a) {
         u32 op = ins.x & 0xff, ext = ins.x >> 8, x = ins.z, y = ins.w;
         E2 v;
         switch (op) {
-            case 0: v = gl::e2(a.main_cm[(size_t)y * N + (x ? rn : r)], 0); break;
-            case 2: v = gl::e2(a.publics[x], 0); break;
-            case 3: v = gl::e2(a.challenges[2 * x], a.challenges[2 * x + 1]); break;
-            case 8: v = gl::e2(a.prog.consts[x], 0); break;
-            case 9: v = gl::e2(a.prog.consts[x], a.prog.consts[x + 1]); break;
-            case 10: v = ext ? gl::e2_add(slot[x], slot[y]) : gl::e2(gl::add(slot[x].a, slot[y].a), 0); break;
-            case 11: v = ext ? gl::e2_sub(slot[x], slot[y]) : gl::e2(gl::sub(slot[x].a, slot[y].a), 0); break;
-            case 12: v = ext ? gl::e2_mul(slot[x], slot[y]) : gl::e2(gl::mul(slot[x].a, slot[y].a), 0); break;
-            case 13: v = ext ? gl::e2_neg(slot[x]) : gl::e2(gl::neg(slot[x].a), 0); break;
-            case 14: v = gl::e2(a.prog.periodic[per_row + x], 0); break;
+            LOOKUP_NODE_CASES(a, N, r, rn, per_row, slot, x, y, ext, v)
             default: {   // 17 EMIT of interaction k = ext
                 u32 fs = x & 0xffffu, ms = x >> 16, k = ext;
                 if (fs != 0xffffu && slot[fs].a == 0) continue;           // builder.rs:245: a zero flag skips the push
@@ -1092,6 +1088,117 @@ void launch_balance_finish(const BalanceTable& t, unsigned long long* counters, 
     size_t slots = (size_t)t.mask + 1;
     k_balance_finish<<<(unsigned)((slots + 255) / 256), 256, 0, st>>>(t, counters, out);
     COUNT_LAUNCH();
+}
+
+// =============================================================================================
+// LogUp constraint-path folds (debug/trace collect_column_oracle_folds): the lookup program of k_logup_rows folded
+// batch by batch and group by group as DebugTraceBuilder folds it, compared with an aux trace (kernels.cuh LookupFoldArgs)
+// =============================================================================================
+template <int MAXS>
+__global__ void __launch_bounds__(128) k_fold_rows(LookupFoldArgs a) {
+    size_t N = (size_t)1 << a.log_n;
+    size_t r = a.row0 + (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= a.row0 + a.n_rows) return;
+    size_t rn = (r + 1) & (N - 1);
+    size_t per_row = (r & (((size_t)1 << a.prog.log_max_period) - 1)) * a.prog.n_periodic;
+    E2 slot[MAXS];
+    E2 V[LOGUP_MAX_COLS], U[LOGUP_MAX_COLS], F[LOGUP_MAX_COLS];
+    for (u32 c = 0; c < a.n_cols; c++) { V[c] = gl::e2(0, 0); U[c] = gl::e2(1, 0); }
+    const E2 zero = gl::e2(0, 0), one = gl::e2(1, 0);
+    E2 bn = zero, bd = one, vg = zero, ug = one;   // the open batch (N, D) and the open group (V_g, U_g)
+    u64 bf = 0;                                    // the open batch's flag
+    u32 cur = 0;                                   // the open group's column
+    auto close_batch = [&]() {
+        ug = gl::e2_add(ug, gl::e2_mulf(gl::e2_sub(bd, one), bf));
+        vg = gl::e2_add(vg, gl::e2_mulf(bn, bf));
+        bn = zero; bd = one;
+    };
+    auto close_group = [&]() {
+        V[cur] = gl::e2_add(gl::e2_mul(V[cur], ug), gl::e2_mul(vg, U[cur]));
+        U[cur] = gl::e2_mul(U[cur], ug);
+        vg = zero; ug = one;
+    };
+    const uint4* code = reinterpret_cast<const uint4*>(a.prog.code);
+    for (u32 i = 0; i < a.prog.n_instr; i++) {
+        uint4 ins = code[i];
+        u32 op = ins.x & 0xff, ext = ins.x >> 8, x = ins.z, y = ins.w;
+        E2 v;
+        switch (op) {
+            LOOKUP_NODE_CASES(a, N, r, rn, per_row, slot, x, y, ext, v)
+            default: {   // 17 EMIT of interaction k = ext
+                u32 fs = x & 0xffffu, ms = x >> 16, mark = a.marks ? a.marks[ext] : 3u;
+                if (mark & 1) close_batch();
+                if (mark & 2) { close_group(); cur = ins.y; }
+                if (mark & 1) bf = fs == 0xffffu ? 1 : slot[fs].a;
+                E2 d = slot[y];
+                bn = gl::e2_add(gl::e2_mul(bn, d), gl::e2_mulf(bd, slot[ms].a));
+                bd = gl::e2_mul(bd, d);
+                continue;
+            }
+        }
+        slot[ins.y] = v;
+    }
+    close_batch();
+    close_group();
+
+    if (a.folds_out && a.folds_cm) {
+        for (u32 c = 0; c < a.n_cols; c++) {
+            u64* o = a.folds_out + (size_t)(4 * c) * N + r;
+            o[0] = V[c].a; o[N] = V[c].b; o[2 * N] = U[c].a; o[3 * N] = U[c].b;
+        }
+    } else if (a.folds_out) {
+        ulonglong2* o = reinterpret_cast<ulonglong2*>(a.folds_out) + 2 * r * a.n_cols;
+        for (u32 c = 0; c < a.n_cols; c++) { o[2 * c] = make_ulonglong2(V[c].a, V[c].b); o[2 * c + 1] = make_ulonglong2(U[c].a, U[c].b); }
+    }
+
+    // F[c] = V_c / U_c with one inversion (Montgomery's trick over the columns whose U is non-zero)
+    u32 zero_mask = 0, n_zero = 0;
+    E2 acc = one;
+    for (u32 c = 0; c < a.n_cols; c++) {
+        F[c] = acc;
+        if ((U[c].a | U[c].b) == 0) { zero_mask |= 1u << c; n_zero++; } else acc = gl::e2_mul(acc, U[c]);
+    }
+    E2 inv = gl::e2_inv(acc), total = zero;
+    for (u32 c = a.n_cols; c-- > 0;) {
+        if ((zero_mask >> c) & 1) { F[c] = zero; continue; }
+        F[c] = gl::e2_mul(V[c], gl::e2_mul(inv, F[c]));
+        inv = gl::e2_mul(inv, U[c]);
+        total = gl::e2_add(total, F[c]);
+    }
+    u32 first_c = 0xFFFFFFFFu;
+    for (u32 c = 0; c < a.n_cols; c++) {
+        E2 expected = F[c], actual = gl::e2(a.aux_cm[(size_t)(2 * c) * N + r], a.aux_cm[(size_t)(2 * c + 1) * N + r]);
+        u32 kind = 0;
+        if (c == 0) {
+            E2 next = r == N - 1 ? a.final : gl::e2(a.aux_cm[r + 1], a.aux_cm[N + r + 1]);
+            expected = total; actual = gl::e2_sub(next, actual);
+        }
+        if ((zero_mask >> c) & 1) kind = 3;
+        else if (c == 0 ? (zero_mask == 0 && !gl::e2_eq(expected, actual)) : !gl::e2_eq(expected, actual)) kind = c ? 1 : 2;
+        if (kind && first_c == 0xFFFFFFFFu) first_c = c;
+        if (a.probe && c == a.probe_col) {
+            a.probe[0] = kind;
+            a.probe[1] = V[c].a; a.probe[2] = V[c].b; a.probe[3] = U[c].a; a.probe[4] = U[c].b;
+            a.probe[5] = expected.a; a.probe[6] = expected.b; a.probe[7] = actual.a; a.probe[8] = actual.b;
+        }
+    }
+    if (first_c != 0xFFFFFFFFu) {
+        atomicMin(a.first, (unsigned long long)(((u64)r << 32) | first_c));
+        atomicAdd(a.failing_rows, 1ull);
+    }
+    if (n_zero) atomicAdd(a.zero_u, (unsigned long long)n_zero);
+}
+int launch_fold_rows(const LookupFoldArgs& a, cudaStream_t st) {
+    if (a.n_cols == 0 || a.n_cols > LOGUP_MAX_COLS) return -1;
+    if (a.n_rows == 0) return 0;
+    unsigned blocks = (unsigned)((a.n_rows + 127) / 128);
+    if (a.prog.n_slots <= 16) k_fold_rows<16><<<blocks, 128, 0, st>>>(a);
+    else if (a.prog.n_slots <= 64) k_fold_rows<64><<<blocks, 128, 0, st>>>(a);
+    else if (a.prog.n_slots <= 256) k_fold_rows<256><<<blocks, 128, 0, st>>>(a);
+    else if (a.prog.n_slots <= 1024) k_fold_rows<1024><<<blocks, 128, 0, st>>>(a);
+    else return -1;
+    COUNT_LAUNCH();
+    return 0;
 }
 
 // three-phase scan, 2048 rows per block (8 per thread): block totals -> serial scan of the (<= 2048) block

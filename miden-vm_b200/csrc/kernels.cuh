@@ -249,6 +249,37 @@ void launch_balance_boundary(const BalanceTable& t, const u64* triples, u32 n, c
 void launch_balance_finish(const BalanceTable& t, unsigned long long* counters, u64* out, cudaStream_t st);
 
 // ---------------------------------------------------------------------------------------------
+// LogUp constraint-path folds without proving (mdn_check_lookup_folds; reference air/src/lookup/debug/trace/mod.rs:191-207)
+// ---------------------------------------------------------------------------------------------
+// One thread per trace row r of [row0, row0 + n_rows) interprets the compiled lookup program and folds every aux
+// column the way DebugTraceBuilder does (debug/trace/builder.rs), all interactions taking part whatever their flag:
+//   batch  (N, D) <- (N * d + D * m, D * d) per interaction, from (0, 1)                        builder.rs:353-355
+//   group  (V_g, U_g) <- (V_g + N * flag, U_g + (D - 1) * flag) per insert / batch, from (0, 1) builder.rs:251-252,278-279
+//   column (V, U) <- (V * U_g + V_g * U, U * U_g) per group, from (0, 1)                        builder.rs:144-146
+// marks[k] of interaction k (emission order): bit 0 = it opens a new insert / batch call, bit 1 = it opens a new group
+// (then bit 0 is set as well); NULL = every interaction is a group of its own.
+// The row then (a) stores its folds, (b) divides V_c / U_c for every column with one inversion, leaving out the
+// columns whose U_c is zero, and (c) compares: column c >= 1 with aux[r][c]; column 0, when no U of the row is zero,
+// sum_c V_c / U_c with aux[r + 1][0] - aux[r][0] (`final` closes the last row).  A row with a disagreement or a zero U
+// does atomicMin(first, row << 32 | its lowest such column) and atomicAdd(failing_rows, 1); zero_u counts the zero U.
+// With probe set, the thread stores {kind, V c0, c1, U c0, c1, expected c0, c1, actual c0, c1} of column probe_col.
+struct LookupFoldArgs {
+    const u64* main_cm; u32 log_n, n_cols;   // raw main trace, column-major [col][row]; LookupAir::num_columns
+    AirDev prog;                          // lookup program; periodic = RAW periodic matrix, row-major
+    const u64* publics; const u64* challenges;
+    const u32* marks;                     // device, one word per interaction, or NULL
+    const u64* aux_cm;                    // aux trace, column-major planes [2c + coord][row]
+    E2 final;                             // the value aux[N][0] would hold
+    u64* folds_out; u32 folds_cm;         // NULL; row-major [row][column][V c0, c1, U c0, c1]; or planes [4c + word][row]
+    size_t row0, n_rows;
+    unsigned long long* first;            // init ~0
+    unsigned long long* failing_rows;     // init 0
+    unsigned long long* zero_u;           // init 0
+    u32 probe_col; u64* probe;            // 9 u64, or NULL
+};
+int launch_fold_rows(const LookupFoldArgs& a, cudaStream_t st);   // 0, or -1 when the program needs too many slots/columns
+
+// ---------------------------------------------------------------------------------------------
 // DEEP / FRI / misc
 // ---------------------------------------------------------------------------------------------
 // wvec[i] = y^(bitrev_n(p0 + i)) for i < cnt  (EF interleaved; p0 = 0, cnt = 2^n: the whole vector);

@@ -334,6 +334,8 @@ struct mdn_session {
                            mdn_aux_builder build_aux, void* aux_ctx, u32 flags, mdn_constraint_report* out);
     void check_trace_balance(const mdn_statement* st, const mdn_matrix* traces, const u64* rnd, const u64* boundary, size_t n_boundary,
                              const uint32_t* const* mutex_sites, u64 max_contrib, u32 flags, mdn_balance_report* out);
+    void check_lookup_folds(const mdn_statement* st, const mdn_matrix* traces, const u64* rnd, const uint32_t* const* fold_marks,
+                            const mdn_matrix* aux, const u64* const* aux_finals, u64* const* folds_out, u32 flags, mdn_fold_report* out);
     // the last balance report's lists (mdn_balance_report points into them)
     std::vector<mdn_unmatched> bal_unmatched;
     std::vector<mdn_balance_push> bal_contrib;
@@ -1757,6 +1759,191 @@ void mdn_session::check_trace_balance(const mdn_statement* st, const mdn_matrix*
     out->holds = n_unm == 0 && n_mutex == 0;
 }
 
+// ---------------------------------------------------------------------------------------------
+// check_lookup_folds: the constraint-path fold of every LogUp column on every row against an aux trace, without a
+// proof  (debug/trace/mod.rs:191-207, builder.rs; the comparison of processor/src/trace/tests/lookup.rs:185-265)
+// ---------------------------------------------------------------------------------------------
+// The validation, program compilation and main-trace upload of check_trace_balance; the challenges are an argument.
+// The aux traces come with the call (host row-major through the transpose, column-major device read in place) or from
+// build_logup_aux on the same traces.  k_fold_rows runs once per AIR with a lowered lookup program; a second launch on
+// the one failing row fetches its fold, expected and actual values.
+void mdn_session::check_lookup_folds(const mdn_statement* st, const mdn_matrix* traces, const u64* rnd, const uint32_t* const* fold_marks,
+                                     const mdn_matrix* aux, const u64* const* aux_finals, u64* const* folds_out, u32 flags, mdn_fold_report* out) {
+    const bool cm = column_major(flags);
+    reset_proof();
+    prof.st = stream; prof.reset();
+    if (!d_flag.p) { ArenaScope persistent(nullptr); d_flag.alloc(1, stream); CUDA_OK(cudaMemsetAsync(d_flag.p, 0, 8, stream)); }
+    if (!out) fail(MDN_ERR_INVALID_ARG, "null argument");
+    const mdn_challenger no_challenger{};   // nothing is observed: validate_statement only checks the statement
+    validate_statement(st, traces, &no_challenger);
+    if (cm) for (u32 i = 0; i < st->n_airs; i++) check_column_major(traces[i], "trace", i);
+    const bool on_device = (flags & MDN_FLAG_DEVICE_TRACES) != 0;
+    const u32 k = st->n_airs;
+    bind_airs(st, traces, false);
+    bind_order(st, false);
+
+    // arguments: challenges, aux traces and their closing values, fold marks, fold buffers
+    u32 max_rand = 0;
+    for (auto& a : airs) max_rand = std::max(max_rand, a.desc.num_randomness);
+    if (max_rand && !rnd) fail(MDN_ERR_INVALID_ARG, "randomness is NULL");
+    for (u32 i = 0; i < 2 * max_rand; i++) if (rnd[i] >= gl::P) fail(MDN_ERR_INVALID_ARG, "randomness word %u is not a canonical field element (>= p)", i);
+    if (!aux && aux_finals) fail(MDN_ERR_INVALID_ARG, "aux_finals given without aux: the device LogUp build supplies its own closing values");
+    u32 skipped = 0;
+    size_t staging_words = 0;
+    for (u32 i = 0; i < k; i++) {
+        const uint32_t* marks = fold_marks ? fold_marks[i] : nullptr;
+        if (!airs[i].has_lookup) {
+            skipped++;
+            if (marks) fail(MDN_ERR_INVALID_ARG, "AIR %u: fold marks given for an AIR without a lookup program", i);
+            if (folds_out && folds_out[i]) fail(MDN_ERR_INVALID_ARG, "AIR %u: a fold buffer given for an AIR without a lookup program", i);
+            continue;
+        }
+        const u32 C = airs[i].desc.aux_width;
+        if (aux) {
+            if (aux[i].width != 2 * C || aux[i].log_height != log_heights[i]) fail(MDN_ERR_INVALID_ARG, "AIR %u: the aux trace must be 2^%u rows of %u base columns", i, log_heights[i], 2 * C);
+            if (!aux[i].values) fail(MDN_ERR_INVALID_ARG, "aux trace %u is NULL", i);
+            if (cm) check_column_major(aux[i], "aux trace", i);
+            if (!aux_finals || !aux_finals[i]) fail(MDN_ERR_INVALID_ARG, "AIR %u: aux_finals is NULL", i);
+            if (aux_finals[i][0] >= gl::P || aux_finals[i][1] >= gl::P) fail(MDN_ERR_INVALID_ARG, "AIR %u: aux_finals is not a canonical field element (>= p)", i);
+        }
+        if (folds_out && folds_out[i]) {
+            if (on_device && ((uintptr_t)folds_out[i] & 15)) fail(MDN_ERR_INVALID_ARG, "AIR %u: a device fold buffer must be 16-byte aligned", i);
+            if (!on_device) staging_words = std::max(staging_words, ((size_t)4 * C) << log_heights[i]);
+        }
+        if (!marks) continue;
+        const u32* w = st->airs[i].lookup->program;
+        const u32 nn = w[2], nc = w[3];
+        const u32* items = w + 5 + 3 * (size_t)nn;   // {column, flag, multiplicity, denominator}
+        for (u32 q = 0; q < nc; q++) {
+            const u32 m = marks[q];
+            if (m != 0 && m != 1 && m != 3) fail(MDN_ERR_INVALID_ARG, "AIR %u: fold mark %u of interaction %u (0, 1 or 3)", i, m, q);
+            if (m != 3 && (q == 0 || items[4 * (size_t)q] != items[4 * (size_t)(q - 1)]))
+                fail(MDN_ERR_INVALID_ARG, "AIR %u: interaction %u starts a column and must open a group (fold mark 3)", i, q);
+            if (m == 0 && items[4 * (size_t)q + 1] != items[4 * (size_t)(q - 1) + 1])
+                fail(MDN_ERR_INVALID_ARG, "AIR %u: interactions %u and %u are marked as one batch but do not share a flag node", i, q - 1, q);
+        }
+    }
+
+    // raw main traces of the lookup AIRs, column-major (column-major device traces are read where the caller keeps them)
+    std::vector<const u64*> main_cm(k, nullptr);
+    std::vector<u64*> aux_cm(k, nullptr);
+    size_t main_total = 0, aux_total = 0;
+    for (u32 i = 0; i < k; i++) if (airs[i].has_lookup) {
+        size_t N = (size_t)1 << log_heights[i];
+        if (!cm) main_total += N * airs[i].desc.width;
+        if (!(aux && cm)) aux_total += N * 2 * airs[i].desc.aux_width;
+    }
+    if (main_total) main_c.coef_buf.alloc(main_total, stream);
+    if (aux_total) aux_c.coef_buf.alloc(aux_total, stream);
+    size_t co = 0, ao = 0;
+    for (u32 i = 0; i < k; i++) {
+        if (!airs[i].has_lookup) continue;
+        size_t N = (size_t)1 << log_heights[i];
+        u64* dst = cm ? const_cast<u64*>(traces[i].values) : main_c.coef_buf.p + co;
+        if (!cm) co += N * airs[i].desc.width;
+        upload_matrix(traces[i], on_device, dst, cm);   // column-major: check only
+        main_cm[i] = dst;
+        if (aux && cm) aux_cm[i] = const_cast<u64*>(aux[i].values);
+        else { aux_cm[i] = aux_c.coef_buf.p + ao; ao += N * 2 * airs[i].desc.aux_width; }
+    }
+    check_input_flag("a main trace");
+    if (aux) {
+        for (u32 i = 0; i < k; i++) if (airs[i].has_lookup) upload_matrix(aux[i], on_device, aux_cm[i], cm);
+        check_input_flag("an aux trace");
+    }
+    d_publics.alloc(std::max<size_t>(1, publics.size()), stream);
+    if (!publics.empty()) CUDA_OK(cudaMemcpyAsync(d_publics.p, publics.data(), publics.size() * sizeof(u64), cudaMemcpyHostToDevice, stream));
+    d_randomness.alloc(std::max<size_t>(1, 2 * (size_t)max_rand), stream);
+    if (max_rand) CUDA_OK(cudaMemcpyAsync(d_randomness.p, rnd, 2 * (size_t)max_rand * sizeof(u64), cudaMemcpyHostToDevice, stream));
+    std::vector<DevBuf> d_marks(k);
+    for (u32 i = 0; i < k; i++) {
+        if (!airs[i].has_lookup || !fold_marks || !fold_marks[i]) continue;
+        const u32 nc = st->airs[i].lookup->program[3];
+        if (!nc) continue;
+        d_marks[i].alloc(((size_t)nc + 1) / 2, stream);
+        CUDA_OK(cudaMemcpyAsync(d_marks[i].p, fold_marks[i], nc * sizeof(u32), cudaMemcpyHostToDevice, stream));
+    }
+    // the prover path to check when no aux trace is given: k_logup_rows + the scan, as mdn_prove builds it
+    std::vector<E2> finals(k, gl::e2(0, 0));
+    std::vector<u32> pos(k);
+    for (u32 j = 0; j < k; j++) pos[order[j]] = j;
+    for (u32 i = 0; i < k; i++) {
+        if (!airs[i].has_lookup) continue;
+        if (aux) { finals[i] = gl::e2(aux_finals[i][0], aux_finals[i][1]); continue; }
+        u64 fin[2] = {0, 0};
+        build_logup_aux(pos[i], main_cm[i], aux_cm[i], fin);
+        finals[i] = gl::e2(fin[0], fin[1]);
+    }
+    // host fold buffers are filled through one device staging buffer, sized for the largest of them
+    DevBuf staging;
+    if (staging_words) {
+        auto too_large = [&](const char* what) {
+            fail(MDN_ERR_UNSUPPORTED, "the folds of the largest AIR need %.1f GiB of device memory: %s", staging_words * sizeof(u64) / 1073741824.0, what);
+        };
+#ifndef MDN_EMULATED   // tests/emu has no device memory of its own: only the failed allocation below is reported there
+        size_t arena_b = 0, free_b = 0, total_b = 0;
+        for (auto& sl : arena.slabs) arena_b += sl.size - sl.used;
+        CUDA_OK(cudaMemGetInfo(&free_b, &total_b));
+        char msg[64];
+        snprintf(msg, sizeof msg, "%.1f GiB are free", (free_b + arena_b) / 1073741824.0);
+        if (staging_words * sizeof(u64) > free_b + arena_b) too_large(msg);
+#endif
+        try { staging.alloc(staging_words, stream); }
+        catch (const MdnError&) { cudaGetLastError(); too_large("the allocation failed"); }
+    }
+
+    // per AIR: {first (row << 32 | column), failing rows, zero U}; then the probe's 9 words and its scratch counters
+    DevBuf res; res.alloc(3 * (size_t)k + 12, stream);
+    std::vector<u64> host_res(3 * (size_t)k + 12, 0);
+    for (u32 i = 0; i < k; i++) host_res[3 * i] = ~0ull;
+    host_res[3 * (size_t)k + 9] = ~0ull;
+    CUDA_OK(cudaMemcpyAsync(res.p, host_res.data(), host_res.size() * sizeof(u64), cudaMemcpyHostToDevice, stream));
+    std::vector<mk::LookupFoldArgs> fa(k);
+    for (u32 i = 0; i < k; i++) {
+        if (!airs[i].has_lookup) continue;
+        mk::LookupFoldArgs& f = fa[i];
+        f = mk::LookupFoldArgs{};
+        f.main_cm = main_cm[i]; f.log_n = log_heights[i]; f.n_cols = airs[i].desc.aux_width; f.prog = airs[i].lookup_dev;
+        f.publics = d_publics.p; f.challenges = d_randomness.p; f.marks = (const u32*)d_marks[i].p;
+        f.aux_cm = aux_cm[i]; f.final = finals[i];
+        u64* user = folds_out ? folds_out[i] : nullptr;
+        f.folds_out = user && !on_device ? staging.p : user; f.folds_cm = cm;
+        f.row0 = 0; f.n_rows = (size_t)1 << log_heights[i];
+        f.first = (unsigned long long*)(res.p + 3 * i); f.failing_rows = f.first + 1; f.zero_u = f.first + 2;
+        if (mk::launch_fold_rows(f, stream) != 0) fail(MDN_ERR_UNSUPPORTED, "AIR %u: lookup program too large for the interpreter", i);
+        if (user && !on_device) {
+            CUDA_OK(cudaMemcpyAsync(user, staging.p, (((size_t)4 * f.n_cols) << f.log_n) * sizeof(u64), cudaMemcpyDeviceToHost, stream));
+            CUDA_OK(cudaStreamSynchronize(stream));   // the staging buffer serves the next AIR
+            f.folds_out = nullptr;
+        }
+    }
+    CUDA_OK(cudaMemcpyAsync(host_res.data(), res.p, 3 * (size_t)k * sizeof(u64), cudaMemcpyDeviceToHost, stream));
+    CUDA_OK(cudaStreamSynchronize(stream));
+    CUDA_OK(cudaGetLastError());
+
+    memset(out, 0, sizeof *out);
+    out->n_skipped_airs = skipped;
+    for (u32 i = 0; i < k; i++) { out->failing_rows += host_res[3 * i + 1]; out->zero_u += host_res[3 * i + 2]; }
+    for (u32 i = 0; i < k; i++) {
+        u64 first = host_res[3 * i];
+        if (!airs[i].has_lookup || first == ~0ull) continue;
+        out->instance = i; out->row = first >> 32; out->column = (u32)first;
+        // the values: the same kernel on that one row, recording that column (its own atomics go to scratch words)
+        mk::LookupFoldArgs f = fa[i];
+        u64* probe = res.p + 3 * (size_t)k;
+        f.folds_out = nullptr; f.row0 = out->row; f.n_rows = 1; f.probe_col = out->column; f.probe = probe;
+        f.first = (unsigned long long*)(probe + 9); f.failing_rows = f.first + 1; f.zero_u = f.first + 2;
+        if (mk::launch_fold_rows(f, stream) != 0) fail(MDN_ERR_UNSUPPORTED, "AIR %u: lookup program too large for the interpreter", i);
+        u64 pv[9];
+        CUDA_OK(cudaMemcpyAsync(pv, probe, sizeof pv, cudaMemcpyDeviceToHost, stream));
+        CUDA_OK(cudaStreamSynchronize(stream));
+        out->kind = (u32)pv[0];
+        memcpy(out->fold, pv + 1, 4 * sizeof(u64)); memcpy(out->expected, pv + 5, 2 * sizeof(u64)); memcpy(out->actual, pv + 7, 2 * sizeof(u64));
+        break;
+    }
+    out->holds = out->failing_rows == 0;
+}
+
 // mdn_aux_builder_device for instance `inst`: the aux columns go straight into `aux_slot` (column-major, on the session's
 // stream), the aux values into `values`
 void mdn_session::call_device_aux_builder(u32 inst, const mdn_matrix& main, u64* aux_slot, std::vector<u64>& values) {
@@ -2583,6 +2770,23 @@ int mdn_check_trace_balance(mdn_session* s, const mdn_statement* st, const mdn_m
         ArenaScope proof_memory(s->use_arena ? &s->arena : nullptr);
         CUDA_OK(cudaSetDevice(s->device));
         s->check_trace_balance(st, traces, randomness, boundary, n_boundary, mutex_sites, max_contributions, flags, out);
+    }
+    s->reset_proof();
+    API_CATCH(s)
+}
+
+int mdn_check_lookup_folds(mdn_session* s, const mdn_statement* st, const mdn_matrix* traces, const uint64_t* randomness,
+                           const uint32_t* const* fold_marks, const mdn_matrix* aux, const uint64_t* const* aux_finals,
+                           uint64_t* const* folds_out, uint32_t flags, mdn_fold_report* out) {
+    if (!s) return MDN_ERR_INVALID_ARG;
+    // refused before any device work, so that a staged proof in progress stays intact
+    if (s->in_proof) { s->error = "mdn_check_lookup_folds called inside a proof (between mdn_prove_begin and mdn_prove_finish)"; return MDN_ERR_INVALID_ARG; }
+    if (s->shard_world > 1) { s->error = "mdn_check_lookup_folds does not run on a session split over ranks (mdn_session_set_shard world > 1)"; return MDN_ERR_UNSUPPORTED; }
+    API_TRY(s)
+    {
+        ArenaScope proof_memory(s->use_arena ? &s->arena : nullptr);
+        CUDA_OK(cudaSetDevice(s->device));
+        s->check_lookup_folds(st, traces, randomness, fold_marks, aux, aux_finals, folds_out, flags, out);
     }
     s->reset_proof();
     API_CATCH(s)

@@ -17,6 +17,7 @@
 //   debug::check_constraints(&prover_statement, challenger)       miden::check_constraints(config, statement, challenger)
 //     (debug.rs:70-214; panics -> ConstraintViolation)             (every constraint on every row, on the device, no proof)
 //   lookup::debug::check_trace_balance(air, main, .., challenges)  miden::check_trace_balance(config, statement, challenges, ..)
+//   lookup::debug::collect_column_oracle_folds(air, main, ..)      miden::check_lookup_folds(config, statement, challenges, ..)
 //     (air/src/lookup/debug/trace/mod.rs:169-309) -> BalanceReport  -> miden::BalanceReport (to_string() = its Display)
 //   ProverError::{Instance, Domain, ..}  prover/mod.rs:582-596    miden::ProverError { kind, what() }
 //   HashFunction::{Blake3_256, Keccak, Rpo256, Poseidon2, Rpx256} -> the config constructor (prover/src/lib.rs:245-301)
@@ -425,6 +426,59 @@ inline BalanceReport check_trace_balance(const StarkConfig& config, const Prover
         const mdn_mutex_violation& m = r.mutex_violations[j];
         out.mutex_violations.push_back({m.instance, m.row, m.column, m.group, m.active_flags});
     }
+    return out;
+}
+
+// collect_column_oracle_folds(air, main_trace, .., challenges) (air/src/lookup/debug/trace/mod.rs:196-207) on the device,
+// compared with an aux trace as assert_prover_matches_oracle compares them (processor/src/trace/tests/lookup.rs:185-265).
+// `fold_marks` = per AIR, empty or one word per interaction (include/miden_b200.h); `aux` = empty to check the device
+// LogUp build of the same traces, else per AIR the aux trace (host row-major, base-flattened) with its closing value in
+// `aux_finals`; `folds` = NULL, or filled per AIR with rows x num_columns (V, U) pairs.  Throws ProverError on malformed input only.
+struct FoldReport {
+    bool holds = true;
+    uint32_t kind = 0, instance = 0, column = 0;      // kind: 1 fraction column, 2 accumulator, 3 zero U
+    uint64_t row = 0;
+    QuadFelt v{}, u{}, expected{}, actual{};
+    uint64_t failing_rows = 0, zero_u = 0;
+    uint32_t n_skipped_airs = 0;
+};
+inline FoldReport check_lookup_folds(const StarkConfig& config, const ProverStatement& ps, const std::vector<QuadFelt>& challenges,
+                                     const std::vector<std::vector<uint32_t>>& fold_marks = {}, const std::vector<RowMajorMatrix>& aux = {},
+                                     const std::vector<QuadFelt>& aux_finals = {},
+                                     std::vector<std::vector<std::pair<QuadFelt, QuadFelt>>>* folds = nullptr) {
+    detail::Lowered low(ps.statement);
+    const size_t k = ps.statement.airs.size();
+    std::vector<mdn_matrix> mats, aux_mats;
+    for (const RowMajorMatrix& t : ps.traces) mats.push_back(t.raw());
+    for (const RowMajorMatrix& t : aux) aux_mats.push_back(t.raw());
+    std::vector<Felt> rnd;
+    for (const QuadFelt& c : challenges) { rnd.push_back(c[0]); rnd.push_back(c[1]); }
+    std::vector<const uint32_t*> marks(k, nullptr);
+    for (size_t i = 0; i < fold_marks.size() && i < k; i++) if (!fold_marks[i].empty()) marks[i] = fold_marks[i].data();
+    std::vector<std::array<uint64_t, 2>> fin(k);
+    std::vector<const uint64_t*> fin_p(k, nullptr);
+    for (size_t i = 0; i < aux_finals.size() && i < k; i++) { fin[i] = {aux_finals[i][0], aux_finals[i][1]}; fin_p[i] = fin[i].data(); }
+    std::vector<std::vector<uint64_t>> bufs(k);
+    std::vector<uint64_t*> buf_p(k, nullptr);
+    if (folds) for (size_t i = 0; i < k; i++) if (low.st.airs[i].lookup) {
+        bufs[i].assign((size_t(4) * low.st.airs[i].aux_width) << mats[i].log_height, 0);
+        buf_p[i] = bufs[i].data();
+    }
+    mdn_fold_report r{};
+    detail::check(config, mdn_check_lookup_folds(config.session(), &low.st, mats.data(), rnd.empty() ? nullptr : rnd.data(),
+                                                  fold_marks.empty() ? nullptr : marks.data(), aux.empty() ? nullptr : aux_mats.data(),
+                                                  aux.empty() ? nullptr : fin_p.data(), folds ? buf_p.data() : nullptr, 0, &r));
+    if (folds) {
+        folds->assign(k, {});
+        for (size_t i = 0; i < k; i++)
+            for (size_t e = 0; e + 3 < bufs[i].size(); e += 4)
+                (*folds)[i].push_back({QuadFelt{bufs[i][e], bufs[i][e + 1]}, QuadFelt{bufs[i][e + 2], bufs[i][e + 3]}});
+    }
+    FoldReport out;
+    out.holds = r.holds != 0; out.kind = r.kind; out.instance = r.instance; out.column = r.column; out.row = r.row;
+    out.v = {r.fold[0], r.fold[1]}; out.u = {r.fold[2], r.fold[3]};
+    out.expected = {r.expected[0], r.expected[1]}; out.actual = {r.actual[0], r.actual[1]};
+    out.failing_rows = r.failing_rows; out.zero_u = r.zero_u; out.n_skipped_airs = r.n_skipped_airs;
     return out;
 }
 
