@@ -333,6 +333,45 @@ int mdn_check_constraints(mdn_session* s, const mdn_statement* st, const mdn_mat
                           uint32_t flags, uint64_t* randomness_out /* 2*max num_randomness, may be NULL */,
                           mdn_constraint_report* out);
 
+/* ---- list every violated constraint, without proving: the census of mdn_check_constraints ----------------------
+ * The same inputs, challenges, aux traces, external check, trace layouts and refusals as mdn_check_constraints; the row
+ * pass keeps every (instance, row, constraint) whose value is non-zero instead of stopping at the first.
+ *   failures : host, room for max_failures (NULL iff max_failures == 0): the first max_failures violations in
+ *              (instance, row, constraint) order, instance order as in mdn_check_constraints -- the failures the
+ *              reference would panic on one after another if each were fixed in turn.
+ *   tallies  : host, room for max_tallies (NULL iff max_tallies == 0): each (instance, constraint) that is non-zero on
+ *              at least one row, in (instance, constraint) order, truncated to max_tallies.
+ *   out      : the counts; out->first is field for field the report mdn_check_constraints gives for the same call
+ *              (its least failure and value come from the tallies; a failing external assertion takes precedence).
+ * A NULL list with a non-zero capacity, or a NULL out, is MDN_ERR_INVALID_ARG before any device work.  The outputs do
+ * not depend on the order in which device atomics ran: two calls on the same inputs give byte-identical outputs.
+ * Refused, as mdn_check_constraints, inside a staged proof and on a session split over ranks; uses and releases the
+ * proof arena; leaves mdn_get_info, mdn_get_timings and later proofs unchanged. */
+typedef struct {                 /* one violation: constraint `constraint` of instance `instance` is non-zero at `row` */
+    uint32_t instance, constraint;
+    uint64_t row;
+    uint64_t value[2];           /* EF (c0, c1); c1 = 0 for base constraints */
+} mdn_constraint_failure;        /* 32 bytes */
+typedef struct {                 /* one (instance, constraint) that is non-zero on at least one row */
+    uint32_t instance, constraint;
+    uint64_t failing_rows;       /* rows where it is non-zero */
+    uint64_t first_row, last_row;
+    uint64_t first_value[2];     /* its value at first_row */
+} mdn_constraint_tally;          /* 48 bytes */
+typedef struct mdn_constraint_census {   /* the typedef cannot share the function's name in C */
+    mdn_constraint_report first; /* field for field what mdn_check_constraints returns for the same call */
+    uint64_t violations;         /* (instance, row, constraint) triples that are non-zero */
+    uint64_t n_failures;         /* written to failures[] = min(violations, max_failures) */
+    uint64_t failing_constraints;/* (instance, constraint) pairs with failing_rows > 0 */
+    uint64_t n_tallies;          /* written to tallies[] = min(failing_constraints, max_tallies) */
+} mdn_constraint_census_report;
+int mdn_constraint_census(mdn_session* s, const mdn_statement* st, const mdn_matrix* traces,
+                          const mdn_matrix* preprocessed, const mdn_challenger* challenger,
+                          mdn_aux_builder build_aux, void* aux_ctx, uint32_t flags, uint64_t* randomness_out,
+                          mdn_constraint_failure* failures, uint64_t max_failures,
+                          mdn_constraint_tally* tallies, uint64_t max_tallies,
+                          mdn_constraint_census_report* out);
+
 /* ---- find unbalanced LogUp bus messages, without proving: check_trace_balance ----------------------------------
  * (air/src/lookup/debug/trace/mod.rs:169-309, builder.rs:201-375).  Walks every row of every AIR of the statement that
  * carries a lowered mdn_air.lookup, keys every active push by its encoded denominator and sums the multiplicities

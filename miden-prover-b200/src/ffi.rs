@@ -233,6 +233,39 @@ pub struct MdnBalanceReport {
     pub n_mutex_listed: u64,
 }
 
+/// `mdn_constraint_failure`: constraint `constraint` of instance `instance` is non-zero at `row`.
+#[repr(C)]
+#[derive(Clone, Copy, Debug, Default)]
+pub struct MdnConstraintFailure {
+    pub instance: u32,
+    pub constraint: u32,
+    pub row: u64,
+    pub value: [u64; 2],
+}
+
+/// `mdn_constraint_tally`: one (instance, constraint) that is non-zero on at least one row.
+#[repr(C)]
+#[derive(Clone, Copy, Debug, Default)]
+pub struct MdnConstraintTally {
+    pub instance: u32,
+    pub constraint: u32,
+    pub failing_rows: u64,
+    pub first_row: u64,
+    pub last_row: u64,
+    pub first_value: [u64; 2],
+}
+
+/// `mdn_constraint_census_report`: the counts of `mdn_constraint_census`; `first` is what `mdn_check_constraints` reports.
+#[repr(C)]
+#[derive(Clone, Copy, Debug, Default)]
+pub struct MdnConstraintCensus {
+    pub first: MdnConstraintReport,
+    pub violations: u64,
+    pub n_failures: u64,
+    pub failing_constraints: u64,
+    pub n_tallies: u64,
+}
+
 /// `mdn_fold_report`: the outcome of `mdn_check_lookup_folds` (kind 1 fraction column, 2 accumulator, 3 zero U).
 #[repr(C)]
 #[derive(Clone, Copy, Debug, Default)]
@@ -316,6 +349,23 @@ unsafe extern "C" {
         flags: u32,
         randomness_out: *mut u64,
         out: *mut MdnConstraintReport,
+    ) -> c_int;
+    /// Declared only; like the rest of the crate, not compiled yet.
+    pub fn mdn_constraint_census(
+        s: *mut MdnSession,
+        st: *const MdnStatement,
+        traces: *const MdnMatrix,
+        preprocessed: *const MdnMatrix,
+        challenger: *const MdnChallenger,
+        build_aux: MdnAuxBuilder,
+        aux_ctx: *mut c_void,
+        flags: u32,
+        randomness_out: *mut u64,
+        failures: *mut MdnConstraintFailure,
+        max_failures: u64,
+        tallies: *mut MdnConstraintTally,
+        max_tallies: u64,
+        out: *mut MdnConstraintCensus,
     ) -> c_int;
     pub fn mdn_check_trace_balance(
         s: *mut MdnSession,

@@ -73,6 +73,23 @@ class ConstraintReport(C.Structure):
                 ("row", C.c_uint64), ("value", C.c_uint64 * 2), ("failing_rows", C.c_uint64)]
 
 
+class ConstraintFailure(C.Structure):
+    """`mdn_constraint_failure`: constraint `constraint` of instance `instance` is non-zero at `row`."""
+    _fields_ = [("instance", C.c_uint32), ("constraint", C.c_uint32), ("row", C.c_uint64), ("value", C.c_uint64 * 2)]
+
+
+class ConstraintTally(C.Structure):
+    """`mdn_constraint_tally`: one (instance, constraint) that is non-zero on at least one row."""
+    _fields_ = [("instance", C.c_uint32), ("constraint", C.c_uint32), ("failing_rows", C.c_uint64), ("first_row", C.c_uint64),
+                ("last_row", C.c_uint64), ("first_value", C.c_uint64 * 2)]
+
+
+class ConstraintCensus(C.Structure):
+    """`mdn_constraint_census`: the counts of mdn_constraint_census; `first` is mdn_check_constraints' report."""
+    _fields_ = [("first", ConstraintReport), ("violations", C.c_uint64), ("n_failures", C.c_uint64),
+                ("failing_constraints", C.c_uint64), ("n_tallies", C.c_uint64)]
+
+
 class Unmatched(C.Structure):
     """`mdn_unmatched`: a denominator whose multiplicities do not sum to zero, with its least push."""
     _fields_ = [("denom", C.c_uint64 * 2), ("net_multiplicity", C.c_uint64), ("n_pushes", C.c_uint64), ("first_row", C.c_uint64),
@@ -146,7 +163,7 @@ EXPORTS = [
     "mdn_session_set_preprocessed", "mdn_session_set_jit", "mdn_jit_compile_check", "mdn_jit_status", "mdn_abi_layout",
     "mdn_session_set_external_check", "mdn_session_set_hash", "mdn_session_set_hash_challenger",
     "mdn_check_constraints", "mdn_session_set_device_aux_builder", "mdn_check_trace_balance",
-    "mdn_check_lookup_folds",
+    "mdn_check_lookup_folds", "mdn_constraint_census",
 ]
 
 _lib = None
@@ -187,6 +204,10 @@ def lib():
         L.mdn_check_constraints.argtypes = [C.c_void_p, C.POINTER(Statement), C.POINTER(Matrix), C.POINTER(Matrix),
                                             C.POINTER(Challenger), AUX_BUILDER, C.c_void_p, C.c_uint32, u64p,
                                             C.POINTER(ConstraintReport)]
+        L.mdn_constraint_census.argtypes = [C.c_void_p, C.POINTER(Statement), C.POINTER(Matrix), C.POINTER(Matrix),
+                                            C.POINTER(Challenger), AUX_BUILDER, C.c_void_p, C.c_uint32, u64p,
+                                            C.POINTER(ConstraintFailure), C.c_uint64, C.POINTER(ConstraintTally), C.c_uint64,
+                                            C.POINTER(ConstraintCensus)]
         L.mdn_check_trace_balance.argtypes = [C.c_void_p, C.POINTER(Statement), C.POINTER(Matrix), u64p, u64p, C.c_size_t,
                                               C.POINTER(u32p), C.c_uint64, C.c_uint32, C.POINTER(BalanceReport)]
         L.mdn_check_lookup_folds.argtypes = [C.c_void_p, C.POINTER(Statement), C.POINTER(Matrix), u64p, C.POINTER(u32p),
@@ -357,6 +378,24 @@ class Session:
                                                 C.byref(challenger) if challenger is not None else None, cb, None, flags,
                                                 ptr(rnd), C.byref(rep)))
         return rep, rnd[: 2 * n_rand]
+
+    def constraint_census(self, statement: Statement, traces, challenger: Challenger, aux_builder=None, preprocessed=None,
+                          flags=0, max_failures: int = 1 << 16, max_tallies: int = 1 << 16):
+        """check_constraints without stopping at the first failure: every (instance, row, constraint) that is non-zero.
+        Returns (ConstraintCensus, failures, tallies, randomness u64[2 * max num_randomness]), with `failures` the
+        first min(violations, max_failures) ConstraintFailure in (instance, row, constraint) order and `tallies` the
+        first min(failing_constraints, max_tallies) ConstraintTally in (instance, constraint) order."""
+        out = ConstraintCensus()
+        n_rand = max((statement.airs[i].num_randomness for i in range(statement.n_airs)), default=0)
+        rnd = np.zeros(max(1, 2 * n_rand), dtype=np.uint64)
+        fails = (ConstraintFailure * max(1, max_failures))()
+        tallies = (ConstraintTally * max(1, max_tallies))()
+        cb = aux_builder if aux_builder is not None else C.cast(None, AUX_BUILDER)
+        self._check(lib().mdn_constraint_census(self._h, C.byref(statement), traces, preprocessed,
+                                                C.byref(challenger) if challenger is not None else None, cb, None, flags,
+                                                ptr(rnd), fails if max_failures else None, max_failures,
+                                                tallies if max_tallies else None, max_tallies, C.byref(out)))
+        return out, list(fails[: out.n_failures]), list(tallies[: out.n_tallies]), rnd[: 2 * n_rand]
 
     def check_trace_balance(self, statement: Statement, traces, randomness, boundary=(), mutex_sites=None,
                             max_contributions: int = 1 << 16, flags=0) -> dict:

@@ -886,6 +886,27 @@ int launch_logup_rows(const LogupArgs& a, cudaStream_t st) {
 // Constraint check on the trace domain (debug.rs check_constraints): the constraint program of k_constraints, read
 // on raw rows with exact 0/1 selectors; FOLD k tests constraint k instead of folding it
 // =============================================================================================
+// one instruction of a compiled constraint program that is not a FOLD, at trace row r (rn = the next row, wrapping).
+// Shared by the kernels that check constraint programs on the trace domain (k_check_rows, k_census_rows, k_census_list).
+#define CHECK_NODE_CASES(a, N, r, rn, per_row, slot, x, y, ext, v, is_first, is_last, is_trans)                         \
+    case 0: v = gl::e2((a).main_cm[(size_t)(y) * (N) + ((x) ? (rn) : (r))], 0); break;                                  \
+    case 1: { size_t p_ = (x) ? (rn) : (r);                                                                             \
+              v = gl::e2((a).aux_cm[(size_t)(2 * (y)) * (N) + p_], (a).aux_cm[(size_t)(2 * (y) + 1) * (N) + p_]); break; } \
+    case 2: v = gl::e2((a).publics[x], 0); break;                                                                       \
+    case 3: v = gl::e2((a).challenges[2 * (x)], (a).challenges[2 * (x) + 1]); break;                                    \
+    case 4: v = gl::e2((a).aux_values[2 * (x)], (a).aux_values[2 * (x) + 1]); break;                                    \
+    case 5: v = is_first; break;                                                                                        \
+    case 6: v = is_last; break;                                                                                         \
+    case 7: v = is_trans; break;                                                                                        \
+    case 8: v = gl::e2((a).prog.consts[x], 0); break;                                                                   \
+    case 9: v = gl::e2((a).prog.consts[x], (a).prog.consts[(x) + 1]); break;                                            \
+    case 10: v = (ext) ? gl::e2_add(slot[x], slot[y]) : gl::e2(gl::add(slot[x].a, slot[y].a), 0); break;                \
+    case 11: v = (ext) ? gl::e2_sub(slot[x], slot[y]) : gl::e2(gl::sub(slot[x].a, slot[y].a), 0); break;                \
+    case 12: v = (ext) ? gl::e2_mul(slot[x], slot[y]) : gl::e2(gl::mul(slot[x].a, slot[y].a), 0); break;                \
+    case 13: v = (ext) ? gl::e2_neg(slot[x]) : gl::e2(gl::neg(slot[x].a), 0); break;                                    \
+    case 14: v = gl::e2((a).prog.periodic[(per_row) + (x)], 0); break;                                                  \
+    case 16: v = gl::e2((a).prep_cm[(size_t)(y) * (N) + ((x) ? (rn) : (r))], 0); break;
+
 template <int MAXS>
 __global__ void __launch_bounds__(128) k_check_rows(CheckArgs a) {
     size_t N = (size_t)1 << a.log_n;
@@ -902,22 +923,7 @@ __global__ void __launch_bounds__(128) k_check_rows(CheckArgs a) {
         u32 op = ins.x & 0xff, ext = ins.x >> 8, x = ins.z, y = ins.w;
         E2 v;
         switch (op) {
-            case 0: v = gl::e2(a.main_cm[(size_t)y * N + (x ? rn : r)], 0); break;
-            case 1: { size_t p = x ? rn : r; v = gl::e2(a.aux_cm[(size_t)(2 * y) * N + p], a.aux_cm[(size_t)(2 * y + 1) * N + p]); break; }
-            case 2: v = gl::e2(a.publics[x], 0); break;
-            case 3: v = gl::e2(a.challenges[2 * x], a.challenges[2 * x + 1]); break;
-            case 4: v = gl::e2(a.aux_values[2 * x], a.aux_values[2 * x + 1]); break;
-            case 5: v = is_first; break;
-            case 6: v = is_last; break;
-            case 7: v = is_trans; break;
-            case 8: v = gl::e2(a.prog.consts[x], 0); break;
-            case 9: v = gl::e2(a.prog.consts[x], a.prog.consts[x + 1]); break;
-            case 10: v = ext ? gl::e2_add(slot[x], slot[y]) : gl::e2(gl::add(slot[x].a, slot[y].a), 0); break;
-            case 11: v = ext ? gl::e2_sub(slot[x], slot[y]) : gl::e2(gl::sub(slot[x].a, slot[y].a), 0); break;
-            case 12: v = ext ? gl::e2_mul(slot[x], slot[y]) : gl::e2(gl::mul(slot[x].a, slot[y].a), 0); break;
-            case 13: v = ext ? gl::e2_neg(slot[x]) : gl::e2(gl::neg(slot[x].a), 0); break;
-            case 14: v = gl::e2(a.prog.periodic[per_row + x], 0); break;
-            case 16: v = gl::e2(a.prep_cm[(size_t)y * N + (x ? rn : r)], 0); break;
+            CHECK_NODE_CASES(a, N, r, rn, per_row, slot, x, y, ext, v, is_first, is_last, is_trans)
             default: {   // 15: the compiler places the k-th FOLD for constraint k (emission order)
                 E2 c = slot[x];
                 if (a.probe_value && k == a.probe_k) { a.probe_value[0] = c.a; a.probe_value[1] = c.b; }
@@ -940,6 +946,145 @@ int launch_check_rows(const CheckArgs& a, cudaStream_t st) {
     else if (a.prog.n_slots <= 64) k_check_rows<64><<<blocks, 128, 0, st>>>(a);
     else if (a.prog.n_slots <= 256) k_check_rows<256><<<blocks, 128, 0, st>>>(a);
     else if (a.prog.n_slots <= 1024) k_check_rows<1024><<<blocks, 128, 0, st>>>(a);
+    else return -1;
+    COUNT_LAUNCH();
+    return 0;
+}
+
+// =============================================================================================
+// Constraint census (every violation, not only the first): the program of k_check_rows counted per row and tallied
+// per constraint, then listed in (row, constraint) order from an exclusive scan of the per-row counts (kernels.cuh CensusArgs)
+// =============================================================================================
+#ifdef MDN_EMULATED
+// tests/emu runs every fiber on one OS thread, so a plain read-modify-write is atomic there
+template <class T> static inline T census_max(T* p, T v) { T o = *p; if (v > o) *p = v; return o; }
+#else
+template <class T> __device__ __forceinline__ T census_max(T* p, T v) { return atomicMax(p, v); }
+#endif
+template <int MAXS>
+__global__ void __launch_bounds__(128) k_census_rows(CensusArgs a) {
+    // per-block tally of each constraint: failing rows, least and greatest row (rows fit 32 bits: log_n <= 24)
+    __shared__ u32 s_cnt[CENSUS_SHARED_K], s_min[CENSUS_SHARED_K], s_max[CENSUS_SHARED_K];
+    __shared__ u32 s_rows;
+    const bool shared_tally = a.n_cons <= CENSUS_SHARED_K;
+    if (shared_tally) for (u32 k = threadIdx.x; k < a.n_cons; k += blockDim.x) { s_cnt[k] = 0; s_min[k] = 0xFFFFFFFFu; s_max[k] = 0; }
+    if (threadIdx.x == 0) s_rows = 0;
+    __syncthreads();
+    size_t N = (size_t)1 << a.log_n;
+    size_t r = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (r < N) {
+        size_t rn = (r + 1) & (N - 1);
+        E2 is_first = gl::e2(r == 0, 0), is_last = gl::e2(r == N - 1, 0), is_trans = gl::e2(r != N - 1, 0);
+        size_t per_row = (r & (((size_t)1 << a.prog.log_max_period) - 1)) * a.prog.n_periodic;
+        E2 slot[MAXS];
+        u32 k = 0, n_fail = 0;
+        const uint4* code = reinterpret_cast<const uint4*>(a.prog.code);
+        for (u32 i = 0; i < a.prog.n_instr; i++) {
+            uint4 ins = code[i];
+            u32 op = ins.x & 0xff, ext = ins.x >> 8, x = ins.z, y = ins.w;
+            E2 v;
+            switch (op) {
+                CHECK_NODE_CASES(a, N, r, rn, per_row, slot, x, y, ext, v, is_first, is_last, is_trans)
+                default: {   // 15: FOLD of constraint k
+                    E2 c = slot[x];
+                    if ((c.a | c.b) != 0) {
+                        n_fail++;
+                        if (shared_tally) {
+                            atomicAdd(&s_cnt[k], 1u); atomicMin(&s_min[k], (u32)r); census_max(&s_max[k], (u32)r);
+                        } else {   // more constraints than the shared table holds: straight to the global tally
+                            atomicAdd(&a.tally[3 * k], 1ull);
+                            atomicMin(&a.tally[3 * k + 1], (unsigned long long)r);
+                            census_max(&a.tally[3 * k + 2], (unsigned long long)r);
+                        }
+                    }
+                    k++;
+                    continue;
+                }
+            }
+            slot[ins.y] = v;
+        }
+        a.row_count[r] = n_fail;
+        if (n_fail) atomicAdd(&s_rows, 1u);
+    }
+    __syncthreads();
+    // one global update per (block, failing constraint)
+    if (shared_tally) for (u32 k = threadIdx.x; k < a.n_cons; k += blockDim.x) {
+        if (!s_cnt[k]) continue;
+        atomicAdd(&a.tally[3 * k], (unsigned long long)s_cnt[k]);
+        atomicMin(&a.tally[3 * k + 1], (unsigned long long)s_min[k]);
+        census_max(&a.tally[3 * k + 2], (unsigned long long)s_max[k]);
+    }
+    if (threadIdx.x == 0 && s_rows) atomicAdd(a.failing_rows, (unsigned long long)s_rows);
+}
+
+// list mode: rows with failures whose first slot is below max_failures write (row, k, value) per failing k in
+// ascending k from slot offsets[r]; probe mode: thread p writes the record of (row, k) = probes[2p], probes[2p + 1]
+template <int MAXS>
+__global__ void __launch_bounds__(128) k_census_list(CensusArgs a) {
+    size_t N = (size_t)1 << a.log_n;
+    size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    size_t r;
+    u32 want;             // the probed constraint, or 0xFFFFFFFF: every failing one
+    u64 o, end;           // failure slots [o, end) of this thread
+    if (a.probes) {
+        if (t >= a.n_probes) return;
+        r = a.probes[2 * t]; want = (u32)a.probes[2 * t + 1]; o = t; end = t + 1;
+    } else {
+        if (t >= N) return;
+        r = t;
+        u32 cnt = a.row_count[r];
+        if (!cnt) return;
+        o = a.offsets[r];
+        if (o >= a.max_failures) return;
+        want = 0xFFFFFFFFu; end = o + cnt < a.max_failures ? o + cnt : a.max_failures;
+    }
+    size_t rn = (r + 1) & (N - 1);
+    E2 is_first = gl::e2(r == 0, 0), is_last = gl::e2(r == N - 1, 0), is_trans = gl::e2(r != N - 1, 0);
+    size_t per_row = (r & (((size_t)1 << a.prog.log_max_period) - 1)) * a.prog.n_periodic;
+    E2 slot[MAXS];
+    u32 k = 0;
+    const uint4* code = reinterpret_cast<const uint4*>(a.prog.code);
+    for (u32 i = 0; i < a.prog.n_instr; i++) {
+        uint4 ins = code[i];
+        u32 op = ins.x & 0xff, ext = ins.x >> 8, x = ins.z, y = ins.w;
+        E2 v;
+        switch (op) {
+            CHECK_NODE_CASES(a, N, r, rn, per_row, slot, x, y, ext, v, is_first, is_last, is_trans)
+            default: {   // 15: FOLD of constraint k
+                E2 c = slot[x];
+                if (want == 0xFFFFFFFFu ? (c.a | c.b) != 0 : k == want) {
+                    ulonglong2* rec = reinterpret_cast<ulonglong2*>(a.failures + 4 * o);
+                    rec[0] = make_ulonglong2((u64)a.instance | ((u64)k << 32), r);
+                    rec[1] = make_ulonglong2(c.a, c.b);
+                    if (++o == end) return;
+                }
+                k++;
+                continue;
+            }
+        }
+        slot[ins.y] = v;
+    }
+}
+
+int launch_census_rows(const CensusArgs& a, cudaStream_t st) {
+    size_t N = (size_t)1 << a.log_n;
+    unsigned blocks = (unsigned)((N + 127) / 128);
+    if (a.prog.n_slots <= 16) k_census_rows<16><<<blocks, 128, 0, st>>>(a);
+    else if (a.prog.n_slots <= 64) k_census_rows<64><<<blocks, 128, 0, st>>>(a);
+    else if (a.prog.n_slots <= 256) k_census_rows<256><<<blocks, 128, 0, st>>>(a);
+    else if (a.prog.n_slots <= 1024) k_census_rows<1024><<<blocks, 128, 0, st>>>(a);
+    else return -1;
+    COUNT_LAUNCH();
+    return 0;
+}
+int launch_census_list(const CensusArgs& a, cudaStream_t st) {
+    size_t n = a.probes ? a.n_probes : (size_t)1 << a.log_n;
+    if (n == 0) return 0;
+    unsigned blocks = (unsigned)((n + 127) / 128);
+    if (a.prog.n_slots <= 16) k_census_list<16><<<blocks, 128, 0, st>>>(a);
+    else if (a.prog.n_slots <= 64) k_census_list<64><<<blocks, 128, 0, st>>>(a);
+    else if (a.prog.n_slots <= 256) k_census_list<256><<<blocks, 128, 0, st>>>(a);
+    else if (a.prog.n_slots <= 1024) k_census_list<1024><<<blocks, 128, 0, st>>>(a);
     else return -1;
     COUNT_LAUNCH();
     return 0;
@@ -1260,6 +1405,56 @@ void launch_ef_exclusive_scan(const u64* totals, size_t n, u64* acc0, u64* acc1,
     k_scan_block_totals<<<(unsigned)nb, SCAN_T, 0, st>>>(totals, n, scratch);
     k_scan_block_sums<<<1, 32, 0, st>>>(scratch, nb, final2);
     k_scan_apply<<<(unsigned)nb, SCAN_T, 0, st>>>(totals, n, scratch, acc0, acc1);
+    COUNT_LAUNCH(); COUNT_LAUNCH(); COUNT_LAUNCH();
+}
+
+// the same three phases over u32 counts into u64 offsets (the census's per-row failure counts)
+__global__ void __launch_bounds__(SCAN_T) k_count_scan_block_totals(const u32* __restrict__ counts, size_t n, u64* __restrict__ block_sums) {
+    __shared__ u64 sh[SCAN_T];
+    size_t base = (size_t)blockIdx.x * SCAN_B + (size_t)threadIdx.x * SCAN_E;
+    u64 s = 0;
+    for (int e = 0; e < SCAN_E; e++) if (base + e < n) s += counts[base + e];
+    sh[threadIdx.x] = s;
+    __syncthreads();
+    for (int off = SCAN_T / 2; off > 0; off >>= 1) {
+        if (threadIdx.x < off) sh[threadIdx.x] += sh[threadIdx.x + off];
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) block_sums[blockIdx.x] = sh[0];
+}
+__global__ void k_count_scan_block_sums(u64* block_sums, size_t n_blocks, u64* total) {
+    if (threadIdx.x || blockIdx.x) return;
+    u64 acc = 0;
+    for (size_t b = 0; b < n_blocks; b++) { u64 v = block_sums[b]; block_sums[b] = acc; acc += v; }
+    *total = acc;
+}
+__global__ void __launch_bounds__(SCAN_T) k_count_scan_apply(const u32* __restrict__ counts, size_t n, const u64* __restrict__ block_sums,
+                                                             u64* __restrict__ offsets) {
+    __shared__ u64 sh[SCAN_T];
+    size_t base = (size_t)blockIdx.x * SCAN_B + (size_t)threadIdx.x * SCAN_E;
+    u32 v[SCAN_E];
+    u64 s = 0;
+    for (int e = 0; e < SCAN_E; e++) { v[e] = base + e < n ? counts[base + e] : 0; s += v[e]; }
+    sh[threadIdx.x] = s;
+    __syncthreads();
+    // Hillis-Steele inclusive scan of the per-thread sums
+    for (int off = 1; off < SCAN_T; off <<= 1) {
+        u64 add = (int)threadIdx.x >= off ? sh[threadIdx.x - off] : 0;
+        __syncthreads();
+        sh[threadIdx.x] += add;
+        __syncthreads();
+    }
+    u64 run = block_sums[blockIdx.x] + (threadIdx.x > 0 ? sh[threadIdx.x - 1] : 0);
+    for (int e = 0; e < SCAN_E; e++) {
+        if (base + e < n) offsets[base + e] = run;
+        run += v[e];
+    }
+}
+void launch_count_exclusive_scan(const u32* counts, size_t n, u64* offsets, u64* total, u64* scratch, cudaStream_t st) {
+    size_t nb = (n + SCAN_B - 1) / SCAN_B;
+    k_count_scan_block_totals<<<(unsigned)nb, SCAN_T, 0, st>>>(counts, n, scratch);
+    k_count_scan_block_sums<<<1, 32, 0, st>>>(scratch, nb, total);
+    k_count_scan_apply<<<(unsigned)nb, SCAN_T, 0, st>>>(counts, n, scratch, offsets);
     COUNT_LAUNCH(); COUNT_LAUNCH(); COUNT_LAUNCH();
 }
 

@@ -203,6 +203,40 @@ struct CheckArgs {
 int launch_check_rows(const CheckArgs& a, cudaStream_t st);   // 0, or -1 when the program needs too many slots
 
 // ---------------------------------------------------------------------------------------------
+// Constraint census: every violation, not only the first (mdn_constraint_census)
+// ---------------------------------------------------------------------------------------------
+// The program and trace-domain reads of CheckArgs, one thread per row of the whole AIR.
+//   k_census_rows: row_count[r] = the number of non-zero constraints at row r (every row is written); per constraint k
+//     tally[3k] += rows where k is non-zero, tally[3k + 1] = min row (init ~0), tally[3k + 2] = max row (init 0),
+//     aggregated per block in shared memory when n_cons <= CENSUS_SHARED_K (one global atomic of each kind per block
+//     and failing constraint), else straight to global memory; failing_rows += rows with at least one failure.
+//   k_census_list: with probes == NULL, a row whose count is non-zero and whose offsets[r] < max_failures writes its
+//     failures in ascending k to slots [offsets[r], min(offsets[r] + count, max_failures)); with probes, thread p
+//     writes the record of (row, k) = (probes[2p], probes[2p + 1]) to slot p.  A record is 4 u64, the layout of
+//     mdn_constraint_failure: instance | k << 32, row, value c0, value c1.
+static constexpr u32 CENSUS_SHARED_K = 256;
+struct CensusArgs {
+    const u64* main_cm; const u64* aux_cm; const u64* prep_cm;   // as CheckArgs
+    u32 log_n;
+    AirDev prog;
+    const u64* publics; const u64* challenges; const u64* aux_values;
+    u32 n_cons;                          // constraints (FOLDs) of the program
+    u32 instance;                        // written into every record
+    u32* row_count;                      // 2^log_n counts of this AIR
+    unsigned long long* tally;           // 3 * n_cons
+    unsigned long long* failing_rows;
+    const u64* offsets;                  // exclusive scan of row_count, offset by the failures of earlier AIRs
+    u64 max_failures;
+    u64* failures;                       // 4 u64 per record
+    const u64* probes; size_t n_probes;  // probe mode, or NULL
+};
+int launch_census_rows(const CensusArgs& a, cudaStream_t st);   // 0, or -1 when the program needs too many slots
+int launch_census_list(const CensusArgs& a, cudaStream_t st);   // list or probe mode; 0 or -1 as above
+// Exclusive prefix sum of n u32 counts into u64 offsets, the grand total into *total (device); `scratch` needs
+// ceil(n / 2048) u64.
+void launch_count_exclusive_scan(const u32* counts, size_t n, u64* offsets, u64* total, u64* scratch, cudaStream_t st);
+
+// ---------------------------------------------------------------------------------------------
 // LogUp bus balance without proving (mdn_check_trace_balance; reference air/src/lookup/debug/trace/mod.rs:169-309)
 // ---------------------------------------------------------------------------------------------
 // Open-addressing hash table keyed by the 128-bit encoded denominator (c0, c1), `mask + 1` slots (a power of two, at

@@ -332,6 +332,17 @@ struct mdn_session {
     int eval_external(u32* failed);
     void check_constraints(const mdn_statement* st, const mdn_matrix* traces, const mdn_matrix* prep, const mdn_challenger* ch,
                            mdn_aux_builder build_aux, void* aux_ctx, u32 flags, mdn_constraint_report* out);
+    // what prepare_check leaves per instance for the row pass of check_constraints / constraint_census
+    struct CheckSetup {
+        std::vector<u32> pos;                    // proof position of each instance (main_c / aux_c index)
+        std::vector<DevBuf> prep_cm, periodic;   // raw preprocessed trace and periodic matrix, or empty
+        int ext_rc = 0; u32 ext_failed = 0;      // the external check: > 0 with ext_failed = the failing assertion
+    };
+    void prepare_check(const mdn_statement* st, const mdn_matrix* traces, const mdn_matrix* prep, const mdn_challenger* ch,
+                       mdn_aux_builder build_aux, void* aux_ctx, u32 flags, CheckSetup& cs);
+    void constraint_census(const mdn_statement* st, const mdn_matrix* traces, const mdn_matrix* prep, const mdn_challenger* ch,
+                           mdn_aux_builder build_aux, void* aux_ctx, u32 flags, mdn_constraint_failure* failures, u64 max_failures,
+                           mdn_constraint_tally* tallies, u64 max_tallies, mdn_constraint_census_report* out);
     void check_trace_balance(const mdn_statement* st, const mdn_matrix* traces, const u64* rnd, const u64* boundary, size_t n_boundary,
                              const uint32_t* const* mutex_sites, u64 max_contrib, u32 flags, mdn_balance_report* out);
     void check_lookup_folds(const mdn_statement* st, const mdn_matrix* traces, const u64* rnd, const uint32_t* const* fold_marks,
@@ -1348,13 +1359,72 @@ int mdn_session::eval_external(u32* failed) {
 // the instance shape only (no commitment is observed); aux traces from the device LogUp build, the host callback or
 // zeros; the session's external check; then k_check_rows per AIR in instance order.  Nothing of the last proof's
 // outputs, timings or introspection is touched; the caller releases the proof arena afterwards.
+// prepare_check is everything before the row pass, shared with constraint_census.
 void mdn_session::check_constraints(const mdn_statement* st, const mdn_matrix* traces, const mdn_matrix* prep, const mdn_challenger* chal,
                                     mdn_aux_builder build_aux, void* aux_ctx, u32 flags, mdn_constraint_report* out) {
+    if (!out) fail(MDN_ERR_INVALID_ARG, "null argument");
+    CheckSetup cs;
+    prepare_check(st, traces, prep, chal, build_aux, aux_ctx, flags, cs);
+    const u32 k = st->n_airs;
+    const std::vector<u32>& pos = cs.pos;
+    const int ext_rc = cs.ext_rc;
+    const u32 ext_failed = cs.ext_failed;
+
+    // row checks (debug.rs:120-214): per AIR the lowest (row, constraint) that is non-zero and the failing-row count
+    DevBuf res; res.alloc(2 * (size_t)k + 4, stream);
+    std::vector<u64> host_res(2 * (size_t)k + 4, 0);
+    for (u32 i = 0; i < k; i++) host_res[2 * i] = ~0ull;
+    CUDA_OK(cudaMemcpyAsync(res.p, host_res.data(), host_res.size() * sizeof(u64), cudaMemcpyHostToDevice, stream));
+    std::vector<mk::CheckArgs> ca(k);
+    for (u32 i = 0; i < k; i++) {
+        u32 j = pos[i];
+        AirHost& h = airs[i];
+        mk::CheckArgs& c = ca[i];
+        c = mk::CheckArgs{};
+        c.main_cm = main_c.mats[j].coef;
+        c.aux_cm = h.desc.aux_width ? aux_c.mats[j].coef : nullptr;
+        c.prep_cm = cs.prep_cm[i].p;
+        c.log_n = log_heights[i];
+        c.prog = h.dev;
+        c.prog.periodic = cs.periodic[i].p;
+        c.publics = d_publics.p; c.challenges = d_randomness.p; c.aux_values = d_aux_values.p + aux_values_off[j];
+        c.row0 = 0; c.n_rows = (size_t)1 << log_heights[i];
+        c.first = (unsigned long long*)(res.p + 2 * i); c.failing_rows = (unsigned long long*)(res.p + 2 * i + 1);
+        if (mk::launch_check_rows(c, stream) != 0) fail(MDN_ERR_UNSUPPORTED, "AIR %u: constraint program too large for the interpreter", i);
+    }
+    CUDA_OK(cudaMemcpyAsync(host_res.data(), res.p, 2 * (size_t)k * sizeof(u64), cudaMemcpyDeviceToHost, stream));
+    CUDA_OK(cudaStreamSynchronize(stream));
+    CUDA_OK(cudaGetLastError());
+
+    memset(out, 0, sizeof *out);
+    for (u32 i = 0; i < k; i++) out->failing_rows += host_res[2 * i + 1];
+    if (ext_rc > 0) { out->kind = 2; out->constraint = ext_failed; }
+    else for (u32 i = 0; i < k; i++) {
+        u64 f = host_res[2 * i];
+        if (f == ~0ull) continue;
+        out->kind = 1; out->instance = i; out->row = f >> 32; out->constraint = (u32)f;
+        // the value: the same kernel on that one row, recording constraint K (its own atomics go to scratch words)
+        mk::CheckArgs c = ca[i];
+        c.row0 = out->row; c.n_rows = 1; c.probe_k = out->constraint; c.probe_value = res.p + 2 * (size_t)k;
+        c.first = (unsigned long long*)(res.p + 2 * (size_t)k + 2); c.failing_rows = (unsigned long long*)(res.p + 2 * (size_t)k + 3);
+        if (mk::launch_check_rows(c, stream) != 0) fail(MDN_ERR_UNSUPPORTED, "AIR %u: constraint program too large for the interpreter", i);
+        CUDA_OK(cudaMemcpyAsync(out->value, res.p + 2 * (size_t)k, 2 * sizeof(u64), cudaMemcpyDeviceToHost, stream));
+        CUDA_OK(cudaStreamSynchronize(stream));
+        break;
+    }
+    out->holds = ext_rc == 0 && out->failing_rows == 0;
+}
+
+// Validation, challenges, main / preprocessed / periodic upload, aux traces and the external check of a constraint
+// check (debug.rs:70-118): after it, main_c / aux_c hold the raw column-major traces in proof order (cs.pos[instance]),
+// d_publics / d_randomness / d_aux_values the leaves, and cs the per-instance preprocessed and periodic buffers and
+// the external check's outcome.
+void mdn_session::prepare_check(const mdn_statement* st, const mdn_matrix* traces, const mdn_matrix* prep, const mdn_challenger* chal,
+                                mdn_aux_builder build_aux, void* aux_ctx, u32 flags, CheckSetup& cs) {
     const bool cm = column_major(flags);
     reset_proof();
     prof.st = stream; prof.reset();
     if (!d_flag.p) { ArenaScope persistent(nullptr); d_flag.alloc(1, stream); CUDA_OK(cudaMemsetAsync(d_flag.p, 0, 8, stream)); }
-    if (!out) fail(MDN_ERR_INVALID_ARG, "null argument");
     validate_statement(st, traces, chal);
     if (cm) for (u32 i = 0; i < st->n_airs; i++) check_column_major(traces[i], "trace", i);
     const bool on_device = (flags & MDN_FLAG_DEVICE_TRACES) != 0;
@@ -1387,7 +1457,8 @@ void mdn_session::check_constraints(const mdn_statement* st, const mdn_matrix* t
 
     // raw main traces, column-major, proof order (the layout build_logup_aux reads); column-major device traces are
     // read where the caller keeps them (only read: the const_cast feeds the common CommittedMat)
-    std::vector<u32> pos(k);
+    std::vector<u32>& pos = cs.pos;
+    pos.assign(k, 0);
     size_t main_total = 0, aux_total = 0;
     for (u32 j = 0; j < k; j++) {
         u32 inst = order[j];
@@ -1408,7 +1479,10 @@ void mdn_session::check_constraints(const mdn_statement* st, const mdn_matrix* t
     }
     for (u32 j = 0; j < k; j++) upload_matrix(traces[order[j]], on_device, main_c.mats[j].coef, cm);   // column-major: check only
     check_input_flag("a main trace");
-    std::vector<DevBuf> prep_cm(k), periodic(k);
+    std::vector<DevBuf>& prep_cm = cs.prep_cm;
+    std::vector<DevBuf>& periodic = cs.periodic;
+    prep_cm.clear(); prep_cm.resize(k);
+    periodic.clear(); periodic.resize(k);
     if (prep) {
         for (u32 i = 0; i < k; i++) if (prep[i].width) {
             prep_cm[i].alloc(((size_t)1 << prep[i].log_height) * prep[i].width, stream);
@@ -1467,53 +1541,142 @@ void mdn_session::check_constraints(const mdn_statement* st, const mdn_matrix* t
     if (!flat_values.empty()) CUDA_OK(cudaMemcpyAsync(d_aux_values.p, flat_values.data(), flat_values.size() * sizeof(u64), cudaMemcpyHostToDevice, stream));
 
     // external assertions before the row checks (debug.rs:108-118); a failing one is reported, the rows still run
-    u32 ext_failed = 0;
-    int ext_rc = eval_external(&ext_failed);
-    if (ext_rc < 0) fail(MDN_ERR_EXTERNAL_ASSERTION, "eval_external reported a reduction error");
+    cs.ext_failed = 0;
+    cs.ext_rc = eval_external(&cs.ext_failed);
+    if (cs.ext_rc < 0) fail(MDN_ERR_EXTERNAL_ASSERTION, "eval_external reported a reduction error");
+}
 
-    // row checks (debug.rs:120-214): per AIR the lowest (row, constraint) that is non-zero and the failing-row count
-    DevBuf res; res.alloc(2 * (size_t)k + 4, stream);
-    std::vector<u64> host_res(2 * (size_t)k + 4, 0);
-    for (u32 i = 0; i < k; i++) host_res[2 * i] = ~0ull;
-    CUDA_OK(cudaMemcpyAsync(res.p, host_res.data(), host_res.size() * sizeof(u64), cudaMemcpyHostToDevice, stream));
-    std::vector<mk::CheckArgs> ca(k);
+// ---------------------------------------------------------------------------------------------
+// constraint_census: every violated constraint of every AIR, per constraint and in row order, without a proof
+// ---------------------------------------------------------------------------------------------
+// prepare_check as check_constraints; then per AIR (instance order) k_census_rows fills that AIR's slice of one
+// per-row count array, concatenated in instance order, and its per-constraint tally; one exclusive scan of the counts
+// gives every failing row its first failure slot and the total.  k_census_list then writes the first max_failures
+// records in (instance, row, constraint) order, and in probe mode the values at the reported tallies' first rows (plus
+// the least failure's, when truncation drops it).  Counts, minima, maxima and the scan do not depend on the order
+// the atomics ran in, so neither does anything reported.
+void mdn_session::constraint_census(const mdn_statement* st, const mdn_matrix* traces, const mdn_matrix* prep, const mdn_challenger* chal,
+                                    mdn_aux_builder build_aux, void* aux_ctx, u32 flags, mdn_constraint_failure* failures, u64 max_failures,
+                                    mdn_constraint_tally* tallies, u64 max_tallies, mdn_constraint_census_report* out) {
+    CheckSetup cs;
+    prepare_check(st, traces, prep, chal, build_aux, aux_ctx, flags, cs);
+    const u32 k = st->n_airs;
+
+    // per-row counts of all AIRs (u32, instance order), their offsets, one tally table per AIR, two counters
+    std::vector<size_t> row_base(k + 1, 0), tally_base(k + 1, 0);
     for (u32 i = 0; i < k; i++) {
-        u32 j = pos[i];
+        row_base[i + 1] = row_base[i] + ((size_t)1 << log_heights[i]);
+        tally_base[i + 1] = tally_base[i] + 3 * (size_t)airs[i].n_constraints;
+    }
+    const size_t rows = row_base[k];
+    DevBuf counts, offsets, tally, words, scratch;
+    counts.alloc((rows + 1) / 2, stream);
+    offsets.alloc(rows, stream);
+    tally.alloc(std::max<size_t>(1, tally_base[k]), stream);
+    words.alloc(2, stream);                       // rows with a failure, violations
+    scratch.alloc((rows + 2047) / 2048, stream);  // block sums of the scan
+    std::vector<u64> host_tally(std::max<size_t>(1, tally_base[k]), 0);
+    for (size_t q = 0; q < tally_base[k]; q += 3) host_tally[q + 1] = ~0ull;
+    CUDA_OK(cudaMemcpyAsync(tally.p, host_tally.data(), host_tally.size() * sizeof(u64), cudaMemcpyHostToDevice, stream));
+    CUDA_OK(cudaMemsetAsync(words.p, 0, 2 * sizeof(u64), stream));
+    u32* d_counts = reinterpret_cast<u32*>(counts.p);
+    std::vector<mk::CensusArgs> ca(k);
+    for (u32 i = 0; i < k; i++) {
+        u32 j = cs.pos[i];
         AirHost& h = airs[i];
-        mk::CheckArgs& c = ca[i];
-        c = mk::CheckArgs{};
+        mk::CensusArgs& c = ca[i];
+        c = mk::CensusArgs{};
         c.main_cm = main_c.mats[j].coef;
         c.aux_cm = h.desc.aux_width ? aux_c.mats[j].coef : nullptr;
-        c.prep_cm = prep_cm[i].p;
+        c.prep_cm = cs.prep_cm[i].p;
         c.log_n = log_heights[i];
         c.prog = h.dev;
-        c.prog.periodic = periodic[i].p;
+        c.prog.periodic = cs.periodic[i].p;
         c.publics = d_publics.p; c.challenges = d_randomness.p; c.aux_values = d_aux_values.p + aux_values_off[j];
-        c.row0 = 0; c.n_rows = (size_t)1 << log_heights[i];
-        c.first = (unsigned long long*)(res.p + 2 * i); c.failing_rows = (unsigned long long*)(res.p + 2 * i + 1);
-        if (mk::launch_check_rows(c, stream) != 0) fail(MDN_ERR_UNSUPPORTED, "AIR %u: constraint program too large for the interpreter", i);
+        c.n_cons = h.n_constraints;
+        c.instance = i;
+        c.row_count = d_counts + row_base[i];
+        c.tally = (unsigned long long*)(tally.p + tally_base[i]);
+        c.failing_rows = (unsigned long long*)words.p;
+        c.offsets = offsets.p + row_base[i];
+        if (mk::launch_census_rows(c, stream) != 0) fail(MDN_ERR_UNSUPPORTED, "AIR %u: constraint program too large for the interpreter", i);
     }
-    CUDA_OK(cudaMemcpyAsync(host_res.data(), res.p, 2 * (size_t)k * sizeof(u64), cudaMemcpyDeviceToHost, stream));
+    mk::launch_count_exclusive_scan(d_counts, rows, offsets.p, words.p + 1, scratch.p, stream);
+    u64 host_words[2];
+    CUDA_OK(cudaMemcpyAsync(host_tally.data(), tally.p, host_tally.size() * sizeof(u64), cudaMemcpyDeviceToHost, stream));
+    CUDA_OK(cudaMemcpyAsync(host_words, words.p, sizeof host_words, cudaMemcpyDeviceToHost, stream));
     CUDA_OK(cudaStreamSynchronize(stream));
     CUDA_OK(cudaGetLastError());
 
+    // the failing (instance, constraint) pairs in order, and the least failure: the first failing instance's least
+    // (first_row, constraint)
+    std::vector<mdn_constraint_tally> all;
+    size_t least = SIZE_MAX;
+    for (u32 i = 0; i < k; i++)
+        for (u32 c = 0; c < airs[i].n_constraints; c++) {
+            const u64* t = host_tally.data() + tally_base[i] + 3 * (size_t)c;
+            if (!t[0]) continue;
+            all.push_back(mdn_constraint_tally{i, c, t[0], t[1], t[2], {0, 0}});
+            if (least == SIZE_MAX || (all[least].instance == i && t[1] < all[least].first_row)) least = all.size() - 1;
+        }
     memset(out, 0, sizeof *out);
-    for (u32 i = 0; i < k; i++) out->failing_rows += host_res[2 * i + 1];
-    if (ext_rc > 0) { out->kind = 2; out->constraint = ext_failed; }
-    else for (u32 i = 0; i < k; i++) {
-        u64 f = host_res[2 * i];
-        if (f == ~0ull) continue;
-        out->kind = 1; out->instance = i; out->row = f >> 32; out->constraint = (u32)f;
-        // the value: the same kernel on that one row, recording constraint K (its own atomics go to scratch words)
-        mk::CheckArgs c = ca[i];
-        c.row0 = out->row; c.n_rows = 1; c.probe_k = out->constraint; c.probe_value = res.p + 2 * (size_t)k;
-        c.first = (unsigned long long*)(res.p + 2 * (size_t)k + 2); c.failing_rows = (unsigned long long*)(res.p + 2 * (size_t)k + 3);
-        if (mk::launch_check_rows(c, stream) != 0) fail(MDN_ERR_UNSUPPORTED, "AIR %u: constraint program too large for the interpreter", i);
-        CUDA_OK(cudaMemcpyAsync(out->value, res.p + 2 * (size_t)k, 2 * sizeof(u64), cudaMemcpyDeviceToHost, stream));
-        CUDA_OK(cudaStreamSynchronize(stream));
-        break;
+    out->violations = host_words[1];
+    out->n_failures = std::min<u64>(out->violations, max_failures);
+    out->failing_constraints = all.size();
+    out->n_tallies = std::min<u64>(all.size(), max_tallies);
+
+    // values at the first rows of the reported tallies and of the least failure: probe mode, one launch per instance
+    std::vector<size_t> probed;
+    for (size_t q = 0; q < out->n_tallies; q++) probed.push_back(q);
+    if (least != SIZE_MAX && least >= out->n_tallies) probed.push_back(least);   // `all` is in instance order: still sorted
+    DevBuf d_probes, d_records, d_failures;
+    if (!probed.empty()) {
+        std::vector<u64> pr;
+        for (size_t q : probed) { pr.push_back(all[q].first_row); pr.push_back(all[q].constraint); }
+        d_probes.alloc(pr.size(), stream);
+        d_records.alloc(4 * probed.size(), stream);
+        CUDA_OK(cudaMemcpyAsync(d_probes.p, pr.data(), pr.size() * sizeof(u64), cudaMemcpyHostToDevice, stream));
+        for (size_t b = 0; b < probed.size();) {
+            u32 i = all[probed[b]].instance;
+            size_t e = b;
+            while (e < probed.size() && all[probed[e]].instance == i) e++;
+            mk::CensusArgs c = ca[i];
+            c.probes = d_probes.p + 2 * b; c.n_probes = e - b; c.failures = d_records.p + 4 * b;
+            if (mk::launch_census_list(c, stream) != 0) fail(MDN_ERR_UNSUPPORTED, "AIR %u: constraint program too large for the interpreter", i);
+            b = e;
+        }
     }
-    out->holds = ext_rc == 0 && out->failing_rows == 0;
+    // the first n_failures records, every AIR with a failing constraint writing its own slots
+    if (out->n_failures) {
+        d_failures.alloc(4 * out->n_failures, stream);
+        for (u32 i = 0; i < k; i++) {
+            bool any = false;
+            for (u32 c = 0; c < airs[i].n_constraints && !any; c++) any = host_tally[tally_base[i] + 3 * (size_t)c] != 0;
+            if (!any) continue;
+            mk::CensusArgs c = ca[i];
+            c.max_failures = out->n_failures; c.failures = d_failures.p;
+            if (mk::launch_census_list(c, stream) != 0) fail(MDN_ERR_UNSUPPORTED, "AIR %u: constraint program too large for the interpreter", i);
+        }
+    }
+    std::vector<u64> records(4 * probed.size());
+    if (!probed.empty()) CUDA_OK(cudaMemcpyAsync(records.data(), d_records.p, records.size() * sizeof(u64), cudaMemcpyDeviceToHost, stream));
+    static_assert(sizeof(mdn_constraint_failure) == 4 * sizeof(u64), "mdn_constraint_failure is the kernel's record");
+    if (out->n_failures) CUDA_OK(cudaMemcpyAsync(failures, d_failures.p, out->n_failures * sizeof(mdn_constraint_failure), cudaMemcpyDeviceToHost, stream));
+    CUDA_OK(cudaStreamSynchronize(stream));
+    CUDA_OK(cudaGetLastError());
+    for (size_t q = 0; q < probed.size(); q++) { all[probed[q]].first_value[0] = records[4 * q + 2]; all[probed[q]].first_value[1] = records[4 * q + 3]; }
+    for (size_t q = 0; q < out->n_tallies; q++) tallies[q] = all[q];
+
+    // `first`: what check_constraints reports for the same call
+    mdn_constraint_report& f = out->first;
+    f.failing_rows = host_words[0];
+    if (cs.ext_rc > 0) { f.kind = 2; f.constraint = cs.ext_failed; }
+    else if (least != SIZE_MAX) {
+        const mdn_constraint_tally& t = all[least];
+        f.kind = 1; f.instance = t.instance; f.row = t.first_row; f.constraint = t.constraint;
+        f.value[0] = t.first_value[0]; f.value[1] = t.first_value[1];
+    }
+    f.holds = cs.ext_rc == 0 && f.failing_rows == 0;
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -2752,6 +2915,28 @@ int mdn_check_constraints(mdn_session* s, const mdn_statement* st, const mdn_mat
         ArenaScope proof_memory(s->use_arena ? &s->arena : nullptr);
         CUDA_OK(cudaSetDevice(s->device));
         s->check_constraints(st, traces, preprocessed, challenger, build_aux, aux_ctx, flags, out);
+        if (randomness_out) for (size_t i = 0; i < s->randomness.size(); i++) { randomness_out[2 * i] = s->randomness[i].a; randomness_out[2 * i + 1] = s->randomness[i].b; }
+    }
+    s->reset_proof();
+    API_CATCH(s)
+}
+
+int mdn_constraint_census(mdn_session* s, const mdn_statement* st, const mdn_matrix* traces, const mdn_matrix* preprocessed,
+                          const mdn_challenger* challenger, mdn_aux_builder build_aux, void* aux_ctx, uint32_t flags,
+                          uint64_t* randomness_out, mdn_constraint_failure* failures, uint64_t max_failures,
+                          mdn_constraint_tally* tallies, uint64_t max_tallies, mdn_constraint_census_report* out) {
+    if (!s) return MDN_ERR_INVALID_ARG;
+    // refused before any device work, so that a staged proof in progress stays intact
+    if (s->in_proof) { s->error = "mdn_constraint_census called inside a proof (between mdn_prove_begin and mdn_prove_finish)"; return MDN_ERR_INVALID_ARG; }
+    if (s->shard_world > 1) { s->error = "mdn_constraint_census does not run on a session split over ranks (mdn_session_set_shard world > 1)"; return MDN_ERR_UNSUPPORTED; }
+    if (!out) { s->error = "null argument"; return MDN_ERR_INVALID_ARG; }
+    if (!failures && max_failures) { s->error = "failures is NULL but max_failures is not 0"; return MDN_ERR_INVALID_ARG; }
+    if (!tallies && max_tallies) { s->error = "tallies is NULL but max_tallies is not 0"; return MDN_ERR_INVALID_ARG; }
+    API_TRY(s)
+    {
+        ArenaScope proof_memory(s->use_arena ? &s->arena : nullptr);
+        CUDA_OK(cudaSetDevice(s->device));
+        s->constraint_census(st, traces, preprocessed, challenger, build_aux, aux_ctx, flags, failures, max_failures, tallies, max_tallies, out);
         if (randomness_out) for (size_t i = 0; i < s->randomness.size(); i++) { randomness_out[2 * i] = s->randomness[i].a; randomness_out[2 * i + 1] = s->randomness[i].b; }
     }
     s->reset_proof();

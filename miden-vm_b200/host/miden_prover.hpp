@@ -354,6 +354,55 @@ inline void check_constraints(const StarkConfig& config, const DeviceProverState
     if (!rep.holds) throw ConstraintViolation(rep);
 }
 
+// Every violated constraint of a statement (mdn_constraint_census), copied out of the call: `first` is what
+// check_constraints reports, `tallies` one entry per failing (instance, constraint) and `failures` the violations in
+// (instance, row, constraint) order, each list truncated to the capacity the call was given.
+struct ConstraintCensus {
+    mdn_constraint_census_report counts{};
+    std::vector<mdn_constraint_failure> failures;
+    std::vector<mdn_constraint_tally> tallies;
+    const mdn_constraint_report& first() const { return counts.first; }
+    bool holds() const { return counts.first.holds != 0; }
+    // one line per failing constraint, then one per listed failure, in the wording of check_constraints' panics
+    std::string to_string() const {
+        std::string s;
+        if (counts.first.kind == 2) s += ConstraintViolation::message(counts.first) + "\n";
+        for (const mdn_constraint_tally& t : tallies)
+            s += "constraint " + std::to_string(t.constraint) + " of instance " + std::to_string(t.instance) + " not satisfied on " +
+                 std::to_string(t.failing_rows) + " rows (rows " + std::to_string(t.first_row) + " .. " + std::to_string(t.last_row) + ")\n";
+        if (tallies.size() < counts.failing_constraints) s += "... " + std::to_string(counts.failing_constraints - tallies.size()) + " more failing constraints\n";
+        for (const mdn_constraint_failure& f : failures)
+            s += "constraint not satisfied at instance " + std::to_string(f.instance) + ", row " + std::to_string(f.row) +
+                 " (constraint " + std::to_string(f.constraint) + ")\n";
+        if (failures.size() < counts.violations) s += "... " + std::to_string(counts.violations - failures.size()) + " more violations\n";
+        return s;
+    }
+};
+// check_constraints without stopping at the first failure: returns the census instead of throwing (errors of the call
+// itself still throw ProverError).  At most max_failures violations and max_tallies tallies are listed.
+inline ConstraintCensus constraint_census(const StarkConfig& config, const ProverStatement& ps, Challenger challenger, AuxBuilder aux = nullptr,
+                                          uint64_t max_failures = 1024, uint64_t max_tallies = 1024) {
+    detail::Lowered low(ps.statement);
+    std::vector<mdn_matrix> mats, prep;
+    bool any_prep = false;
+    for (const RowMajorMatrix& t : ps.traces) mats.push_back(t.raw());
+    for (const Air& a : ps.statement.airs) {
+        prep.push_back(a.preprocessed_width ? a.preprocessed_trace.raw() : mdn_matrix{nullptr, 0, 0});
+        any_prep |= a.preprocessed_width > 0;
+    }
+    detail::AuxCall ctx{&ps, &aux};
+    ConstraintCensus out;
+    out.failures.resize(max_failures);
+    out.tallies.resize(max_tallies);
+    detail::check(config, mdn_constraint_census(config.session(), &low.st, mats.data(), any_prep ? prep.data() : nullptr,
+                                                config.hash_challenger() ? nullptr : &challenger.raw, aux ? &detail::AuxCall::call : nullptr,
+                                                &ctx, 0, nullptr, max_failures ? out.failures.data() : nullptr, max_failures,
+                                                max_tallies ? out.tallies.data() : nullptr, max_tallies, &out.counts));
+    out.failures.resize(out.counts.n_failures);
+    out.tallies.resize(out.counts.n_tallies);
+    return out;
+}
+
 // check_trace_balance's BalanceReport (air/src/lookup/debug/trace/mod.rs:44-95), copied out of the session.  A push names its
 // interaction (the index in the AIR's lookup program) where the reference names its group and message; the caller maps
 // the index back to its insert site.  Boundary emissions have instance / column 0xFFFFFFFF and row UINT64_MAX.
