@@ -42,6 +42,7 @@ typedef enum {
     MDN_ERR_AUX_BUILDER = -5,      /* aux-trace callback failed */
     MDN_ERR_NO_DEVICE = -6,
     MDN_ERR_EXTERNAL_ASSERTION = -7,   /* ProverError::ExternalAssertionFailed / ::Reduction (prover/mod.rs:383-395) */
+    MDN_ERR_CONSTRAINT_VIOLATED = -8,  /* the constraint guard refused the proof (mdn_session_set_constraint_guard) */
 } mdn_status;
 
 /* PcsParams::new(log_blowup, log_folding_arity, log_final_degree, folding_pow_bits,
@@ -333,6 +334,34 @@ int mdn_check_constraints(mdn_session* s, const mdn_statement* st, const mdn_mat
                           uint32_t flags, uint64_t* randomness_out /* 2*max num_randomness, may be NULL */,
                           mdn_constraint_report* out);
 
+/* ---- refuse to prove a statement that does not hold: the constraint guard ---------------------------------------
+ * enable = 1 makes every later mdn_prove / mdn_prove_commit_aux of this session check every constraint of every AIR on
+ * every trace row before anything of the aux phase is committed; 0 (the default) turns it off.  Any other value, and a
+ * call between mdn_prove_begin and mdn_prove_finish, is MDN_ERR_INVALID_ARG.
+ * When: after the aux traces and aux values are final (host builder, device aux builder, device LogUp build, the
+ * caller's aux of mdn_prove_commit_aux, or zeros) and the external assertions hold -- a failing assertion is still
+ * MDN_ERR_EXTERNAL_ASSERTION and the guard does not run -- and before the aux commitment.
+ * What it reads: the raw main traces (a copy kept from before the inverse NTT, or a column-major device trace in place,
+ * which the caller keeps unchanged until mdn_prove_commit_aux returns, as for a LogUp build), the raw aux traces and aux
+ * values about to be committed, the raw preprocessed rows (re-derived on the device from the installed bundle) and the
+ * raw periodic matrices.  The challenges are the PROOF's randomness, sampled after the main commitment (what
+ * mdn_prove_begin writes to randomness_out), and the proof's public values -- not the debug challenges of
+ * mdn_check_constraints, which observe no commitment.  Rows, next row, selectors and the first failure (least
+ * (instance, row, constraint)) are exactly those of mdn_check_constraints.
+ * A non-zero constraint makes the call return MDN_ERR_CONSTRAINT_VIOLATED: mdn_last_error names the instance, row and
+ * constraint, nothing is committed and the proof is abandoned, as after a failing external assertion.  A statement that
+ * holds gets the byte-identical proof it gets with the guard off: the guard observes and samples nothing.
+ * Cost: the raw main copies (N x width x 8 bytes per AIR of the proof arena) and one k_check_rows pass per AIR; its
+ * launches count in mdn_timings.kernel_launches and its time in kernel class 4 and in commit_aux.
+ * A session split over ranks (mdn_session_set_shard): every rank holds the whole raw main and aux traces and runs the
+ * whole check on them, with no communication; every rank returns the same status and report. */
+int mdn_session_set_constraint_guard(mdn_session* s, uint32_t enable);
+/* The report of the last guard run: kind 1 with instance, row, constraint, value and failing_rows (over all AIRs) as
+ * mdn_check_constraints fills them, holds = 0, after a refusal; holds = 1, kind = 0 and every other field 0 after a
+ * guard run that passed and before any guard run.  Proofs with the guard off, proofs that fail before the guard and
+ * mdn_check_constraints leave it unchanged.  NULL s or out: MDN_ERR_INVALID_ARG. */
+int mdn_last_constraint_report(const mdn_session* s, mdn_constraint_report* out);
+
 /* ---- list every violated constraint, without proving: the census of mdn_check_constraints ----------------------
  * The same inputs, challenges, aux traces, external check, trace layouts and refusals as mdn_check_constraints; the row
  * pass keeps every (instance, row, constraint) whose value is non-zero instead of stopping at the first.
@@ -584,7 +613,8 @@ typedef struct {
     float lde_main, hash_main;          /* inside commit_main */
     /* per kernel class, summed over the last prove's launches (CUDA events on the session stream):
      * 0 transpose (or the ingest of column-major device traces), 1 NTT/LDE, 2 leaf sponge, 3 Merkle compress, 4 constraints, 5 OOD dot products,
-     * 6 DEEP quotient, 7 FRI (leaf+compress+fold), 8 PoW grind, 9 opening gather */
+     * 6 DEEP quotient, 7 FRI (leaf+compress+fold), 8 PoW grind, 9 opening gather.  The constraint guard's row check (and
+     * the re-derivation of the preprocessed rows it reads) is one more region of class 4 and is inside commit_aux. */
     float kernel_ms[10];
     unsigned kernel_regions[10];        /* timed regions per class */
     unsigned long long kernel_launches; /* kernels launched by the last prove */

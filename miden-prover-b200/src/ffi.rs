@@ -17,6 +17,8 @@ pub const MDN_ERR_UNSUPPORTED: c_int = -4;
 pub const MDN_ERR_AUX_BUILDER: c_int = -5;
 pub const MDN_ERR_NO_DEVICE: c_int = -6;
 pub const MDN_ERR_EXTERNAL_ASSERTION: c_int = -7;
+/// The constraint guard refused the proof (`mdn_session_set_constraint_guard`); `mdn_last_constraint_report` has the report.
+pub const MDN_ERR_CONSTRAINT_VIOLATED: c_int = -8;
 pub const MDN_FLAG_DEVICE_TRACES: u32 = 1;
 /// With `MDN_FLAG_DEVICE_TRACES` only: the device matrices are column-major, entry (r, c) at `values[(c << log_height) | r]`.
 pub const MDN_FLAG_COLUMN_MAJOR: u32 = 2;
@@ -399,6 +401,11 @@ unsafe extern "C" {
     ) -> c_int;
     pub fn mdn_session_set_shard(s: *mut MdnSession, rank: u32, world: u32, f: MdnAllgather, ctx: *mut c_void) -> c_int;
     pub fn mdn_session_set_external_check(s: *mut MdnSession, f: MdnExternalCheck, ctx: *mut c_void) -> c_int;
+    /// 1: every later proof checks every constraint on every row with the proof's own challenges and returns
+    /// `MDN_ERR_CONSTRAINT_VIOLATED` instead of proving a statement that does not hold; 0 (default): off.
+    pub fn mdn_session_set_constraint_guard(s: *mut MdnSession, enable: u32) -> c_int;
+    /// The report of the last guard run (`holds = 1`, `kind = 0` before any refusal and after a guard run that passed).
+    pub fn mdn_last_constraint_report(s: *const MdnSession, out: *mut MdnConstraintReport) -> c_int;
     pub fn mdn_session_set_device_aux_builder(s: *mut MdnSession, f: MdnAuxBuilderDevice, ctx: *mut c_void) -> c_int;
     pub fn mdn_session_set_hash(s: *mut MdnSession, kind: c_int) -> c_int;
     pub fn mdn_session_set_hash_challenger(s: *mut MdnSession, c: *const MdnHashChallenger) -> c_int;

@@ -163,8 +163,9 @@ EXPORTS = [
     "mdn_session_set_preprocessed", "mdn_session_set_jit", "mdn_jit_compile_check", "mdn_jit_status", "mdn_abi_layout",
     "mdn_session_set_external_check", "mdn_session_set_hash", "mdn_session_set_hash_challenger",
     "mdn_check_constraints", "mdn_session_set_device_aux_builder", "mdn_check_trace_balance",
-    "mdn_check_lookup_folds", "mdn_constraint_census",
+    "mdn_check_lookup_folds", "mdn_constraint_census", "mdn_session_set_constraint_guard", "mdn_last_constraint_report",
 ]
+ERR_CONSTRAINT_VIOLATED = -8
 
 _lib = None
 
@@ -234,6 +235,8 @@ def lib():
         L.mdn_abi_layout.restype = C.c_size_t
         L.mdn_abi_layout.argtypes = [u32p, C.c_size_t]
         L.mdn_session_set_jit.argtypes = [C.c_void_p, C.c_uint32]
+        L.mdn_session_set_constraint_guard.argtypes = [C.c_void_p, C.c_uint32]
+        L.mdn_last_constraint_report.argtypes = [C.c_void_p, C.POINTER(ConstraintReport)]
         L.mdn_jit_status.restype = C.c_char_p
         L.mdn_jit_status.argtypes = [C.c_void_p]
         L.mdn_jit_compile_check.restype = C.c_longlong
@@ -253,6 +256,14 @@ def ptr(a: np.ndarray):
 
 class ProverError(RuntimeError):
     """Mirrors `ExecutionError::ProvingError(String)` (reference prover/src/lib.rs:336-345)."""
+
+
+class ConstraintViolation(ProverError):
+    """The constraint guard refused the proof (MDN_ERR_CONSTRAINT_VIOLATED); `report` is its ConstraintReport."""
+
+    def __init__(self, message: str, report: "ConstraintReport"):
+        super().__init__(message)
+        self.report = report
 
 
 class Session:
@@ -276,6 +287,8 @@ class Session:
             pass
 
     def _check(self, rc):
+        if rc == ERR_CONSTRAINT_VIOLATED:
+            raise ConstraintViolation(f"[{rc}] {lib().mdn_last_error(self._h).decode()}", self.last_constraint_report())
         if rc != 0:
             raise ProverError(f"[{rc}] {lib().mdn_last_error(self._h).decode()}")
 
@@ -344,6 +357,19 @@ class Session:
     def set_jit(self, min_nodes: int):
         """Node threshold above which constraint programs are NVRTC-compiled (0 = interpreter only)."""
         self._check(lib().mdn_session_set_jit(self._h, min_nodes))
+
+    def set_constraint_guard(self, enable: bool):
+        """Check every constraint on every row inside each later proof, with the proof's own challenges, and refuse a
+        statement that does not hold with ConstraintViolation (mdn_session_set_constraint_guard)."""
+        self._check(lib().mdn_session_set_constraint_guard(self._h, 1 if enable else 0))
+
+    def last_constraint_report(self) -> ConstraintReport:
+        """The report of the last guard run (mdn_last_constraint_report)."""
+        rep = ConstraintReport()
+        rc = lib().mdn_last_constraint_report(self._h, C.byref(rep))
+        if rc != 0:
+            raise ProverError(f"[{rc}] {lib().mdn_last_error(self._h).decode()}")
+        return rep
 
     def jit_status(self) -> str:
         return lib().mdn_jit_status(self._h).decode()

@@ -180,9 +180,10 @@ struct AirHost {
     mk::AirDev dev;
     // lowered LookupAir (mdn_air.lookup): compiled program, raw periodic matrix, and the raw column-major main
     // trace kept from before the in-place inverse NTT (the LogUp fractions are evaluated on the trace domain):
-    // raw_main_cm points at the copy in raw_main, or at the caller's column-major device trace (MDN_FLAG_COLUMN_MAJOR)
+    // raw_main_cm points at the copy in raw_main, or at the caller's column-major device trace (MDN_FLAG_COLUMN_MAJOR).
+    // Under the constraint guard every AIR keeps its raw main trace, and raw_periodic holds its raw periodic matrix.
     bool has_lookup = false;
-    DevBuf lookup_program, raw_main;
+    DevBuf lookup_program, raw_main, raw_periodic;
     const u64* raw_main_cm = nullptr;
     mk::AirDev lookup_dev;
     // NVRTC-specialised constraint kernel (jit.hpp) for large programs; NULL = interpreter
@@ -251,6 +252,10 @@ struct mdn_session {
     }
     mdn_external_check external_check = nullptr; void* external_ctx = nullptr;   // Statement::eval_external (mdn_session_set_external_check)
     mdn_aux_builder_device dev_aux = nullptr; void* dev_aux_ctx = nullptr;        // mdn_session_set_device_aux_builder
+    // mdn_session_set_constraint_guard: every proof checks its rows before the aux commitment; guard_report is the
+    // report of the last guard run (mdn_last_constraint_report)
+    bool constraint_guard = false;
+    mdn_constraint_report guard_report{1, 0, 0, 0, 0, {0, 0}, 0};
     void shard_map_slab(char* base, size_t size);
     void shard_unmap_slabs();
     void shard_teardown();
@@ -311,6 +316,7 @@ struct mdn_session {
     NttPlan& ntt(u32 n);
     PremulPlan& premul_trace(u32 n);
     PremulPlan& premul_quotient(u32 n, u32 log_d);
+    PremulPlan& premul_unshifted(u32 n);
     void build_tree(Committed& c);
     void lde_matrix(CommittedMat& m);
     void keep_raw_main(u32 j, const u64* caller_cm);
@@ -340,6 +346,8 @@ struct mdn_session {
     };
     void prepare_check(const mdn_statement* st, const mdn_matrix* traces, const mdn_matrix* prep, const mdn_challenger* ch,
                        mdn_aux_builder build_aux, void* aux_ctx, u32 flags, CheckSetup& cs);
+    void check_rows(std::vector<mk::CheckArgs>& ca, bool locate, mdn_constraint_report* out);
+    void guard_constraints(const std::vector<u64>& flat_values);
     void constraint_census(const mdn_statement* st, const mdn_matrix* traces, const mdn_matrix* prep, const mdn_challenger* ch,
                            mdn_aux_builder build_aux, void* aux_ctx, u32 flags, mdn_constraint_failure* failures, u64 max_failures,
                            mdn_constraint_tally* tallies, u64 max_tallies, mdn_constraint_census_report* out);
@@ -423,6 +431,16 @@ PremulPlan& mdn_session::premul_quotient(u32 n, u32 log_d) {
     for (u32 t = 0; t < D; t++)
         for (u32 t2 = 0; t2 < B; t2++) bases[t * B + t2] = gl::mul(gl::pow(wji, t), gl::pow(wl, t2));
     auto plan = make_premul(bases, n, stream);
+    auto& ref = *plan;
+    premul_plans[key] = std::move(plan);
+    return ref;
+}
+// the one base 1: a forward NTT with it evaluates bit-reversed coefficients back on H, the rows of the trace
+PremulPlan& mdn_session::premul_unshifted(u32 n) {
+    auto key = std::make_pair(n, ~0u);
+    auto it = premul_plans.find(key);
+    if (it != premul_plans.end()) return *it->second;
+    auto plan = make_premul(std::vector<u64>{1}, n, stream);
     auto& ref = *plan;
     premul_plans[key] = std::move(plan);
     return ref;
@@ -931,6 +949,13 @@ void mdn_session::prove_begin(const mdn_statement* st, const mdn_matrix* traces,
 
     u32 k = st->n_airs;
     bind_airs(st, traces, true);
+    if (constraint_guard) for (u32 i = 0; i < k; i++) {   // the guard's raw periodic matrices (canonical: checked by bind_airs)
+        const mdn_air& a = st->airs[i];
+        if (!a.num_periodic_columns) continue;
+        size_t n = ((size_t)1 << a.log_max_period) * a.num_periodic_columns;
+        airs[i].raw_periodic.alloc(n, stream);
+        CUDA_OK(cudaMemcpyAsync(airs[i].raw_periodic.p, a.periodic_values, n * sizeof(u64), cudaMemcpyHostToDevice, stream));
+    }
     // preprocessed presence / shape parity (ProverInstance::new, prover/mod.rs:139-153; validate_preprocessed,
     // preprocessed.rs:147-260): a bundle must be installed exactly when some AIR declares preprocessed columns,
     // and each committed trace must have its AIR's declared width and its main trace's height
@@ -1265,11 +1290,12 @@ void mdn_session::set_preprocessed(const mdn_statement* st, const mdn_matrix* ma
     has_prep = true;
 }
 
-// the raw main trace of a LogUp AIR for its aux build: the caller's column-major device trace when there is one (read in
-// place: the caller keeps it unchanged until the aux commit), otherwise a copy made before the in-place inverse NTT
+// the raw main trace of a LogUp AIR for its aux build, and of every AIR for the constraint guard: the caller's
+// column-major device trace when there is one (read in place: the caller keeps it unchanged until the aux commit),
+// otherwise a copy made before the in-place inverse NTT
 void mdn_session::keep_raw_main(u32 j, const u64* caller_cm) {
     AirHost& h = airs[order[j]];
-    if (!h.has_lookup) return;
+    if (!h.has_lookup && !constraint_guard) return;
     if (caller_cm) { h.raw_main_cm = caller_cm; return; }
     CommittedMat& m = main_c.mats[j];
     size_t n = ((size_t)1 << m.log_n) * m.width;
@@ -1332,7 +1358,7 @@ void mdn_session::build_logup_aux(u32 j, const u64* main_cm, u64* aux_cm, u64 fi
     u32 flag = 0;
     CUDA_OK(cudaMemcpyAsync(&flag, d_flag.p, sizeof flag, cudaMemcpyDeviceToHost, stream));
     CUDA_OK(cudaStreamSynchronize(stream));
-    h.raw_main.release();
+    if (!constraint_guard) h.raw_main.release();   // the guard reads it after the build (commit_aux releases it)
     if (flag) {
         CUDA_OK(cudaMemsetAsync(d_flag.p, 0, 8, stream));
         if (flag & 2) fail(MDN_ERR_INVALID_ARG, "AIR %u: LogUp denominator must be non-zero", order[j]);   // aux_builder.rs:240-243
@@ -1370,11 +1396,6 @@ void mdn_session::check_constraints(const mdn_statement* st, const mdn_matrix* t
     const int ext_rc = cs.ext_rc;
     const u32 ext_failed = cs.ext_failed;
 
-    // row checks (debug.rs:120-214): per AIR the lowest (row, constraint) that is non-zero and the failing-row count
-    DevBuf res; res.alloc(2 * (size_t)k + 4, stream);
-    std::vector<u64> host_res(2 * (size_t)k + 4, 0);
-    for (u32 i = 0; i < k; i++) host_res[2 * i] = ~0ull;
-    CUDA_OK(cudaMemcpyAsync(res.p, host_res.data(), host_res.size() * sizeof(u64), cudaMemcpyHostToDevice, stream));
     std::vector<mk::CheckArgs> ca(k);
     for (u32 i = 0; i < k; i++) {
         u32 j = pos[i];
@@ -1388,7 +1409,26 @@ void mdn_session::check_constraints(const mdn_statement* st, const mdn_matrix* t
         c.prog = h.dev;
         c.prog.periodic = cs.periodic[i].p;
         c.publics = d_publics.p; c.challenges = d_randomness.p; c.aux_values = d_aux_values.p + aux_values_off[j];
-        c.row0 = 0; c.n_rows = (size_t)1 << log_heights[i];
+    }
+    check_rows(ca, ext_rc == 0, out);
+    if (ext_rc > 0) { out->kind = 2; out->constraint = ext_failed; }
+    out->holds = ext_rc == 0 && out->failing_rows == 0;
+}
+
+// The row pass (debug.rs:120-214) of check_constraints and of the constraint guard: k_check_rows on every row of every
+// AIR, instance order (ca[i]: AIR i's traces, program and leaves; the rows and result words are set here).  `out` gets
+// the failing-row total over all AIRs and, when `locate`, kind 1 with the least failing (instance, row, constraint)
+// and that constraint's value, from a one-row relaunch; every other field is zero.
+void mdn_session::check_rows(std::vector<mk::CheckArgs>& ca, bool locate, mdn_constraint_report* out) {
+    const u32 k = (u32)ca.size();
+    // per AIR the lowest (row, constraint) that is non-zero and the failing-row count
+    DevBuf res; res.alloc(2 * (size_t)k + 4, stream);
+    std::vector<u64> host_res(2 * (size_t)k + 4, 0);
+    for (u32 i = 0; i < k; i++) host_res[2 * i] = ~0ull;
+    CUDA_OK(cudaMemcpyAsync(res.p, host_res.data(), host_res.size() * sizeof(u64), cudaMemcpyHostToDevice, stream));
+    for (u32 i = 0; i < k; i++) {
+        mk::CheckArgs& c = ca[i];
+        c.row0 = 0; c.n_rows = (size_t)1 << c.log_n;
         c.first = (unsigned long long*)(res.p + 2 * i); c.failing_rows = (unsigned long long*)(res.p + 2 * i + 1);
         if (mk::launch_check_rows(c, stream) != 0) fail(MDN_ERR_UNSUPPORTED, "AIR %u: constraint program too large for the interpreter", i);
     }
@@ -1398,8 +1438,7 @@ void mdn_session::check_constraints(const mdn_statement* st, const mdn_matrix* t
 
     memset(out, 0, sizeof *out);
     for (u32 i = 0; i < k; i++) out->failing_rows += host_res[2 * i + 1];
-    if (ext_rc > 0) { out->kind = 2; out->constraint = ext_failed; }
-    else for (u32 i = 0; i < k; i++) {
+    if (locate) for (u32 i = 0; i < k; i++) {
         u64 f = host_res[2 * i];
         if (f == ~0ull) continue;
         out->kind = 1; out->instance = i; out->row = f >> 32; out->constraint = (u32)f;
@@ -1412,7 +1451,53 @@ void mdn_session::check_constraints(const mdn_statement* st, const mdn_matrix* t
         CUDA_OK(cudaStreamSynchronize(stream));
         break;
     }
-    out->holds = ext_rc == 0 && out->failing_rows == 0;
+}
+
+// The constraint guard (mdn_session_set_constraint_guard), from commit_aux once the aux traces and values are final and
+// the external assertions hold, before the aux commitment: the row pass of check_constraints on what this proof is about
+// to commit.  Main rows: the raw copies of keep_raw_main (or the caller's column-major traces); aux rows: aux_c's
+// coefficient slots, still raw; `flat_values`: the aux values in proof order; challenges and publics: the proof's own.
+// Preprocessed rows are re-derived from the bundle's coefficients by a forward NTT with shift 1 -- exact, and the
+// bundle needs no raw copy whenever the guard was turned on.  Every rank of a split proof runs the whole check on its
+// own whole copies.  A non-zero constraint fails the proof with MDN_ERR_CONSTRAINT_VIOLATED.
+void mdn_session::guard_constraints(const std::vector<u64>& flat_values) {
+    const u32 k = (u32)airs.size();
+    ProfScope ps(prof, PC_CONSTRAINTS);
+    DevBuf values; values.alloc(std::max<size_t>(1, flat_values.size()), stream);
+    if (!flat_values.empty()) CUDA_OK(cudaMemcpyAsync(values.p, flat_values.data(), flat_values.size() * sizeof(u64), cudaMemcpyHostToDevice, stream));
+    std::vector<DevBuf> prep_rows(k);
+    std::vector<mk::CheckArgs> ca(k);
+    for (u32 j = 0; j < k; j++) {
+        const u32 i = order[j];
+        AirHost& h = airs[i];
+        const size_t N = (size_t)1 << log_heights[i];
+        if (h.desc.preprocessed_width) {
+            const u32 q = (u32)(std::find(prep_air.begin(), prep_air.end(), i) - prep_air.begin());   // present: checked by prove_begin
+            const CommittedMat& pm = prep_c.mats[q];
+            prep_rows[i].alloc(N * pm.width, stream);
+            std::vector<mk::FwdItem> items;
+            for (u32 c = 0; c < pm.width; c++) items.push_back(mk::FwdItem{pm.coef + (size_t)c * N, prep_rows[i].p + (size_t)c * N, 0, 0});
+            DevBuf d_items; d_items.alloc(items.size() * sizeof(mk::FwdItem) / sizeof(u64), stream);
+            CUDA_OK(cudaMemcpyAsync(d_items.p, items.data(), items.size() * sizeof(mk::FwdItem), cudaMemcpyHostToDevice, stream));
+            mk::launch_fwd_ntt((const mk::FwdItem*)d_items.p, pm.width, ntt(pm.log_n).T, premul_unshifted(pm.log_n).P, stream);
+        }
+        mk::CheckArgs& c = ca[i];
+        c = mk::CheckArgs{};
+        c.main_cm = h.raw_main_cm;
+        c.aux_cm = h.desc.aux_width ? aux_c.mats[j].coef : nullptr;
+        c.prep_cm = prep_rows[i].p;
+        c.log_n = log_heights[i];
+        c.prog = h.dev;
+        c.prog.periodic = h.raw_periodic.p;
+        c.publics = d_publics.p; c.challenges = d_randomness.p; c.aux_values = values.p + aux_values_off[j];
+    }
+    mdn_constraint_report rep;
+    check_rows(ca, true, &rep);
+    rep.holds = rep.failing_rows == 0;
+    guard_report = rep;
+    if (!rep.holds)
+        fail(MDN_ERR_CONSTRAINT_VIOLATED, "constraint %u of AIR %u is non-zero at row %llu (%llu failing rows): the statement does not hold, nothing was committed",
+             rep.constraint, rep.instance, (unsigned long long)rep.row, (unsigned long long)rep.failing_rows);
 }
 
 // Validation, challenges, main / preprocessed / periodic upload, aux traces and the external check of a constraint
@@ -2200,6 +2285,10 @@ void mdn_session::commit_aux(const mdn_matrix* aux, const u64* const* aux_values
         int rc = eval_external(&failed);
         if (rc > 0) fail(MDN_ERR_EXTERNAL_ASSERTION, "external assertion %u failed", failed);
         if (rc < 0) fail(MDN_ERR_EXTERNAL_ASSERTION, "eval_external reported a reduction error");
+    }
+    if (constraint_guard) {
+        guard_constraints(flat_values);
+        for (AirHost& h : airs) h.raw_main.release();
     }
     lde_and_commit(aux_c, nullptr, nullptr);
     tr.send_commitment(aux_c.root);
@@ -3165,6 +3254,20 @@ int mdn_session_set_hash_challenger(mdn_session* s, const mdn_hash_challenger* c
 int mdn_session_set_external_check(mdn_session* s, mdn_external_check fn, void* ctx) {
     if (!s) return MDN_ERR_INVALID_ARG;
     s->external_check = fn; s->external_ctx = ctx;
+    return MDN_OK;
+}
+
+int mdn_session_set_constraint_guard(mdn_session* s, uint32_t enable) {
+    if (!s) return MDN_ERR_INVALID_ARG;
+    if (enable > 1) { s->error = "mdn_session_set_constraint_guard: enable must be 0 or 1"; return MDN_ERR_INVALID_ARG; }
+    if (s->in_proof) { s->error = "mdn_session_set_constraint_guard called inside a proof (between mdn_prove_begin and mdn_prove_finish)"; return MDN_ERR_INVALID_ARG; }
+    s->constraint_guard = enable == 1;
+    return MDN_OK;
+}
+
+int mdn_last_constraint_report(const mdn_session* s, mdn_constraint_report* out) {
+    if (!s || !out) return MDN_ERR_INVALID_ARG;
+    *out = s->guard_report;
     return MDN_OK;
 }
 

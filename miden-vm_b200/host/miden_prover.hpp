@@ -43,8 +43,10 @@ using QuadFelt = std::array<Felt, 2>;        // (c0, c1) of F[u]/(u^2 - 7)
 using Commitment = std::array<Felt, 4>;      // Hash<Felt, Felt, 4>
 
 struct ProverError : std::runtime_error {
-    enum Kind { Instance, Domain, Cuda, Unsupported, AuxBuilder, NoDevice, ExternalAssertion } kind;
+    enum Kind { Instance, Domain, Cuda, Unsupported, AuxBuilder, NoDevice, ExternalAssertion, ConstraintViolated } kind;
+    mdn_constraint_report report{};   // ConstraintViolated: the constraint guard's report (mdn_last_constraint_report)
     ProverError(Kind k, const std::string& m) : std::runtime_error(m), kind(k) {}
+    ProverError(Kind k, const std::string& m, const mdn_constraint_report& r) : std::runtime_error(m), kind(k), report(r) {}
     static Kind from_status(int rc) {
         switch (rc) {
             case MDN_ERR_DOMAIN: return Domain;
@@ -53,6 +55,7 @@ struct ProverError : std::runtime_error {
             case MDN_ERR_AUX_BUILDER: return AuxBuilder;
             case MDN_ERR_NO_DEVICE: return NoDevice;
             case MDN_ERR_EXTERNAL_ASSERTION: return ExternalAssertion;
+            case MDN_ERR_CONSTRAINT_VIOLATED: return ConstraintViolated;
             default: return Instance;
         }
     }
@@ -209,6 +212,13 @@ public:
         hash_ = h;
         return *this;
     }
+    // refuse to prove a statement that does not hold (mdn_session_set_constraint_guard): prove_stark then throws
+    // ProverError::ConstraintViolated with the guard's report instead of returning a proof no verifier accepts
+    StarkConfig& with_constraint_guard(bool enable) {
+        int rc = mdn_session_set_constraint_guard(session_.get(), enable ? 1 : 0);
+        if (rc != MDN_OK) throw ProverError(ProverError::from_status(rc), mdn_last_error(session_.get()));
+        return *this;
+    }
     HashFunction hash() const { return hash_; }
     bool hash_challenger() const { return hash_ == HashFunction::Blake3_256 || hash_ == HashFunction::Keccak; }
     const PcsParams& pcs() const { return params_; }
@@ -253,6 +263,11 @@ struct Lowered {                                   // C structs pointing into a 
     }
 };
 inline void check(const StarkConfig& c, int rc) {
+    if (rc == MDN_ERR_CONSTRAINT_VIOLATED) {
+        mdn_constraint_report r{};
+        mdn_last_constraint_report(c.session(), &r);
+        throw ProverError(ProverError::ConstraintViolated, mdn_last_error(c.session()), r);
+    }
     if (rc != MDN_OK) throw ProverError(ProverError::from_status(rc), mdn_last_error(c.session()));
 }
 // the mdn_aux_builder seam over an AuxBuilder
