@@ -336,6 +336,28 @@ struct mdn_session {
     void bind_challenger(const mdn_challenger* ch);
     void upload_and_commit_main(const mdn_matrix* traces, bool on_device);
     int eval_external(u32* failed);
+    // what every trace check starts with (start_check) and the pieces its callers share
+    struct CheckStart { bool cm, on_device; u32 k; };
+    CheckStart start_check(const mdn_statement* st, const mdn_matrix* traces, const mdn_challenger* ch, u32 flags, const void* out);
+    std::vector<u64*> stage_main(const mdn_matrix* traces, const std::vector<u32>& insts, bool cm, bool on_device);
+    u32 check_randomness(const u64* rnd);
+    void upload_leaves(const u64* rnd, size_t n_words);
+    void alloc_checked(const std::string& what, std::initializer_list<std::pair<DevBuf*, size_t>> bufs);
+    bool lookup_air(u32 i, const char* given, u32& skipped);
+    // the row program's inputs of AIR i (proof position j) for k_check_rows and k_census_rows, whose argument structs
+    // name them alike; `values`: the aux values in proof order
+    template <class Args> Args row_args(u32 i, u32 j, const u64* main_cm, const u64* prep_cm, const u64* periodic, const u64* values) const {
+        const AirHost& h = airs[i];
+        Args c{};
+        c.main_cm = main_cm;
+        c.aux_cm = h.desc.aux_width ? aux_c.mats[j].coef : nullptr;
+        c.prep_cm = prep_cm;
+        c.log_n = log_heights[i];
+        c.prog = h.dev;
+        c.prog.periodic = periodic;
+        c.publics = d_publics.p; c.challenges = d_randomness.p; c.aux_values = values + aux_values_off[j];
+        return c;
+    }
     void check_constraints(const mdn_statement* st, const mdn_matrix* traces, const mdn_matrix* prep, const mdn_challenger* ch,
                            mdn_aux_builder build_aux, void* aux_ctx, u32 flags, mdn_constraint_report* out);
     // what prepare_check leaves per instance for the row pass of check_constraints / constraint_census
@@ -345,7 +367,7 @@ struct mdn_session {
         int ext_rc = 0; u32 ext_failed = 0;      // the external check: > 0 with ext_failed = the failing assertion
     };
     void prepare_check(const mdn_statement* st, const mdn_matrix* traces, const mdn_matrix* prep, const mdn_challenger* ch,
-                       mdn_aux_builder build_aux, void* aux_ctx, u32 flags, CheckSetup& cs);
+                       mdn_aux_builder build_aux, void* aux_ctx, u32 flags, const void* out, CheckSetup& cs);
     void check_rows(std::vector<mk::CheckArgs>& ca, bool locate, mdn_constraint_report* out);
     void guard_constraints(const std::vector<u64>& flat_values);
     void constraint_census(const mdn_statement* st, const mdn_matrix* traces, const mdn_matrix* prep, const mdn_challenger* ch,
@@ -933,7 +955,6 @@ void mdn_session::prove_begin(const mdn_statement* st, const mdn_matrix* traces,
     memset(&timings, 0, sizeof timings);
     mk::reset_launch_count();
     prof.st = stream; prof.reset(); leaf_bytes = ntt_bytes = 0; perms = 0;
-    if (!d_flag.p) { ArenaScope persistent(nullptr); d_flag.alloc(1, stream); CUDA_OK(cudaMemsetAsync(d_flag.p, 0, 8, stream)); }
     validate_statement(st, traces, chal);
     if (cm) for (u32 i = 0; i < st->n_airs; i++) check_column_major(traces[i], "trace", i);
     col_major = cm;
@@ -1261,7 +1282,6 @@ void mdn_session::set_preprocessed(const mdn_statement* st, const mdn_matrix* ma
     if (!st) fail(MDN_ERR_INVALID_ARG, "null argument");
     u32 lb = params.log_blowup;
     if (lb == 0 || lb > 4) fail(MDN_ERR_UNSUPPORTED, "log_blowup must be in 1..=4");
-    if (!d_flag.p) { ArenaScope persistent(nullptr); d_flag.alloc(1, stream); CUDA_OK(cudaMemsetAsync(d_flag.p, 0, 8, stream)); }
     std::vector<u32> ids;
     for (u32 i = 0; i < st->n_airs; i++) {
         if (mats[i].width != st->airs[i].preprocessed_width) fail(MDN_ERR_INVALID_ARG, "AIR %u: preprocessed matrix width %u does not match the declared %u", i, mats[i].width, st->airs[i].preprocessed_width);
@@ -1379,6 +1399,105 @@ int mdn_session::eval_external(u32* failed) {
 }
 
 // ---------------------------------------------------------------------------------------------
+// the trace checks' shared host steps
+// ---------------------------------------------------------------------------------------------
+namespace {
+const mdn_challenger no_challenger{};   // for the checks that take their challenges as an argument: nothing is observed
+
+// the interaction items {column, flag node, multiplicity, denominator} of a lowered lookup program (compiled by
+// bind_airs, so the header and the items are in range)
+struct LookupItems {
+    const u32* items; u32 n;
+    explicit LookupItems(const mdn_lookup& lk) : items(lk.program + 5 + 3 * (size_t)lk.program[2]), n(lk.program[3]) {}
+    u32 column(u32 q) const { return items[4 * (size_t)q]; }
+    u32 flag(u32 q) const { return items[4 * (size_t)q + 1]; }
+};
+}  // namespace
+
+// The start of a trace check: a fresh proof state, the statement validated (`chal` NULL-checked as mdn_prove does;
+// &no_challenger when nothing is observed) and its AIRs compiled.  The caller validates what it takes besides and then
+// calls bind_order, in that order: the order of the errors a call reports is part of its behaviour.
+mdn_session::CheckStart mdn_session::start_check(const mdn_statement* st, const mdn_matrix* traces, const mdn_challenger* chal, u32 flags, const void* out) {
+    const bool cm = column_major(flags);
+    reset_proof();
+    prof.st = stream; prof.reset();
+    if (!out) fail(MDN_ERR_INVALID_ARG, "null argument");
+    validate_statement(st, traces, chal);
+    if (cm) for (u32 i = 0; i < st->n_airs; i++) check_column_major(traces[i], "trace", i);
+    bind_airs(st, traces, false);
+    return CheckStart{cm, (flags & MDN_FLAG_DEVICE_TRACES) != 0, st->n_airs};
+}
+
+// Raw main traces of the instances `insts`, column-major, laid out in that order in main_c.coef_buf; column-major
+// device traces are read where the caller keeps them (only read: the const_cast feeds the common pointer type).
+// Returns each instance's trace, NULL for the instances not staged.
+std::vector<u64*> mdn_session::stage_main(const mdn_matrix* traces, const std::vector<u32>& insts, bool cm, bool on_device) {
+    std::vector<u64*> main_cm(airs.size(), nullptr);
+    size_t total = 0;
+    if (!cm) for (u32 i : insts) total += ((size_t)1 << log_heights[i]) * airs[i].desc.width;
+    main_c.coef_buf.alloc(total, stream);
+    size_t co = 0;
+    for (u32 i : insts) {
+        main_cm[i] = cm ? const_cast<u64*>(traces[i].values) : main_c.coef_buf.p + co;
+        if (!cm) co += ((size_t)1 << log_heights[i]) * airs[i].desc.width;
+    }
+    for (u32 i : insts) upload_matrix(traces[i], on_device, main_cm[i], cm);   // column-major: check only
+    check_input_flag("a main trace");
+    return main_cm;
+}
+
+// challenges given as an argument (2 words per extension element): as many as the AIRs draw, canonical
+u32 mdn_session::check_randomness(const u64* rnd) {
+    u32 max_rand = 0;
+    for (auto& a : airs) max_rand = std::max(max_rand, a.desc.num_randomness);
+    if (max_rand && !rnd) fail(MDN_ERR_INVALID_ARG, "randomness is NULL");
+    for (u32 i = 0; i < 2 * max_rand; i++) if (rnd[i] >= gl::P) fail(MDN_ERR_INVALID_ARG, "randomness word %u is not a canonical field element (>= p)", i);
+    return max_rand;
+}
+
+// device copies of the public values and of the challenges (n_words words), read by the lookup and constraint kernels
+void mdn_session::upload_leaves(const u64* rnd, size_t n_words) {
+    d_publics.alloc(std::max<size_t>(1, publics.size()), stream);
+    if (!publics.empty()) CUDA_OK(cudaMemcpyAsync(d_publics.p, publics.data(), publics.size() * sizeof(u64), cudaMemcpyHostToDevice, stream));
+    d_randomness.alloc(std::max<size_t>(1, n_words), stream);
+    if (n_words) CUDA_OK(cudaMemcpyAsync(d_randomness.p, rnd, n_words * sizeof(u64), cudaMemcpyHostToDevice, stream));
+}
+
+// Allocates buffers whose size depends on the data (each with its word count), refusing with MDN_ERR_UNSUPPORTED and
+// "<what> <GiB> of device memory: <why>" when the device's and the arena's free memory cannot hold them, or when an
+// allocation fails.
+void mdn_session::alloc_checked(const std::string& what, std::initializer_list<std::pair<DevBuf*, size_t>> bufs) {
+    size_t need = 0;
+    for (auto& b : bufs) need += b.second * sizeof(u64);
+    auto too_large = [&](const char* why) {
+        fail(MDN_ERR_UNSUPPORTED, "%s %.1f GiB of device memory: %s", what.c_str(), need / 1073741824.0, why);
+    };
+#ifndef MDN_EMULATED   // tests/emu has no device memory of its own: only the failed allocation below is reported there
+    size_t arena_b = 0, free_b = 0, total_b = 0;
+    for (auto& sl : arena.slabs) arena_b += sl.size - sl.used;
+    CUDA_OK(cudaMemGetInfo(&free_b, &total_b));
+    char msg[64];
+    snprintf(msg, sizeof msg, "%.1f GiB are free", (free_b + arena_b) / 1073741824.0);
+    if (need > free_b + arena_b) too_large(msg);
+#endif
+    try {
+        for (auto& b : bufs) b.first->alloc(b.second, stream);
+    } catch (const MdnError&) {   // an out-of-memory allocation leaves no error behind; nothing has been launched on them yet
+        cudaGetLastError();
+        too_large("the allocation failed");
+    }
+}
+
+// Whether AIR i has a lowered lookup program, which the lookup checks run.  An AIR without one counts in `skipped`,
+// and `given` -- a per-AIR argument of the check given for it, or NULL -- is refused.
+bool mdn_session::lookup_air(u32 i, const char* given, u32& skipped) {
+    if (airs[i].has_lookup) return true;
+    skipped++;
+    if (given) fail(MDN_ERR_INVALID_ARG, "AIR %u: %s given for an AIR without a lookup program", i, given);
+    return false;
+}
+
+// ---------------------------------------------------------------------------------------------
 // check_constraints: every constraint of every AIR on every trace row, without a proof  (debug.rs:70-214)
 // ---------------------------------------------------------------------------------------------
 // The validation, program compilation and main-trace upload of prove_begin; challenges from the statement felts and
@@ -1390,29 +1509,16 @@ void mdn_session::check_constraints(const mdn_statement* st, const mdn_matrix* t
                                     mdn_aux_builder build_aux, void* aux_ctx, u32 flags, mdn_constraint_report* out) {
     if (!out) fail(MDN_ERR_INVALID_ARG, "null argument");
     CheckSetup cs;
-    prepare_check(st, traces, prep, chal, build_aux, aux_ctx, flags, cs);
+    prepare_check(st, traces, prep, chal, build_aux, aux_ctx, flags, out, cs);
     const u32 k = st->n_airs;
-    const std::vector<u32>& pos = cs.pos;
-    const int ext_rc = cs.ext_rc;
-    const u32 ext_failed = cs.ext_failed;
-
     std::vector<mk::CheckArgs> ca(k);
     for (u32 i = 0; i < k; i++) {
-        u32 j = pos[i];
-        AirHost& h = airs[i];
-        mk::CheckArgs& c = ca[i];
-        c = mk::CheckArgs{};
-        c.main_cm = main_c.mats[j].coef;
-        c.aux_cm = h.desc.aux_width ? aux_c.mats[j].coef : nullptr;
-        c.prep_cm = cs.prep_cm[i].p;
-        c.log_n = log_heights[i];
-        c.prog = h.dev;
-        c.prog.periodic = cs.periodic[i].p;
-        c.publics = d_publics.p; c.challenges = d_randomness.p; c.aux_values = d_aux_values.p + aux_values_off[j];
+        const u32 j = cs.pos[i];
+        ca[i] = row_args<mk::CheckArgs>(i, j, main_c.mats[j].coef, cs.prep_cm[i].p, cs.periodic[i].p, d_aux_values.p);
     }
-    check_rows(ca, ext_rc == 0, out);
-    if (ext_rc > 0) { out->kind = 2; out->constraint = ext_failed; }
-    out->holds = ext_rc == 0 && out->failing_rows == 0;
+    check_rows(ca, cs.ext_rc == 0, out);
+    if (cs.ext_rc > 0) { out->kind = 2; out->constraint = cs.ext_failed; }
+    out->holds = cs.ext_rc == 0 && out->failing_rows == 0;
 }
 
 // The row pass (debug.rs:120-214) of check_constraints and of the constraint guard: k_check_rows on every row of every
@@ -1481,15 +1587,7 @@ void mdn_session::guard_constraints(const std::vector<u64>& flat_values) {
             CUDA_OK(cudaMemcpyAsync(d_items.p, items.data(), items.size() * sizeof(mk::FwdItem), cudaMemcpyHostToDevice, stream));
             mk::launch_fwd_ntt((const mk::FwdItem*)d_items.p, pm.width, ntt(pm.log_n).T, premul_unshifted(pm.log_n).P, stream);
         }
-        mk::CheckArgs& c = ca[i];
-        c = mk::CheckArgs{};
-        c.main_cm = h.raw_main_cm;
-        c.aux_cm = h.desc.aux_width ? aux_c.mats[j].coef : nullptr;
-        c.prep_cm = prep_rows[i].p;
-        c.log_n = log_heights[i];
-        c.prog = h.dev;
-        c.prog.periodic = h.raw_periodic.p;
-        c.publics = d_publics.p; c.challenges = d_randomness.p; c.aux_values = values.p + aux_values_off[j];
+        ca[i] = row_args<mk::CheckArgs>(i, j, h.raw_main_cm, prep_rows[i].p, h.raw_periodic.p, values.p);
     }
     mdn_constraint_report rep;
     check_rows(ca, true, &rep);
@@ -1505,17 +1603,9 @@ void mdn_session::guard_constraints(const std::vector<u64>& flat_values) {
 // d_publics / d_randomness / d_aux_values the leaves, and cs the per-instance preprocessed and periodic buffers and
 // the external check's outcome.
 void mdn_session::prepare_check(const mdn_statement* st, const mdn_matrix* traces, const mdn_matrix* prep, const mdn_challenger* chal,
-                                mdn_aux_builder build_aux, void* aux_ctx, u32 flags, CheckSetup& cs) {
-    const bool cm = column_major(flags);
-    reset_proof();
-    prof.st = stream; prof.reset();
-    if (!d_flag.p) { ArenaScope persistent(nullptr); d_flag.alloc(1, stream); CUDA_OK(cudaMemsetAsync(d_flag.p, 0, 8, stream)); }
-    validate_statement(st, traces, chal);
-    if (cm) for (u32 i = 0; i < st->n_airs; i++) check_column_major(traces[i], "trace", i);
-    const bool on_device = (flags & MDN_FLAG_DEVICE_TRACES) != 0;
+                                mdn_aux_builder build_aux, void* aux_ctx, u32 flags, const void* out, CheckSetup& cs) {
+    const auto [cm, on_device, k] = start_check(st, traces, chal, flags, out);
     const bool dev_built = cm && dev_aux;   // aux traces from the device aux builder
-    const u32 k = st->n_airs;
-    bind_airs(st, traces, false);
     // the preprocessed traces come with the call (debug.rs re-materialises BaseAir::preprocessed_trace), not from the
     // session's committed bundle
     bool expected = false;
@@ -1540,30 +1630,21 @@ void mdn_session::prepare_check(const mdn_statement* st, const mdn_matrix* trace
     for (auto& a : airs) max_rand = std::max(max_rand, a.desc.num_randomness);
     for (u32 i = 0; i < max_rand; i++) randomness.push_back(tr.ch.sample_ext());
 
-    // raw main traces, column-major, proof order (the layout build_logup_aux reads); column-major device traces are
-    // read where the caller keeps them (only read: the const_cast feeds the common CommittedMat)
+    // raw main and aux traces, column-major, proof order (the layout build_logup_aux reads)
     std::vector<u32>& pos = cs.pos;
     pos.assign(k, 0);
-    size_t main_total = 0, aux_total = 0;
-    for (u32 j = 0; j < k; j++) {
-        u32 inst = order[j];
-        pos[inst] = j;
-        size_t N = (size_t)1 << log_heights[inst];
-        main_total += N * airs[inst].desc.width; aux_total += N * 2 * airs[inst].desc.aux_width;
-    }
-    if (!cm) main_c.coef_buf.alloc(main_total, stream);
+    for (u32 j = 0; j < k; j++) pos[order[j]] = j;
+    const std::vector<u64*> main_cm = stage_main(traces, order, cm, on_device);
+    size_t aux_total = 0;
+    for (u32 i = 0; i < k; i++) aux_total += ((size_t)1 << log_heights[i]) * 2 * airs[i].desc.aux_width;
     aux_c.coef_buf.alloc(aux_total, stream);
-    size_t co = 0, ao = 0;
+    size_t ao = 0;
     for (u32 j = 0; j < k; j++) {
         u32 inst = order[j];
-        size_t N = (size_t)1 << log_heights[inst];
-        u64* main_cm = cm ? const_cast<u64*>(traces[inst].values) : main_c.coef_buf.p + co;
-        main_c.mats.push_back(CommittedMat{nullptr, main_cm, log_heights[inst], airs[inst].desc.width});
+        main_c.mats.push_back(CommittedMat{nullptr, main_cm[inst], log_heights[inst], airs[inst].desc.width});
         aux_c.mats.push_back(CommittedMat{nullptr, aux_c.coef_buf.p + ao, log_heights[inst], 2 * airs[inst].desc.aux_width});
-        co += N * airs[inst].desc.width; ao += N * 2 * airs[inst].desc.aux_width;
+        ao += ((size_t)1 << log_heights[inst]) * 2 * airs[inst].desc.aux_width;
     }
-    for (u32 j = 0; j < k; j++) upload_matrix(traces[order[j]], on_device, main_c.mats[j].coef, cm);   // column-major: check only
-    check_input_flag("a main trace");
     std::vector<DevBuf>& prep_cm = cs.prep_cm;
     std::vector<DevBuf>& periodic = cs.periodic;
     prep_cm.clear(); prep_cm.resize(k);
@@ -1598,10 +1679,7 @@ void mdn_session::prepare_check(const mdn_statement* st, const mdn_matrix* trace
     }
     if (dev_built) for (u32 i = 0; i < k; i++)
         if (!st->airs[i].lookup) call_device_aux_builder(i, traces[i], aux_c.mats[pos[i]].coef, val_host[i]);
-    d_publics.alloc(std::max<size_t>(1, publics.size()), stream);
-    if (!publics.empty()) CUDA_OK(cudaMemcpyAsync(d_publics.p, publics.data(), publics.size() * sizeof(u64), cudaMemcpyHostToDevice, stream));
-    d_randomness.alloc(std::max<size_t>(1, 2 * randomness.size()), stream);
-    if (!randomness.empty()) CUDA_OK(cudaMemcpyAsync(d_randomness.p, randomness.data(), randomness.size() * sizeof(E2), cudaMemcpyHostToDevice, stream));
+    upload_leaves((const u64*)randomness.data(), 2 * randomness.size());
     std::vector<u64> flat_values;
     aux_values_p.assign(k, {}); aux_values_off.assign(k, 0);
     for (u32 j = 0; j < k; j++) {
@@ -1644,7 +1722,7 @@ void mdn_session::constraint_census(const mdn_statement* st, const mdn_matrix* t
                                     mdn_aux_builder build_aux, void* aux_ctx, u32 flags, mdn_constraint_failure* failures, u64 max_failures,
                                     mdn_constraint_tally* tallies, u64 max_tallies, mdn_constraint_census_report* out) {
     CheckSetup cs;
-    prepare_check(st, traces, prep, chal, build_aux, aux_ctx, flags, cs);
+    prepare_check(st, traces, prep, chal, build_aux, aux_ctx, flags, out, cs);
     const u32 k = st->n_airs;
 
     // per-row counts of all AIRs (u32, instance order), their offsets, one tally table per AIR, two counters
@@ -1667,18 +1745,10 @@ void mdn_session::constraint_census(const mdn_statement* st, const mdn_matrix* t
     u32* d_counts = reinterpret_cast<u32*>(counts.p);
     std::vector<mk::CensusArgs> ca(k);
     for (u32 i = 0; i < k; i++) {
-        u32 j = cs.pos[i];
-        AirHost& h = airs[i];
+        const u32 j = cs.pos[i];
         mk::CensusArgs& c = ca[i];
-        c = mk::CensusArgs{};
-        c.main_cm = main_c.mats[j].coef;
-        c.aux_cm = h.desc.aux_width ? aux_c.mats[j].coef : nullptr;
-        c.prep_cm = cs.prep_cm[i].p;
-        c.log_n = log_heights[i];
-        c.prog = h.dev;
-        c.prog.periodic = cs.periodic[i].p;
-        c.publics = d_publics.p; c.challenges = d_randomness.p; c.aux_values = d_aux_values.p + aux_values_off[j];
-        c.n_cons = h.n_constraints;
+        c = row_args<mk::CensusArgs>(i, j, main_c.mats[j].coef, cs.prep_cm[i].p, cs.periodic[i].p, d_aux_values.p);
+        c.n_cons = airs[i].n_constraints;
         c.instance = i;
         c.row_count = d_counts + row_base[i];
         c.tally = (unsigned long long*)(tally.p + tally_base[i]);
@@ -1767,30 +1837,18 @@ void mdn_session::constraint_census(const mdn_statement* st, const mdn_matrix* t
 // ---------------------------------------------------------------------------------------------
 // check_trace_balance: every active LogUp push keyed by its denominator, without a proof  (debug/trace/mod.rs:169-309)
 // ---------------------------------------------------------------------------------------------
-// The validation, program compilation and main-trace upload of check_constraints; the challenges are an argument.  Per
-// AIR with a lowered lookup program, k_balance_rows counts the pushes (which sizes the table), then inserts them; the
-// boundary triples follow; k_balance_finish reduces every sum and compacts the unmatched denominators; when the report
-// can hold them, a third row pass collects their pushes.  The host sorts what is reported.
+// start_check, then the main traces of the lookup AIRs staged; the challenges are an argument.  Per AIR with a lowered
+// lookup program, k_balance_rows counts the pushes (which sizes the table), then inserts them; the boundary triples
+// follow; k_balance_finish reduces every sum and compacts the unmatched denominators; when the report can hold them, a
+// third row pass collects their pushes.  The host sorts what is reported.
 void mdn_session::check_trace_balance(const mdn_statement* st, const mdn_matrix* traces, const u64* rnd, const u64* boundary, size_t n_boundary,
                                       const uint32_t* const* mutex_sites, u64 max_contrib, u32 flags, mdn_balance_report* out) {
-    const bool cm = column_major(flags);
-    reset_proof();
-    prof.st = stream; prof.reset();
-    if (!d_flag.p) { ArenaScope persistent(nullptr); d_flag.alloc(1, stream); CUDA_OK(cudaMemsetAsync(d_flag.p, 0, 8, stream)); }
-    if (!out) fail(MDN_ERR_INVALID_ARG, "null argument");
-    const mdn_challenger no_challenger{};   // nothing is observed: validate_statement only checks the statement
-    validate_statement(st, traces, &no_challenger);
-    if (cm) for (u32 i = 0; i < st->n_airs; i++) check_column_major(traces[i], "trace", i);
-    const bool on_device = (flags & MDN_FLAG_DEVICE_TRACES) != 0;
-    const u32 k = st->n_airs;
-    bind_airs(st, traces, false);
+    const CheckStart start = start_check(st, traces, &no_challenger, flags, out);
+    const u32 k = start.k;
     bind_order(st, false);
 
     // arguments: challenges, boundary emissions, interaction counts, mutex annotations
-    u32 max_rand = 0;
-    for (auto& a : airs) max_rand = std::max(max_rand, a.desc.num_randomness);
-    if (max_rand && !rnd) fail(MDN_ERR_INVALID_ARG, "randomness is NULL");
-    for (u32 i = 0; i < 2 * max_rand; i++) if (rnd[i] >= gl::P) fail(MDN_ERR_INVALID_ARG, "randomness word %u is not a canonical field element (>= p)", i);
+    const u32 max_rand = check_randomness(rnd);
     if (n_boundary && !boundary) fail(MDN_ERR_INVALID_ARG, "boundary is NULL");
     if (n_boundary >= (1u << 24)) fail(MDN_ERR_UNSUPPORTED, "at most 2^24 - 1 boundary emissions");
     for (size_t q = 0; q < 3 * n_boundary; q++)
@@ -1800,50 +1858,30 @@ void mdn_session::check_trace_balance(const mdn_statement* st, const mdn_matrix*
     u32 skipped = 0;
     for (u32 i = 0; i < k; i++) {
         const uint32_t* ann = mutex_sites ? mutex_sites[i] : nullptr;
-        if (!airs[i].has_lookup) {
-            skipped++;
-            if (ann) fail(MDN_ERR_INVALID_ARG, "AIR %u: mutex sites given for an AIR without a lookup program", i);
-            continue;
-        }
-        const u32* w = st->airs[i].lookup->program;
-        const u32 nn = w[2], nc = w[3];
-        if (nc >= (1u << 24)) fail(MDN_ERR_UNSUPPORTED, "AIR %u: at most 2^24 - 1 lookup interactions", i);
+        if (!lookup_air(i, ann ? "mutex sites" : nullptr, skipped)) continue;
+        const LookupItems items(*st->airs[i].lookup);
+        if (items.n >= (1u << 24)) fail(MDN_ERR_UNSUPPORTED, "AIR %u: at most 2^24 - 1 lookup interactions", i);
         if (!ann) continue;
-        const u32* items = w + 5 + 3 * (size_t)nn;   // {column, flag, multiplicity, denominator}
         std::vector<u32> ids;
-        for (u32 q = 0; q < nc; q++) if (ann[q] != 0xFFFFFFFFu) ids.push_back(q);
+        for (u32 q = 0; q < items.n; q++) if (ann[q] != 0xFFFFFFFFu) ids.push_back(q);
         if (ids.size() > mk::BALANCE_MUTEX_MAX) fail(MDN_ERR_UNSUPPORTED, "AIR %u: %zu interactions in cached-encoding groups (at most %u)", i, ids.size(), mk::BALANCE_MUTEX_MAX);
-        auto group_of = [&](u32 q) { return (items[4 * (size_t)q] << 16) | (ann[q] >> 16); };
+        auto group_of = [&](u32 q) { return (items.column(q) << 16) | (ann[q] >> 16); };
         std::stable_sort(ids.begin(), ids.end(), [&](u32 a, u32 b) {
             return std::make_pair(group_of(a), ann[a] & 0xFFFFu) < std::make_pair(group_of(b), ann[b] & 0xFFFFu); });
         Mutex& m = mx[i];
-        m.pos.assign(nc, 0xFFFFFFFFu);
+        m.pos.assign(items.n, 0xFFFFFFFFu);
         for (size_t b = 0; b < ids.size(); b++) {
             u32 q = ids[b];
-            if (b && group_of(ids[b - 1]) == group_of(q) && (ann[ids[b - 1]] & 0xFFFFu) == (ann[q] & 0xFFFFu) && items[4 * (size_t)ids[b - 1] + 1] != items[4 * (size_t)q + 1])
+            if (b && group_of(ids[b - 1]) == group_of(q) && (ann[ids[b - 1]] & 0xFFFFu) == (ann[q] & 0xFFFFu) && items.flag(ids[b - 1]) != items.flag(q))
                 fail(MDN_ERR_INVALID_ARG, "AIR %u: interactions %u and %u share mutex site %u of group %u but not a flag node (one site is one insert or batch call)", i, ids[b - 1], q, ann[q] & 0xFFFFu, ann[q] >> 16);
             m.pos[q] = (u32)b; m.group.push_back(group_of(q)); m.site.push_back(ann[q] & 0xFFFFu);
         }
     }
 
-    // raw main traces of the lookup AIRs, column-major (column-major device traces are read where the caller keeps them)
-    std::vector<const u64*> main_cm(k, nullptr);
-    size_t main_total = 0;
-    for (u32 i = 0; i < k; i++) if (airs[i].has_lookup && !cm) main_total += ((size_t)1 << log_heights[i]) * airs[i].desc.width;
-    if (main_total) main_c.coef_buf.alloc(main_total, stream);
-    size_t co = 0;
-    for (u32 i = 0; i < k; i++) {
-        if (!airs[i].has_lookup) continue;
-        u64* dst = cm ? const_cast<u64*>(traces[i].values) : main_c.coef_buf.p + co;
-        if (!cm) co += ((size_t)1 << log_heights[i]) * airs[i].desc.width;
-        upload_matrix(traces[i], on_device, dst, cm);   // column-major: check only
-        main_cm[i] = dst;
-    }
-    check_input_flag("a main trace");
-    d_publics.alloc(std::max<size_t>(1, publics.size()), stream);
-    if (!publics.empty()) CUDA_OK(cudaMemcpyAsync(d_publics.p, publics.data(), publics.size() * sizeof(u64), cudaMemcpyHostToDevice, stream));
-    d_randomness.alloc(std::max<size_t>(1, 2 * (size_t)max_rand), stream);
-    if (max_rand) CUDA_OK(cudaMemcpyAsync(d_randomness.p, rnd, 2 * (size_t)max_rand * sizeof(u64), cudaMemcpyHostToDevice, stream));
+    std::vector<u32> lookups;
+    for (u32 i = 0; i < k; i++) if (airs[i].has_lookup) lookups.push_back(i);
+    const std::vector<u64*> main_cm = stage_main(traces, lookups, start.cm, start.on_device);
+    upload_leaves(rnd, 2 * (size_t)max_rand);
     std::vector<DevBuf> d_mx(k);
     for (u32 i = 0; i < k; i++) {
         const Mutex& m = mx[i];
@@ -1872,7 +1910,7 @@ void mdn_session::check_trace_balance(const mdn_statement* st, const mdn_matrix*
         b = mk::BalanceArgs{};
         b.main_cm = main_cm[i]; b.log_n = log_heights[i]; b.prog = airs[i].lookup_dev;
         b.publics = d_publics.p; b.challenges = d_randomness.p; b.instance = i;
-        const u32 nc = st->airs[i].lookup->program[3], na = (u32)mx[i].group.size();
+        const u32 nc = LookupItems(*st->airs[i].lookup).n, na = (u32)mx[i].group.size();
         if (na) {
             const u32* w = (const u32*)d_mx[i].p;
             b.mutex_pos = w; b.mutex_group = w + nc; b.mutex_site = w + nc + na; b.n_mutex = na;
@@ -1888,27 +1926,9 @@ void mdn_session::check_trace_balance(const mdn_statement* st, const mdn_matrix*
     const u64 n_push = cnt[0] + n_boundary, n_mutex = cnt[1];
     u64 slots = 1024;
     while (slots < 2 * n_push) slots <<= 1;
-    const size_t need = (size_t)(6 * slots + 6 * std::max<u64>(1, n_push) + 3 * std::max<u64>(1, n_mutex)) * sizeof(u64);
-    auto too_large = [&](const char* what) {
-        fail(MDN_ERR_UNSUPPORTED, "the balance table for %llu pushes needs %.1f GiB of device memory: %s",
-             (unsigned long long)n_push, need / 1073741824.0, what);
-    };
-    size_t arena_b = 0;
-    for (auto& sl : arena.slabs) arena_b += sl.size - sl.used;
-#ifndef MDN_EMULATED   // tests/emu has no device memory of its own: only the failed allocation below is reported there
-    size_t free_b = 0, total_b = 0;
-    CUDA_OK(cudaMemGetInfo(&free_b, &total_b));
-    char msg[64];
-    snprintf(msg, sizeof msg, "%.1f GiB are free", (free_b + arena_b) / 1073741824.0);
-    if (need > free_b + arena_b) too_large(msg);
-#endif
     DevBuf table, unm, mut;
-    try {
-        table.alloc(6 * slots, stream); unm.alloc(6 * std::max<u64>(1, n_push), stream); mut.alloc(3 * std::max<u64>(1, n_mutex), stream);
-    } catch (const MdnError&) {   // an out-of-memory allocation leaves no error behind; nothing has been launched on the table yet
-        cudaGetLastError();
-        too_large("the allocation failed");
-    }
+    alloc_checked("the balance table for " + std::to_string(n_push) + " pushes needs",
+                  {{&table, 6 * slots}, {&unm, 6 * std::max<u64>(1, n_push)}, {&mut, 3 * std::max<u64>(1, n_mutex)}});
     mk::BalanceTable t;
     t.keys = table.p; t.sums = table.p + 2 * slots;
     t.count = (unsigned long long*)(table.p + 4 * slots); t.first = (unsigned long long*)(table.p + 5 * slots); t.mask = slots - 1;
@@ -1940,7 +1960,6 @@ void mdn_session::check_trace_balance(const mdn_statement* st, const mdn_matrix*
     std::vector<u64> ord(n_unm);
     for (u64 u = 0; u < n_unm; u++) ord[u] = u;
     std::sort(ord.begin(), ord.end(), [&](u64 a, u64 b) { return std::make_pair(uh[6 * a], uh[6 * a + 1]) < std::make_pair(uh[6 * b], uh[6 * b + 1]); });
-    auto column_of = [&](u32 inst, u32 q) { return st->airs[inst].lookup->program[5 + 3 * (size_t)st->airs[inst].lookup->program[2] + 4 * (size_t)q]; };
     bal_unmatched.assign(n_unm, mdn_unmatched{});
     std::map<u64, u64> rank_of_slot;
     std::map<std::pair<u64, u64>, u64> rank_of_denom;
@@ -1983,7 +2002,7 @@ void mdn_session::check_trace_balance(const mdn_statement* st, const mdn_matrix*
             u32 inst = (u32)(r.key >> 48), q = (u32)(r.key & 0xFFFFFFu);
             p.multiplicity = r.m; p.interaction = q;
             if (inst == mk::BALANCE_BOUNDARY) { p.instance = 0xFFFFFFFFu; p.row = ~0ull; p.column = 0xFFFFFFFFu; }
-            else { p.instance = inst; p.row = (r.key >> 24) & 0xFFFFFFu; p.column = column_of(inst, q); }
+            else { p.instance = inst; p.row = (r.key >> 24) & 0xFFFFFFu; p.column = LookupItems(*st->airs[inst].lookup).column(q); }
             bal_contrib.push_back(p);
         }
     }
@@ -2011,41 +2030,23 @@ void mdn_session::check_trace_balance(const mdn_statement* st, const mdn_matrix*
 // check_lookup_folds: the constraint-path fold of every LogUp column on every row against an aux trace, without a
 // proof  (debug/trace/mod.rs:191-207, builder.rs; the comparison of processor/src/trace/tests/lookup.rs:185-265)
 // ---------------------------------------------------------------------------------------------
-// The validation, program compilation and main-trace upload of check_trace_balance; the challenges are an argument.
-// The aux traces come with the call (host row-major through the transpose, column-major device read in place) or from
-// build_logup_aux on the same traces.  k_fold_rows runs once per AIR with a lowered lookup program; a second launch on
-// the one failing row fetches its fold, expected and actual values.
+// start_check, then the main traces of the lookup AIRs staged; the challenges are an argument.  The aux traces come
+// with the call (host row-major through the transpose, column-major device read in place) or from build_logup_aux on
+// the same traces.  k_fold_rows runs once per AIR with a lowered lookup program; a second launch on the one failing row
+// fetches its fold, expected and actual values.
 void mdn_session::check_lookup_folds(const mdn_statement* st, const mdn_matrix* traces, const u64* rnd, const uint32_t* const* fold_marks,
                                      const mdn_matrix* aux, const u64* const* aux_finals, u64* const* folds_out, u32 flags, mdn_fold_report* out) {
-    const bool cm = column_major(flags);
-    reset_proof();
-    prof.st = stream; prof.reset();
-    if (!d_flag.p) { ArenaScope persistent(nullptr); d_flag.alloc(1, stream); CUDA_OK(cudaMemsetAsync(d_flag.p, 0, 8, stream)); }
-    if (!out) fail(MDN_ERR_INVALID_ARG, "null argument");
-    const mdn_challenger no_challenger{};   // nothing is observed: validate_statement only checks the statement
-    validate_statement(st, traces, &no_challenger);
-    if (cm) for (u32 i = 0; i < st->n_airs; i++) check_column_major(traces[i], "trace", i);
-    const bool on_device = (flags & MDN_FLAG_DEVICE_TRACES) != 0;
-    const u32 k = st->n_airs;
-    bind_airs(st, traces, false);
+    const auto [cm, on_device, k] = start_check(st, traces, &no_challenger, flags, out);
     bind_order(st, false);
 
     // arguments: challenges, aux traces and their closing values, fold marks, fold buffers
-    u32 max_rand = 0;
-    for (auto& a : airs) max_rand = std::max(max_rand, a.desc.num_randomness);
-    if (max_rand && !rnd) fail(MDN_ERR_INVALID_ARG, "randomness is NULL");
-    for (u32 i = 0; i < 2 * max_rand; i++) if (rnd[i] >= gl::P) fail(MDN_ERR_INVALID_ARG, "randomness word %u is not a canonical field element (>= p)", i);
+    const u32 max_rand = check_randomness(rnd);
     if (!aux && aux_finals) fail(MDN_ERR_INVALID_ARG, "aux_finals given without aux: the device LogUp build supplies its own closing values");
     u32 skipped = 0;
     size_t staging_words = 0;
     for (u32 i = 0; i < k; i++) {
         const uint32_t* marks = fold_marks ? fold_marks[i] : nullptr;
-        if (!airs[i].has_lookup) {
-            skipped++;
-            if (marks) fail(MDN_ERR_INVALID_ARG, "AIR %u: fold marks given for an AIR without a lookup program", i);
-            if (folds_out && folds_out[i]) fail(MDN_ERR_INVALID_ARG, "AIR %u: a fold buffer given for an AIR without a lookup program", i);
-            continue;
-        }
+        if (!lookup_air(i, marks ? "fold marks" : folds_out && folds_out[i] ? "a fold buffer" : nullptr, skipped)) continue;
         const u32 C = airs[i].desc.aux_width;
         if (aux) {
             if (aux[i].width != 2 * C || aux[i].log_height != log_heights[i]) fail(MDN_ERR_INVALID_ARG, "AIR %u: the aux trace must be 2^%u rows of %u base columns", i, log_heights[i], 2 * C);
@@ -2059,54 +2060,40 @@ void mdn_session::check_lookup_folds(const mdn_statement* st, const mdn_matrix* 
             if (!on_device) staging_words = std::max(staging_words, ((size_t)4 * C) << log_heights[i]);
         }
         if (!marks) continue;
-        const u32* w = st->airs[i].lookup->program;
-        const u32 nn = w[2], nc = w[3];
-        const u32* items = w + 5 + 3 * (size_t)nn;   // {column, flag, multiplicity, denominator}
-        for (u32 q = 0; q < nc; q++) {
+        const LookupItems items(*st->airs[i].lookup);
+        for (u32 q = 0; q < items.n; q++) {
             const u32 m = marks[q];
             if (m != 0 && m != 1 && m != 3) fail(MDN_ERR_INVALID_ARG, "AIR %u: fold mark %u of interaction %u (0, 1 or 3)", i, m, q);
-            if (m != 3 && (q == 0 || items[4 * (size_t)q] != items[4 * (size_t)(q - 1)]))
+            if (m != 3 && (q == 0 || items.column(q) != items.column(q - 1)))
                 fail(MDN_ERR_INVALID_ARG, "AIR %u: interaction %u starts a column and must open a group (fold mark 3)", i, q);
-            if (m == 0 && items[4 * (size_t)q + 1] != items[4 * (size_t)(q - 1) + 1])
+            if (m == 0 && items.flag(q) != items.flag(q - 1))
                 fail(MDN_ERR_INVALID_ARG, "AIR %u: interactions %u and %u are marked as one batch but do not share a flag node", i, q - 1, q);
         }
     }
 
-    // raw main traces of the lookup AIRs, column-major (column-major device traces are read where the caller keeps them)
-    std::vector<const u64*> main_cm(k, nullptr);
+    // raw main traces and aux slots of the lookup AIRs, column-major (column-major device aux traces are read where the
+    // caller keeps them)
+    std::vector<u32> lookups;
+    for (u32 i = 0; i < k; i++) if (airs[i].has_lookup) lookups.push_back(i);
+    const std::vector<u64*> main_cm = stage_main(traces, lookups, cm, on_device);
     std::vector<u64*> aux_cm(k, nullptr);
-    size_t main_total = 0, aux_total = 0;
-    for (u32 i = 0; i < k; i++) if (airs[i].has_lookup) {
-        size_t N = (size_t)1 << log_heights[i];
-        if (!cm) main_total += N * airs[i].desc.width;
-        if (!(aux && cm)) aux_total += N * 2 * airs[i].desc.aux_width;
-    }
-    if (main_total) main_c.coef_buf.alloc(main_total, stream);
-    if (aux_total) aux_c.coef_buf.alloc(aux_total, stream);
-    size_t co = 0, ao = 0;
-    for (u32 i = 0; i < k; i++) {
-        if (!airs[i].has_lookup) continue;
-        size_t N = (size_t)1 << log_heights[i];
-        u64* dst = cm ? const_cast<u64*>(traces[i].values) : main_c.coef_buf.p + co;
-        if (!cm) co += N * airs[i].desc.width;
-        upload_matrix(traces[i], on_device, dst, cm);   // column-major: check only
-        main_cm[i] = dst;
+    size_t aux_total = 0;
+    if (!(aux && cm)) for (u32 i : lookups) aux_total += ((size_t)1 << log_heights[i]) * 2 * airs[i].desc.aux_width;
+    aux_c.coef_buf.alloc(aux_total, stream);
+    size_t ao = 0;
+    for (u32 i : lookups) {
         if (aux && cm) aux_cm[i] = const_cast<u64*>(aux[i].values);
-        else { aux_cm[i] = aux_c.coef_buf.p + ao; ao += N * 2 * airs[i].desc.aux_width; }
+        else { aux_cm[i] = aux_c.coef_buf.p + ao; ao += ((size_t)1 << log_heights[i]) * 2 * airs[i].desc.aux_width; }
     }
-    check_input_flag("a main trace");
     if (aux) {
-        for (u32 i = 0; i < k; i++) if (airs[i].has_lookup) upload_matrix(aux[i], on_device, aux_cm[i], cm);
+        for (u32 i : lookups) upload_matrix(aux[i], on_device, aux_cm[i], cm);
         check_input_flag("an aux trace");
     }
-    d_publics.alloc(std::max<size_t>(1, publics.size()), stream);
-    if (!publics.empty()) CUDA_OK(cudaMemcpyAsync(d_publics.p, publics.data(), publics.size() * sizeof(u64), cudaMemcpyHostToDevice, stream));
-    d_randomness.alloc(std::max<size_t>(1, 2 * (size_t)max_rand), stream);
-    if (max_rand) CUDA_OK(cudaMemcpyAsync(d_randomness.p, rnd, 2 * (size_t)max_rand * sizeof(u64), cudaMemcpyHostToDevice, stream));
+    upload_leaves(rnd, 2 * (size_t)max_rand);
     std::vector<DevBuf> d_marks(k);
     for (u32 i = 0; i < k; i++) {
         if (!airs[i].has_lookup || !fold_marks || !fold_marks[i]) continue;
-        const u32 nc = st->airs[i].lookup->program[3];
+        const u32 nc = LookupItems(*st->airs[i].lookup).n;
         if (!nc) continue;
         d_marks[i].alloc(((size_t)nc + 1) / 2, stream);
         CUDA_OK(cudaMemcpyAsync(d_marks[i].p, fold_marks[i], nc * sizeof(u32), cudaMemcpyHostToDevice, stream));
@@ -2124,21 +2111,7 @@ void mdn_session::check_lookup_folds(const mdn_statement* st, const mdn_matrix* 
     }
     // host fold buffers are filled through one device staging buffer, sized for the largest of them
     DevBuf staging;
-    if (staging_words) {
-        auto too_large = [&](const char* what) {
-            fail(MDN_ERR_UNSUPPORTED, "the folds of the largest AIR need %.1f GiB of device memory: %s", staging_words * sizeof(u64) / 1073741824.0, what);
-        };
-#ifndef MDN_EMULATED   // tests/emu has no device memory of its own: only the failed allocation below is reported there
-        size_t arena_b = 0, free_b = 0, total_b = 0;
-        for (auto& sl : arena.slabs) arena_b += sl.size - sl.used;
-        CUDA_OK(cudaMemGetInfo(&free_b, &total_b));
-        char msg[64];
-        snprintf(msg, sizeof msg, "%.1f GiB are free", (free_b + arena_b) / 1073741824.0);
-        if (staging_words * sizeof(u64) > free_b + arena_b) too_large(msg);
-#endif
-        try { staging.alloc(staging_words, stream); }
-        catch (const MdnError&) { cudaGetLastError(); too_large("the allocation failed"); }
-    }
+    if (staging_words) alloc_checked("the folds of the largest AIR need", {{&staging, staging_words}});
 
     // per AIR: {first (row << 32 | column), failing rows, zero U}; then the probe's 9 words and its scratch counters
     DevBuf res; res.alloc(3 * (size_t)k + 12, stream);
@@ -2220,11 +2193,7 @@ void mdn_session::commit_aux(const mdn_matrix* aux, const u64* const* aux_values
     }
     aux_c.coef_buf.alloc(coef_total, stream);
     aux_c.lde_buf.alloc(lde_total, stream);
-    // device copies of the small per-proof vectors used by the lookup and constraint kernels
-    d_publics.alloc(std::max<size_t>(1, publics.size()), stream);
-    if (!publics.empty()) CUDA_OK(cudaMemcpyAsync(d_publics.p, publics.data(), publics.size() * sizeof(u64), cudaMemcpyHostToDevice, stream));
-    d_randomness.alloc(std::max<size_t>(1, 2 * randomness.size()), stream);
-    if (!randomness.empty()) CUDA_OK(cudaMemcpyAsync(d_randomness.p, randomness.data(), randomness.size() * sizeof(E2), cudaMemcpyHostToDevice, stream));
+    upload_leaves((const u64*)randomness.data(), 2 * randomness.size());
     size_t co = 0, lo = 0;
     std::vector<u32> pos(k);
     for (u32 j = 0; j < k; j++) {
@@ -2848,6 +2817,35 @@ void mdn_session::finish() {
 #define API_CATCH(s) } catch (const MdnError& e) { (s)->error = e.what(); (s)->reset_proof(); return e.code; } \
     catch (const std::exception& e) { (s)->error = e.what(); (s)->reset_proof(); return MDN_ERR_INVALID_ARG; } return MDN_OK;
 
+namespace {
+// the challenges the call sampled, two words each, when the caller asks for them
+void copy_randomness(const mdn_session* s, uint64_t* out) {
+    if (out) for (size_t i = 0; i < s->randomness.size(); i++) { out[2 * i] = s->randomness[i].a; out[2 * i + 1] = s->randomness[i].b; }
+}
+
+const char IN_PROOF[] = " called inside a proof (between mdn_prove_begin and mdn_prove_finish)";
+
+// A trace check (mdn_check_constraints and the others) named `name`: refused before any device work inside a staged
+// proof, so that the proof stays intact, then on a session split over ranks, then with `refused` (the caller's own
+// argument error, or NULL).  `check` runs in the proof arena, which is released afterwards; the challenges it sampled
+// go to `randomness_out` when given.
+template <class F> int run_check(mdn_session* s, const char* name, const char* refused, uint64_t* randomness_out, F check) {
+    if (!s) return MDN_ERR_INVALID_ARG;
+    if (s->in_proof) { s->error = name + std::string(IN_PROOF); return MDN_ERR_INVALID_ARG; }
+    if (s->shard_world > 1) { s->error = name + std::string(" does not run on a session split over ranks (mdn_session_set_shard world > 1)"); return MDN_ERR_UNSUPPORTED; }
+    if (refused) { s->error = refused; return MDN_ERR_INVALID_ARG; }
+    API_TRY(s)
+    {
+        ArenaScope proof_memory(s->use_arena ? &s->arena : nullptr);
+        CUDA_OK(cudaSetDevice(s->device));
+        check();
+        copy_randomness(s, randomness_out);
+    }
+    s->reset_proof();
+    API_CATCH(s)
+}
+}  // namespace
+
 extern "C" {
 
 int mdn_session_create(const mdn_pcs_params* params, int cuda_device, mdn_session** out) {
@@ -2877,6 +2875,9 @@ int mdn_session_create(const mdn_pcs_params* params, int cuda_device, mdn_sessio
         CUDA_OK(cudaStreamCreateWithFlags(&s->copy_stream, cudaStreamNonBlocking));
         for (auto& evn : s->copy_ev) CUDA_OK(cudaEventCreateWithFlags(&evn, cudaEventDisableTiming));
         for (auto& evn : s->ev) CUDA_OK(cudaEventCreate(&evn));
+        // the input and error flag word of the ingest, transpose and compare kernels; outside any proof arena
+        s->d_flag.alloc(1, s->stream);
+        CUDA_OK(cudaMemsetAsync(s->d_flag.p, 0, 8, s->stream));
         cudaMemPool_t pool;
         CUDA_OK(cudaDeviceGetDefaultMemPool(&pool, cuda_device));
         uint64_t thr = ~0ull;
@@ -2926,7 +2927,7 @@ int mdn_prove_begin(mdn_session* s, const mdn_statement* st, const mdn_matrix* t
     CUDA_OK(cudaSetDevice(s->device));
     s->prove_begin(st, traces, challenger, flags);
     if (main_root) memcpy(main_root, s->main_c.root, 32);
-    if (randomness_out) for (size_t i = 0; i < s->randomness.size(); i++) { randomness_out[2 * i] = s->randomness[i].a; randomness_out[2 * i + 1] = s->randomness[i].b; }
+    copy_randomness(s, randomness_out);
     API_CATCH(s)
 }
 
@@ -2995,75 +2996,33 @@ int mdn_prove(mdn_session* s, const mdn_statement* st, const mdn_matrix* traces,
 int mdn_check_constraints(mdn_session* s, const mdn_statement* st, const mdn_matrix* traces, const mdn_matrix* preprocessed,
                           const mdn_challenger* challenger, mdn_aux_builder build_aux, void* aux_ctx, uint32_t flags,
                           uint64_t* randomness_out, mdn_constraint_report* out) {
-    if (!s) return MDN_ERR_INVALID_ARG;
-    // refused before any device work, so that a staged proof in progress stays intact
-    if (s->in_proof) { s->error = "mdn_check_constraints called inside a proof (between mdn_prove_begin and mdn_prove_finish)"; return MDN_ERR_INVALID_ARG; }
-    if (s->shard_world > 1) { s->error = "mdn_check_constraints does not run on a session split over ranks (mdn_session_set_shard world > 1)"; return MDN_ERR_UNSUPPORTED; }
-    API_TRY(s)
-    {
-        ArenaScope proof_memory(s->use_arena ? &s->arena : nullptr);
-        CUDA_OK(cudaSetDevice(s->device));
-        s->check_constraints(st, traces, preprocessed, challenger, build_aux, aux_ctx, flags, out);
-        if (randomness_out) for (size_t i = 0; i < s->randomness.size(); i++) { randomness_out[2 * i] = s->randomness[i].a; randomness_out[2 * i + 1] = s->randomness[i].b; }
-    }
-    s->reset_proof();
-    API_CATCH(s)
+    return run_check(s, "mdn_check_constraints", nullptr, randomness_out,
+                     [&] { s->check_constraints(st, traces, preprocessed, challenger, build_aux, aux_ctx, flags, out); });
 }
 
 int mdn_constraint_census(mdn_session* s, const mdn_statement* st, const mdn_matrix* traces, const mdn_matrix* preprocessed,
                           const mdn_challenger* challenger, mdn_aux_builder build_aux, void* aux_ctx, uint32_t flags,
                           uint64_t* randomness_out, mdn_constraint_failure* failures, uint64_t max_failures,
                           mdn_constraint_tally* tallies, uint64_t max_tallies, mdn_constraint_census_report* out) {
-    if (!s) return MDN_ERR_INVALID_ARG;
-    // refused before any device work, so that a staged proof in progress stays intact
-    if (s->in_proof) { s->error = "mdn_constraint_census called inside a proof (between mdn_prove_begin and mdn_prove_finish)"; return MDN_ERR_INVALID_ARG; }
-    if (s->shard_world > 1) { s->error = "mdn_constraint_census does not run on a session split over ranks (mdn_session_set_shard world > 1)"; return MDN_ERR_UNSUPPORTED; }
-    if (!out) { s->error = "null argument"; return MDN_ERR_INVALID_ARG; }
-    if (!failures && max_failures) { s->error = "failures is NULL but max_failures is not 0"; return MDN_ERR_INVALID_ARG; }
-    if (!tallies && max_tallies) { s->error = "tallies is NULL but max_tallies is not 0"; return MDN_ERR_INVALID_ARG; }
-    API_TRY(s)
-    {
-        ArenaScope proof_memory(s->use_arena ? &s->arena : nullptr);
-        CUDA_OK(cudaSetDevice(s->device));
-        s->constraint_census(st, traces, preprocessed, challenger, build_aux, aux_ctx, flags, failures, max_failures, tallies, max_tallies, out);
-        if (randomness_out) for (size_t i = 0; i < s->randomness.size(); i++) { randomness_out[2 * i] = s->randomness[i].a; randomness_out[2 * i + 1] = s->randomness[i].b; }
-    }
-    s->reset_proof();
-    API_CATCH(s)
+    const char* refused = !out ? "null argument"
+                        : !failures && max_failures ? "failures is NULL but max_failures is not 0"
+                        : !tallies && max_tallies ? "tallies is NULL but max_tallies is not 0" : nullptr;
+    return run_check(s, "mdn_constraint_census", refused, randomness_out,
+                     [&] { s->constraint_census(st, traces, preprocessed, challenger, build_aux, aux_ctx, flags, failures, max_failures, tallies, max_tallies, out); });
 }
 
 int mdn_check_trace_balance(mdn_session* s, const mdn_statement* st, const mdn_matrix* traces, const uint64_t* randomness,
                             const uint64_t* boundary, size_t n_boundary, const uint32_t* const* mutex_sites,
                             uint64_t max_contributions, uint32_t flags, mdn_balance_report* out) {
-    if (!s) return MDN_ERR_INVALID_ARG;
-    // refused before any device work, so that a staged proof in progress stays intact
-    if (s->in_proof) { s->error = "mdn_check_trace_balance called inside a proof (between mdn_prove_begin and mdn_prove_finish)"; return MDN_ERR_INVALID_ARG; }
-    if (s->shard_world > 1) { s->error = "mdn_check_trace_balance does not run on a session split over ranks (mdn_session_set_shard world > 1)"; return MDN_ERR_UNSUPPORTED; }
-    API_TRY(s)
-    {
-        ArenaScope proof_memory(s->use_arena ? &s->arena : nullptr);
-        CUDA_OK(cudaSetDevice(s->device));
-        s->check_trace_balance(st, traces, randomness, boundary, n_boundary, mutex_sites, max_contributions, flags, out);
-    }
-    s->reset_proof();
-    API_CATCH(s)
+    return run_check(s, "mdn_check_trace_balance", nullptr, nullptr,
+                     [&] { s->check_trace_balance(st, traces, randomness, boundary, n_boundary, mutex_sites, max_contributions, flags, out); });
 }
 
 int mdn_check_lookup_folds(mdn_session* s, const mdn_statement* st, const mdn_matrix* traces, const uint64_t* randomness,
                            const uint32_t* const* fold_marks, const mdn_matrix* aux, const uint64_t* const* aux_finals,
                            uint64_t* const* folds_out, uint32_t flags, mdn_fold_report* out) {
-    if (!s) return MDN_ERR_INVALID_ARG;
-    // refused before any device work, so that a staged proof in progress stays intact
-    if (s->in_proof) { s->error = "mdn_check_lookup_folds called inside a proof (between mdn_prove_begin and mdn_prove_finish)"; return MDN_ERR_INVALID_ARG; }
-    if (s->shard_world > 1) { s->error = "mdn_check_lookup_folds does not run on a session split over ranks (mdn_session_set_shard world > 1)"; return MDN_ERR_UNSUPPORTED; }
-    API_TRY(s)
-    {
-        ArenaScope proof_memory(s->use_arena ? &s->arena : nullptr);
-        CUDA_OK(cudaSetDevice(s->device));
-        s->check_lookup_folds(st, traces, randomness, fold_marks, aux, aux_finals, folds_out, flags, out);
-    }
-    s->reset_proof();
-    API_CATCH(s)
+    return run_check(s, "mdn_check_lookup_folds", nullptr, nullptr,
+                     [&] { s->check_lookup_folds(st, traces, randomness, fold_marks, aux, aux_finals, folds_out, flags, out); });
 }
 
 size_t mdn_proof_serialize(const mdn_proof* p, uint8_t* out, size_t cap) {
@@ -3085,7 +3044,6 @@ int mdn_coset_lde_batch(mdn_session* s, const mdn_matrix* mat, uint32_t added_bi
     if (mat->log_height + added_bits > 32) fail(MDN_ERR_DOMAIN, "LDE log order %u exceeds two-adicity 32", mat->log_height + added_bits);
     if (s->in_proof) fail(MDN_ERR_INVALID_ARG, "mdn_coset_lde_batch called inside a proof");
     if (shift != gl::lde_shift(mat->log_height + added_bits)) fail(MDN_ERR_UNSUPPORTED, "only the canonical LDE shift 7^(2^(32-log_lde)) is supported");
-    if (!s->d_flag.p) { s->d_flag.alloc(1, s->stream); CUDA_OK(cudaMemsetAsync(s->d_flag.p, 0, 8, s->stream)); }
     Committed c;
     size_t N = (size_t)1 << mat->log_height, L = N << added_bits;
     c.coef_buf.alloc(N * mat->width, s->stream); c.lde_buf.alloc(L * mat->width, s->stream);
@@ -3107,7 +3065,6 @@ int mdn_lmcs_commit(mdn_session* s, const mdn_matrix* mats, uint32_t n_mats, uin
     API_TRY(s)
     CUDA_OK(cudaSetDevice(s->device));
     u32 lb = s->params.log_blowup;
-    if (!s->d_flag.p) { s->d_flag.alloc(1, s->stream); CUDA_OK(cudaMemsetAsync(s->d_flag.p, 0, 8, s->stream)); }
     Committed c;
     size_t ct = 0, lt = 0;
     for (u32 i = 0; i < n_mats; i++) {
@@ -3260,7 +3217,7 @@ int mdn_session_set_external_check(mdn_session* s, mdn_external_check fn, void* 
 int mdn_session_set_constraint_guard(mdn_session* s, uint32_t enable) {
     if (!s) return MDN_ERR_INVALID_ARG;
     if (enable > 1) { s->error = "mdn_session_set_constraint_guard: enable must be 0 or 1"; return MDN_ERR_INVALID_ARG; }
-    if (s->in_proof) { s->error = "mdn_session_set_constraint_guard called inside a proof (between mdn_prove_begin and mdn_prove_finish)"; return MDN_ERR_INVALID_ARG; }
+    if (s->in_proof) { s->error = std::string("mdn_session_set_constraint_guard") + IN_PROOF; return MDN_ERR_INVALID_ARG; }
     s->constraint_guard = enable == 1;
     return MDN_OK;
 }
