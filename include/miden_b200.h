@@ -318,7 +318,11 @@ int mdn_prove_finish(mdn_session* s, mdn_proof* out);
  * Returns MDN_OK whenever the check ran, whatever it found; malformed input gets mdn_prove's statuses and messages.
  * Refused before any device work: a call between mdn_prove_begin and mdn_prove_finish (MDN_ERR_INVALID_ARG) and a
  * session split over ranks (MDN_ERR_UNSUPPORTED).  The check uses the proof arena and releases it; it changes nothing
- * mdn_get_info / mdn_get_timings report about the last proof, and proofs after it are unchanged. */
+ * mdn_get_info / mdn_get_timings report about the last proof (MDN_INFO_JIT_CHECK is about the checks), and proofs
+ * after it are unchanged.
+ * The row pass of a program with at least the mdn_session_set_jit threshold of nodes runs on an NVRTC-specialised
+ * kernel (k_jit_check), self-checked against the interpreter on its first use; the one-row probe of the reported value
+ * stays on the interpreter.  mdn_get_info(MDN_INFO_JIT_CHECK) says which AIRs used it. */
 typedef struct {
     uint32_t holds;          /* 1: every constraint is zero on every row and every external assertion is zero */
     uint32_t kind;           /* 0 none, 1 AIR constraint, 2 external assertion: the failure the reference panics on first */
@@ -351,8 +355,10 @@ int mdn_check_constraints(mdn_session* s, const mdn_statement* st, const mdn_mat
  * A non-zero constraint makes the call return MDN_ERR_CONSTRAINT_VIOLATED: mdn_last_error names the instance, row and
  * constraint, nothing is committed and the proof is abandoned, as after a failing external assertion.  A statement that
  * holds gets the byte-identical proof it gets with the guard off: the guard observes and samples nothing.
- * Cost: the raw main copies (N x width x 8 bytes per AIR of the proof arena) and one k_check_rows pass per AIR; its
- * launches count in mdn_timings.kernel_launches and its time in kernel class 4 and in commit_aux.
+ * Cost: the raw main copies (N x width x 8 bytes per AIR of the proof arena) and one row pass per AIR -- k_jit_check
+ * for programs at or above the mdn_session_set_jit threshold (its cubin is compiled and loaded by mdn_prove_begin only
+ * while the guard is on), k_check_rows below it; its launches count in mdn_timings.kernel_launches and its time in
+ * kernel class 4 and in commit_aux.  mdn_get_info(MDN_INFO_JIT_CHECK) says which AIRs the last guard run specialised.
  * A session split over ranks (mdn_session_set_shard): every rank holds the whole raw main and aux traces and runs the
  * whole check on them, with no communication; every rank returns the same status and report. */
 int mdn_session_set_constraint_guard(mdn_session* s, uint32_t enable);
@@ -375,7 +381,10 @@ int mdn_last_constraint_report(const mdn_session* s, mdn_constraint_report* out)
  * A NULL list with a non-zero capacity, or a NULL out, is MDN_ERR_INVALID_ARG before any device work.  The outputs do
  * not depend on the order in which device atomics ran: two calls on the same inputs give byte-identical outputs.
  * Refused, as mdn_check_constraints, inside a staged proof and on a session split over ranks; uses and releases the
- * proof arena; leaves mdn_get_info, mdn_get_timings and later proofs unchanged. */
+ * proof arena; leaves mdn_get_info (but for MDN_INFO_JIT_CHECK), mdn_get_timings and later proofs unchanged.
+ * The per-row count and tally pass runs on the NVRTC kernel k_jit_census for programs at or above the mdn_session_set_jit
+ * threshold, as for mdn_check_constraints; the listing of the failures and the values at the tallies' first rows stay on
+ * the interpreter. */
 typedef struct {                 /* one violation: constraint `constraint` of instance `instance` is non-zero at `row` */
     uint32_t instance, constraint;
     uint64_t row;
@@ -585,6 +594,7 @@ typedef enum {
     MDN_INFO_JIT = 8,              /* per AIR (proof order) of the last proof: 1 = NVRTC kernel, 0 = interpreter */
     MDN_INFO_POOL = 9,             /* cudaMallocAsync pool reserved now / high, used now / high (bytes); proof arena capacity (bytes), slabs, driver allocations so far, live blocks */
     MDN_INFO_BUILD = 10,           /* { generation of the field arithmetic, generation of the NTT kernels }: always { 2, 2 } (poseidon2_fast2.cuh, ntt2.cuh) */
+    MDN_INFO_JIT_CHECK = 11,       /* per AIR (instance order) of the last mdn_check_constraints / mdn_constraint_census call or constraint-guard run: 1 = NVRTC row kernel, 0 = interpreter */
 } mdn_info;
 /* QUOTIENT_ACC / DEEP_EVALS are only recorded (extra device->host copies) after mdn_set_debug(s, 1). */
 int mdn_set_debug(mdn_session* s, int enable);
@@ -596,7 +606,11 @@ size_t mdn_abi_layout(uint32_t* out, size_t cap);
 /* ---- run-time specialisation of the constraint evaluator -------------------------------------------
  * AIR programs with at least `min_nodes` nodes (default 256; 0 = never) are lowered to straight-line CUDA,
  * compiled once per program with NVRTC for sm_90a and cached; smaller ones (and all of them when libnvrtc
- * is absent) run on the op-list interpreter.  Both produce identical values. */
+ * is absent) run on the op-list interpreter.  Both produce identical values.  Specialised: the proof's constraint
+ * evaluation and LogUp row build (MDN_INFO_JIT), and the row pass of mdn_check_constraints, mdn_constraint_census and
+ * the constraint guard (MDN_INFO_JIT_CHECK).  Interpreted whatever the size: the lookup checks
+ * (mdn_check_trace_balance, mdn_check_lookup_folds), the census's failure listing and the checks' one-row probes.
+ * Each compiled kernel is compared word for word with the interpreter on its first use in a session. */
 int mdn_session_set_jit(mdn_session* s, uint32_t min_nodes);
 /* "nvrtc <version>" or why it is unavailable, plus the reason the last JIT attempt was dropped (compile error,
  * or the first-use comparison against the interpreter failed -- the interpreter's result is then kept). */

@@ -8,7 +8,8 @@
 // prover/constraints/folder.rs:88-105), compiles it once per AIR with NVRTC for sm_90a and launches the
 // cubin through the driver API.  Field arithmetic is exact, so the result is bit-identical to the interpreter
 // (asserted in tests/test_gpu_parity.py).  libnvrtc / libcuda are dlopen'ed on first use; when NVRTC is
-// missing the session keeps using the interpreter and says so in mdn_get_info(MDN_INFO_JIT).
+// missing the session keeps using the interpreter and says so in mdn_get_info(MDN_INFO_JIT).  The same lowering also
+// gives the LogUp row kernel (MODE_LOOKUP) and the trace-check row kernels (MODE_CHECK, MDN_INFO_JIT_CHECK).
 #pragma once
 #include <cuda_runtime.h>
 #include <dlfcn.h>
@@ -16,6 +17,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <map>
+#include <memory>
 #include <mutex>
 #include <stdexcept>
 #include <string>
@@ -44,6 +46,23 @@ struct LookupJitArgs {
     uint32_t* bad_flag;
     uint32_t log_n, n_periodic, log_max_period, pad;
 };
+
+// Arguments of the generated trace-check kernels k_jit_check / k_jit_census (the semantics of k_check_rows /
+// k_census_rows, kernels.cuh CheckArgs / CensusArgs); layout must equal `struct CheckJitArgs` in PRELUDE_CHECK below.
+struct CheckJitArgs {
+    const uint64_t* main_lde; const uint64_t* aux_lde; const uint64_t* prep_lde;   // raw column-major traces (L = N)
+    const uint64_t* publics; const uint64_t* challenges; const uint64_t* aux_values;
+    const uint64_t* periodic;                         // raw row-major matrix (max_period x n_periodic)
+    unsigned long long* first; unsigned long long* failing_rows;   // k_jit_check: init ~0 / 0; census: failing_rows only
+    uint32_t* row_count; unsigned long long* tally;  // k_jit_census: 2^log_n counts, 3 * n_cons tally words; check: NULL
+    uint64_t row0, n_rows;                           // k_jit_check: rows [row0, row0 + n_rows)
+    uint32_t log_n, n_cons, n_periodic, log_max_period;
+};
+// per-block shared tallies of k_jit_census up to this many constraints (kernels.cuh CENSUS_SHARED_K)
+static constexpr uint32_t CENSUS_SHARED_K = 256;
+
+// what generate() emits: the proof's constraint kernel, the LogUp row kernel, or the two trace-check kernels
+enum Mode : uint32_t { MODE_CONSTRAINTS = 0, MODE_LOOKUP = 1, MODE_CHECK = 2 };
 
 static const char PRELUDE[] = R"CUDA(
 typedef unsigned long long u64;
@@ -110,6 +129,28 @@ struct LookupJitArgs {
     u32 log_n, n_periodic, log_max_period, pad;
 };
 )CUDA";
+// check mode only (the constraint and lookup modes emit the preludes above and nothing else): the argument struct
+// and the failure record of one (row, constraint) -- a count, a least row and a greatest row per constraint, in the
+// block's shared table `sh` ([3][CENSUS_SHARED_K]) or, when sh is NULL, straight in the global tally
+static const char PRELUDE_CHECK[] = R"CUDA(struct CheckJitArgs {
+    const u64* main_lde; const u64* aux_lde; const u64* prep_lde;
+    const u64* publics; const u64* challenges; const u64* aux_values;
+    const u64* periodic;
+    unsigned long long* first; unsigned long long* failing_rows;
+    u32* row_count; unsigned long long* tally;
+    u64 row0, n_rows;
+    u32 log_n, n_cons, n_periodic, log_max_period;
+};
+template <class T> __device__ __forceinline__ T census_max(T* p, T v) { return atomicMax(p, v); }
+__device__ __noinline__ void tally(const CheckJitArgs& a, u32* sh, u32 r, u32 k) {
+    if (sh) { atomicAdd(&sh[k], 1u); atomicMin(&sh[CENSUS_SHARED_K + k], r); census_max(&sh[2 * CENSUS_SHARED_K + k], r); }
+    else {
+        atomicAdd(&a.tally[3 * k], 1ull);
+        atomicMin(&a.tally[3 * k + 1], (unsigned long long)r);
+        census_max(&a.tally[3 * k + 2], (unsigned long long)r);
+    }
+}
+)CUDA";
 
 // ---------------------------------------------------------------------------------------------
 // code generation
@@ -125,9 +166,15 @@ struct GenInfo { uint32_t n_constraints = 0; bool uses_sel = false; uint32_t n_c
 // whose slots are assigned by chunk-granular liveness.
 inline uint32_t chunk_nodes() { const char* e = getenv("MDN_JIT_CHUNK"); uint32_t v = e ? (uint32_t)atoi(e) : 0; return v ? v : 512; }
 
-// lookup == true: `w` is a lowered LookupAir ("MLKP": 4-word interactions instead of constraint ids) and the
+// MODE_LOOKUP: `w` is a lowered LookupAir ("MLKP": 4-word interactions instead of constraint ids) and the
 // kernel is the row kernel of build_logup_aux_trace (one (V, U) rational per aux column, see k_logup_rows).
-inline std::string generate(const uint32_t* w, GenInfo* info, bool lookup = false, uint32_t n_cols = 0) {
+// MODE_CHECK: `w` is a constraint program evaluated on the TRACE domain as CHECK_NODE_CASES does (kernels.cu): raw
+// column-major traces with L = N, the raw row-major periodic matrix, selectors exactly 0 or 1.  Each constraint is
+// tested instead of folded; a chunk returns its failures' count and least constraint index, so the row's result does
+// not depend on the order the chunks visit the constraints in.  Two entry points share the chunks: k_jit_check (the
+// semantics of k_check_rows) and k_jit_census (those of k_census_rows).
+inline std::string generate(const uint32_t* w, GenInfo* info, Mode mode = MODE_CONSTRAINTS, uint32_t n_cols = 0) {
+    const bool lookup = mode == MODE_LOOKUP, check = mode == MODE_CHECK;
     const uint32_t nn = w[2], nc = w[3];
     const uint32_t* cons = w + 5 + 3 * (size_t)nn;
     const uint32_t* kw = cons + (lookup ? 4 : 1) * (size_t)nc;
@@ -239,15 +286,22 @@ inline std::string generate(const uint32_t* w, GenInfo* info, bool lookup = fals
     s += PRELUDE;
     s += PRELUDE_FMUL_G2;
     s += PRELUDE_B;
-    s += lookup ? "typedef LookupJitArgs KArgs;\n" : "typedef JitArgs KArgs;\n";
+    if (check) {
+        snprintf(buf, sizeof buf, "#define CENSUS_SHARED_K %uu\n", CENSUS_SHARED_K);
+        s += buf;
+        s += PRELUDE_CHECK;
+    }
+    s += lookup ? "typedef LookupJitArgs KArgs;\n" : check ? "typedef CheckJitArgs KArgs;\n" : "typedef JitArgs KArgs;\n";
     s += "struct Ctx { size_t L, pos, pn, per_idx, per_stride; u64 is_first, is_last, is_trans; };\n";
     std::vector<uint8_t> seen(nn, 0);
     for (uint32_t c = 0; c < n_chunks; c++) {
         if (lookup) snprintf(buf, sizeof buf, "__device__ __noinline__ void chunk%u(const KArgs& a, const Ctx& c, u64* __restrict__ Sb, E2* __restrict__ Se, E2* __restrict__ V, E2* __restrict__ U) {\n", c);
+        else if (check) snprintf(buf, sizeof buf, "__device__ __noinline__ u64 chunk%u(const KArgs& a, const Ctx& c, u64* __restrict__ Sb, E2* __restrict__ Se, u32* sh) {\n", c);
         else snprintf(buf, sizeof buf, "__device__ __noinline__ void chunk%u(const KArgs& a, const Ctx& c, u64* __restrict__ Sb, E2* __restrict__ Se, E2& acc) {\n", c);
         s += buf;
         s += "  const size_t L = c.L, pos = c.pos, pn = c.pn, per_idx = c.per_idx, per_stride = c.per_stride;\n"
              "  (void)L; (void)pos; (void)pn; (void)per_idx; (void)per_stride; (void)Sb; (void)Se;\n";
+        if (check) s += "  u32 f = 0xFFFFFFFFu, n = 0;   /* least failing constraint, failures */\n";
         // operands needed by this chunk: leaves (re-materialised) and live-in arithmetic values (loaded)
         std::vector<uint32_t> need;
         auto want = [&](uint32_t o) { if (!seen[o]) { seen[o] = 1; need.push_back(o); } };
@@ -264,6 +318,13 @@ inline std::string generate(const uint32_t* w, GenInfo* info, bool lookup = fals
         }
         for (uint32_t j = 0; j < nn; j++) if (chunk_of[j] == c) s += arith_def(j);
         for (uint32_t k : folds[c]) {
+            if (check) {
+                uint32_t cn = cons[k];
+                std::string nz = ext[cn] ? "(" + nm(cn) + ".a | " + nm(cn) + ".b) != 0ull" : nm(cn) + " != 0ull";
+                snprintf(buf, sizeof buf, "  if (%s) { n++; f = f < %uu ? f : %uu; if (a.tally) tally(a, sh, (u32)pos, %uu); }\n", nz.c_str(), k, k, k);
+                s += buf;
+                continue;
+            }
             if (!lookup) {
                 uint32_t cn = cons[k];
                 snprintf(buf, sizeof buf, "  acc = eadd(acc, %s(ldapow(a.apow, %u), %s));\n", ext[cn] ? "emul" : "emulf", k, nm(cn).c_str());
@@ -279,7 +340,63 @@ inline std::string generate(const uint32_t* w, GenInfo* info, bool lookup = fals
             s += buf;
         }
         for (uint32_t j : defined[c]) { snprintf(buf, sizeof buf, "  %s[%u] = %s;\n", ext[j] ? "Se" : "Sb", slot[j], nm(j).c_str()); s += buf; }
+        if (check) s += "  return (u64)n << 32 | f;\n";
         s += "}\n";
+    }
+    if (check) {
+        // row r of the trace domain: (failures << 32) | least failing constraint (0xFFFFFFFF: none)
+        s += "__device__ __forceinline__ u64 check_row(const KArgs& a, size_t r, u32* sh) {\n"
+             "  Ctx c;\n"
+             "  c.L = (size_t)1 << a.log_n;\n"
+             "  c.pos = r;\n"
+             "  c.pn = (r + 1) & (c.L - 1);\n"
+             "  c.per_idx = (r & (((size_t)1 << a.log_max_period) - 1)) * a.n_periodic;\n"
+             "  c.per_stride = 1;\n"
+             "  c.is_first = r == 0; c.is_last = r == c.L - 1; c.is_trans = r != c.L - 1;\n";
+        snprintf(buf, sizeof buf, "  u64 Sb[%u]; E2 Se[%u];\n  u32 f = 0xFFFFFFFFu, n = 0;\n", std::max(1u, nb), std::max(1u, ne));
+        s += buf;
+        for (uint32_t c = 0; c < n_chunks; c++) {
+            snprintf(buf, sizeof buf, "  { const u64 o = chunk%u(a, c, Sb, Se, sh); n += (u32)(o >> 32); f = f < (u32)o ? f : (u32)o; }\n", c);
+            s += buf;
+        }
+        s += "  return (u64)n << 32 | f;\n"
+             "}\n"
+             // k_check_rows: a failing row does one atomicMin(first, row << 32 | least k) and counts once
+             "extern \"C\" __global__ void __launch_bounds__(128) k_jit_check(const KArgs a) {\n"
+             "  const size_t r = a.row0 + (size_t)blockIdx.x * blockDim.x + threadIdx.x;\n"
+             "  if (r >= a.row0 + a.n_rows) return;\n"
+             "  const u32 f = (u32)check_row(a, r, nullptr);\n"
+             "  if (f != 0xFFFFFFFFu) {\n"
+             "    atomicMin(a.first, (unsigned long long)(((u64)r << 32) | f));\n"
+             "    atomicAdd(a.failing_rows, 1ull);\n"
+             "  }\n"
+             "}\n"
+             // k_census_rows: every row's failure count; per constraint count, least and greatest row, per block in
+             // shared memory up to CENSUS_SHARED_K constraints, else straight to the global tally
+             "extern \"C\" __global__ void __launch_bounds__(128) k_jit_census(const KArgs a) {\n"
+             "  __shared__ u32 s_t[3 * CENSUS_SHARED_K];\n"
+             "  __shared__ u32 s_rows;\n"
+             "  const bool shared_tally = a.n_cons <= CENSUS_SHARED_K;\n"
+             "  if (shared_tally) for (u32 k = threadIdx.x; k < a.n_cons; k += blockDim.x) { s_t[k] = 0; s_t[CENSUS_SHARED_K + k] = 0xFFFFFFFFu; s_t[2 * CENSUS_SHARED_K + k] = 0; }\n"
+             "  if (threadIdx.x == 0) s_rows = 0;\n"
+             "  __syncthreads();\n"
+             "  const size_t N = (size_t)1 << a.log_n, r = (size_t)blockIdx.x * blockDim.x + threadIdx.x;\n"
+             "  if (r < N) {\n"
+             "    const u32 n = (u32)(check_row(a, r, shared_tally ? s_t : nullptr) >> 32);\n"
+             "    a.row_count[r] = n;\n"
+             "    if (n) atomicAdd(&s_rows, 1u);\n"
+             "  }\n"
+             "  __syncthreads();\n"
+             "  if (shared_tally) for (u32 k = threadIdx.x; k < a.n_cons; k += blockDim.x) {\n"
+             "    if (!s_t[k]) continue;\n"
+             "    atomicAdd(&a.tally[3 * k], (unsigned long long)s_t[k]);\n"
+             "    atomicMin(&a.tally[3 * k + 1], (unsigned long long)s_t[CENSUS_SHARED_K + k]);\n"
+             "    census_max(&a.tally[3 * k + 2], (unsigned long long)s_t[2 * CENSUS_SHARED_K + k]);\n"
+             "  }\n"
+             "  if (threadIdx.x == 0 && s_rows) atomicAdd(a.failing_rows, (unsigned long long)s_rows);\n"
+             "}\n";
+        if (info) { info->n_constraints = nc; info->uses_sel = uses_sel; info->n_chunks = n_chunks; info->spill_base = nb; info->spill_ext = ne; }
+        return s;
     }
     if (lookup) {
         s += "extern \"C\" __global__ void __launch_bounds__(128) k_jit(const KArgs a) {\n"
@@ -454,18 +571,25 @@ inline Driver& driver() {
 inline std::string cu_err(int rc) { const char* s = nullptr; if (driver().GetErrorString) driver().GetErrorString(rc, &s); return s ? s : "unknown driver error"; }
 
 struct Kernel {
-    void* module = nullptr; void* func = nullptr;
+    std::shared_ptr<void> module;   // shared by the entry points of one cubin (k_jit_check and k_jit_census)
+    void* func = nullptr;
     int checked = 0;   // 0: not yet compared with the interpreter, 1: agreed, -1: disagreed (never used again)
     Kernel() {}
     Kernel(const Kernel&) = delete; Kernel& operator=(const Kernel&) = delete;
-    ~Kernel() { if (module && driver().ok()) driver().ModuleUnload(module); }
     // The caller's device must be current and its primary context initialised (any runtime call does that).
-    void load(const std::vector<char>& cubin) {
+    void load(const std::vector<char>& cubin, const char* name = "k_jit") {
         Driver& d = driver();
         if (!d.ok()) throw std::runtime_error("CUDA driver unavailable: " + d.why);
-        int rc = d.ModuleLoadData(&module, cubin.data());
+        void* m = nullptr;
+        int rc = d.ModuleLoadData(&m, cubin.data());
         if (rc) throw std::runtime_error("cuModuleLoadData: " + cu_err(rc));
-        rc = d.ModuleGetFunction(&func, module, "k_jit");
+        module = std::shared_ptr<void>(m, [](void* p) { if (driver().ok()) driver().ModuleUnload(p); });
+        entry(name);
+    }
+    // another entry point of the module `other` loaded
+    void load(const Kernel& other, const char* name) { module = other.module; entry(name); }
+    void entry(const char* name) {
+        int rc = driver().ModuleGetFunction(&func, module.get(), name);
         if (rc) throw std::runtime_error("cuModuleGetFunction: " + cu_err(rc));
     }
     template <class Args>
@@ -482,15 +606,15 @@ inline uint64_t fnv1a(const uint32_t* w, size_t n) {
     for (size_t i = 0; i < n; i++) { h ^= w[i]; h *= 1099511628211ull; }
     return h;
 }
-inline const std::vector<char>& cubin_for(const uint32_t* w, size_t n_words, GenInfo* info, bool lookup = false, uint32_t n_cols = 0) {
+inline const std::vector<char>& cubin_for(const uint32_t* w, size_t n_words, GenInfo* info, Mode mode = MODE_CONSTRAINTS, uint32_t n_cols = 0) {
     static std::mutex mu;
     static std::map<uint64_t, std::pair<std::vector<char>, GenInfo>> cache;
-    uint64_t key = fnv1a(w, n_words) ^ (uint64_t)n_words << 40 ^ (uint64_t)chunk_nodes() << 20 ^ (uint64_t)n_cols << 8 ^ (uint64_t)lookup;
+    uint64_t key = fnv1a(w, n_words) ^ (uint64_t)n_words << 40 ^ (uint64_t)chunk_nodes() << 20 ^ (uint64_t)n_cols << 8 ^ (uint64_t)mode;
     std::lock_guard<std::mutex> g(mu);
     auto it = cache.find(key);
     if (it == cache.end()) {
         GenInfo gi;
-        std::string src = generate(w, &gi, lookup, n_cols);
+        std::string src = generate(w, &gi, mode, n_cols);
         if (const char* dump = getenv("MDN_JIT_DUMP")) { if (FILE* f = fopen(dump, "w")) { fwrite(src.data(), 1, src.size(), f); fclose(f); } }
         it = cache.emplace(key, std::make_pair(compile(src), gi)).first;
         if (const char* dump = getenv("MDN_JIT_DUMP_CUBIN")) { if (FILE* f = fopen(dump, "wb")) { fwrite(it->second.first.data(), 1, it->second.first.size(), f); fclose(f); } }

@@ -186,8 +186,10 @@ struct AirHost {
     DevBuf lookup_program, raw_main, raw_periodic;
     const u64* raw_main_cm = nullptr;
     mk::AirDev lookup_dev;
-    // NVRTC-specialised constraint kernel (jit.hpp) for large programs; NULL = interpreter
-    std::shared_ptr<jit::Kernel> jit, lookup_jit;
+    // NVRTC-specialised constraint kernel (jit.hpp) for large programs; NULL = interpreter.  check_jit / census_jit:
+    // the two entry points of the program's trace-check cubin (k_jit_check, k_jit_census), loaded for the checks and
+    // for a guarded proof
+    std::shared_ptr<jit::Kernel> jit, lookup_jit, check_jit, census_jit;
     u32 n_constraints = 0;
 };
 
@@ -292,6 +294,7 @@ struct mdn_session {
     u32 jit_min_nodes = 256;
     std::map<u64, std::shared_ptr<jit::Kernel>> jit_kernels;   // loaded modules by program hash
     std::vector<u64> jit_used;       // per AIR of the last proof: 1 = JIT kernel, 0 = interpreter
+    std::vector<u64> jit_check_used; // per AIR (instance order) of the last constraint check, census or guard run: the same
     std::string jit_note;            // why the JIT was not used, if it was wanted
     Committed prep_c; bool has_prep = false;
     std::vector<u32> prep_air, prep_log_h;
@@ -331,14 +334,14 @@ struct mdn_session {
     void upload_matrix(const mdn_matrix& m, bool on_device, u64* dst_cm, bool col_major = false);
     void prove_begin(const mdn_statement* st, const mdn_matrix* traces, const mdn_challenger* ch, u32 flags);
     void validate_statement(const mdn_statement* st, const mdn_matrix* traces, const mdn_challenger* ch);
-    void bind_airs(const mdn_statement* st, const mdn_matrix* traces, bool jit);
+    void bind_airs(const mdn_statement* st, const mdn_matrix* traces, bool jit, bool check_jit);
     void bind_order(const mdn_statement* st, bool tables);
     void bind_challenger(const mdn_challenger* ch);
     void upload_and_commit_main(const mdn_matrix* traces, bool on_device);
     int eval_external(u32* failed);
     // what every trace check starts with (start_check) and the pieces its callers share
     struct CheckStart { bool cm, on_device; u32 k; };
-    CheckStart start_check(const mdn_statement* st, const mdn_matrix* traces, const mdn_challenger* ch, u32 flags, const void* out);
+    CheckStart start_check(const mdn_statement* st, const mdn_matrix* traces, const mdn_challenger* ch, u32 flags, const void* out, bool check_jit = false);
     std::vector<u64*> stage_main(const mdn_matrix* traces, const std::vector<u32>& insts, bool cm, bool on_device);
     u32 check_randomness(const u64* rnd);
     void upload_leaves(const u64* rnd, size_t n_words);
@@ -357,6 +360,15 @@ struct mdn_session {
         c.prog.periodic = periodic;
         c.publics = d_publics.p; c.challenges = d_randomness.p; c.aux_values = values + aux_values_off[j];
         return c;
+    }
+    // the same inputs for the NVRTC trace-check kernels (jit.hpp CheckJitArgs); the result pointers are the caller's
+    static_assert(jit::CENSUS_SHARED_K == mk::CENSUS_SHARED_K, "k_jit_census tallies in shared memory as k_census_rows does");
+    template <class Args> static jit::CheckJitArgs check_jit_args(const Args& c) {
+        jit::CheckJitArgs ja{};
+        ja.main_lde = c.main_cm; ja.aux_lde = c.aux_cm; ja.prep_lde = c.prep_cm;
+        ja.publics = c.publics; ja.challenges = c.challenges; ja.aux_values = c.aux_values; ja.periodic = c.prog.periodic;
+        ja.log_n = c.log_n; ja.n_periodic = c.prog.n_periodic; ja.log_max_period = c.prog.log_max_period;
+        return ja;
     }
     void check_constraints(const mdn_statement* st, const mdn_matrix* traces, const mdn_matrix* prep, const mdn_challenger* ch,
                            mdn_aux_builder build_aux, void* aux_ctx, u32 flags, mdn_constraint_report* out);
@@ -969,7 +981,7 @@ void mdn_session::prove_begin(const mdn_statement* st, const mdn_matrix* traces,
     CUDA_OK(cudaEventRecord(ev[0], stream));
 
     u32 k = st->n_airs;
-    bind_airs(st, traces, true);
+    bind_airs(st, traces, true, constraint_guard);
     if (constraint_guard) for (u32 i = 0; i < k; i++) {   // the guard's raw periodic matrices (canonical: checked by bind_airs)
         const mdn_air& a = st->airs[i];
         if (!a.num_periodic_columns) continue;
@@ -1022,8 +1034,9 @@ void mdn_session::validate_statement(const mdn_statement* st, const mdn_matrix* 
 }
 
 // per-AIR shape checks, constraint program compilation and upload, lowered lookup programs.  `jit`: also load the
-// NVRTC kernels of large programs (the proof's constraint evaluation; a constraint check runs the interpreter only)
-void mdn_session::bind_airs(const mdn_statement* st, const mdn_matrix* traces, bool jit) {
+// NVRTC kernels of large programs for the proof (its constraint evaluation and LogUp row build); `check_jit`: the
+// trace-check kernels of large constraint programs (the constraint check and census, the constraint guard)
+void mdn_session::bind_airs(const mdn_statement* st, const mdn_matrix* traces, bool jit, bool check_jit) {
     u32 k = st->n_airs, lb = params.log_blowup;
     airs.resize(k); log_heights.resize(k);
     for (u32 i = 0; i < k; i++) {
@@ -1101,6 +1114,22 @@ void mdn_session::bind_airs(const mdn_statement* st, const mdn_matrix* traces, b
                 h.jit = it->second;
             } catch (const std::exception& e) { jit_note = e.what(); }
         }
+        h.check_jit.reset(); h.census_jit.reset();
+        if (check_jit && jit_min_nodes && a.program[2] >= jit_min_nodes) {
+            try {
+                // one cubin, two entry points; the keys carry the mode as the lookup kernel's carries "LKUP"
+                const u64 key = jit::fnv1a(a.program, a.program_words) ^ ((u64)a.program_words << 40);
+                const u64 k_check = key ^ 0x4348454Bull, k_census = key ^ 0x43454E53ull;   // "CHEK", "CENS"
+                if (!jit_kernels.count(k_check) || !jit_kernels.count(k_census)) {
+                    const std::vector<char>& cubin = jit::cubin_for(a.program, a.program_words, nullptr, jit::MODE_CHECK);
+                    auto kc = std::make_shared<jit::Kernel>(), ks = std::make_shared<jit::Kernel>();
+                    kc->load(cubin, "k_jit_check");
+                    ks->load(*kc, "k_jit_census");
+                    jit_kernels[k_check] = kc; jit_kernels[k_census] = ks;
+                }
+                h.check_jit = jit_kernels[k_check]; h.census_jit = jit_kernels[k_census];
+            } catch (const std::exception& e) { jit_note = e.what(); }
+        }
         // lowered LookupAir -> the aux trace of this AIR is built on the device (commit_aux)
         h.has_lookup = a.lookup != nullptr;
         if (h.has_lookup) {
@@ -1128,7 +1157,7 @@ void mdn_session::bind_airs(const mdn_statement* st, const mdn_matrix* traces, b
                     u64 key = jit::fnv1a(lk.program, lk.program_words) ^ ((u64)lk.program_words << 40) ^ 0x4C4B5550ull;
                     auto it = jit_kernels.find(key);
                     if (it == jit_kernels.end()) {
-                        const std::vector<char>& cubin = jit::cubin_for(lk.program, lk.program_words, nullptr, true, lk.num_columns);
+                        const std::vector<char>& cubin = jit::cubin_for(lk.program, lk.program_words, nullptr, jit::MODE_LOOKUP, lk.num_columns);
                         auto kn = std::make_shared<jit::Kernel>();
                         kn->load(cubin);
                         it = jit_kernels.emplace(key, kn).first;
@@ -1415,16 +1444,17 @@ struct LookupItems {
 }  // namespace
 
 // The start of a trace check: a fresh proof state, the statement validated (`chal` NULL-checked as mdn_prove does;
-// &no_challenger when nothing is observed) and its AIRs compiled.  The caller validates what it takes besides and then
-// calls bind_order, in that order: the order of the errors a call reports is part of its behaviour.
-mdn_session::CheckStart mdn_session::start_check(const mdn_statement* st, const mdn_matrix* traces, const mdn_challenger* chal, u32 flags, const void* out) {
+// &no_challenger when nothing is observed) and its AIRs compiled (`check_jit`: with the trace-check kernels of large
+// constraint programs).  The caller validates what it takes besides and then calls bind_order, in that order: the order
+// of the errors a call reports is part of its behaviour.
+mdn_session::CheckStart mdn_session::start_check(const mdn_statement* st, const mdn_matrix* traces, const mdn_challenger* chal, u32 flags, const void* out, bool check_jit) {
     const bool cm = column_major(flags);
     reset_proof();
     prof.st = stream; prof.reset();
     if (!out) fail(MDN_ERR_INVALID_ARG, "null argument");
     validate_statement(st, traces, chal);
     if (cm) for (u32 i = 0; i < st->n_airs; i++) check_column_major(traces[i], "trace", i);
-    bind_airs(st, traces, false);
+    bind_airs(st, traces, false, check_jit);
     return CheckStart{cm, (flags & MDN_FLAG_DEVICE_TRACES) != 0, st->n_airs};
 }
 
@@ -1521,26 +1551,58 @@ void mdn_session::check_constraints(const mdn_statement* st, const mdn_matrix* t
     out->holds = cs.ext_rc == 0 && out->failing_rows == 0;
 }
 
-// The row pass (debug.rs:120-214) of check_constraints and of the constraint guard: k_check_rows on every row of every
-// AIR, instance order (ca[i]: AIR i's traces, program and leaves; the rows and result words are set here).  `out` gets
-// the failing-row total over all AIRs and, when `locate`, kind 1 with the least failing (instance, row, constraint)
-// and that constraint's value, from a one-row relaunch; every other field is zero.
+// The row pass (debug.rs:120-214) of check_constraints and of the constraint guard: k_jit_check when AIR i has the
+// NVRTC check kernel, else k_check_rows, on every row of every AIR, instance order (ca[i]: AIR i's traces, program and
+// leaves; the rows and result words are set here).  `out` gets the failing-row total over all AIRs and, when `locate`,
+// kind 1 with the least failing (instance, row, constraint) and that constraint's value, from a one-row relaunch of
+// k_check_rows; every other field is zero.
 void mdn_session::check_rows(std::vector<mk::CheckArgs>& ca, bool locate, mdn_constraint_report* out) {
     const u32 k = (u32)ca.size();
-    // per AIR the lowest (row, constraint) that is non-zero and the failing-row count
-    DevBuf res; res.alloc(2 * (size_t)k + 4, stream);
-    std::vector<u64> host_res(2 * (size_t)k + 4, 0);
-    for (u32 i = 0; i < k; i++) host_res[2 * i] = ~0ull;
+    // per AIR the lowest (row, constraint) that is non-zero and the failing-row count; 4 scratch words for the probe;
+    // then per AIR the interpreter's two words of a check kernel's first-use comparison
+    const size_t twin = 2 * (size_t)k + 4;
+    DevBuf res; res.alloc(twin + 2 * (size_t)k, stream);
+    std::vector<u64> host_res(twin + 2 * (size_t)k, 0);
+    for (u32 i = 0; i < k; i++) host_res[2 * i] = host_res[twin + 2 * i] = ~0ull;
     CUDA_OK(cudaMemcpyAsync(res.p, host_res.data(), host_res.size() * sizeof(u64), cudaMemcpyHostToDevice, stream));
+    jit_check_used.assign(k, 0);
+    std::vector<u32> first_use;
     for (u32 i = 0; i < k; i++) {
         mk::CheckArgs& c = ca[i];
         c.row0 = 0; c.n_rows = (size_t)1 << c.log_n;
         c.first = (unsigned long long*)(res.p + 2 * i); c.failing_rows = (unsigned long long*)(res.p + 2 * i + 1);
-        if (mk::launch_check_rows(c, stream) != 0) fail(MDN_ERR_UNSUPPORTED, "AIR %u: constraint program too large for the interpreter", i);
+        std::shared_ptr<jit::Kernel>& kn = airs[i].check_jit;
+        if (kn && kn->checked < 0) kn.reset();   // failed its self-check earlier in this session
+        if (!kn) {
+            if (mk::launch_check_rows(c, stream) != 0) fail(MDN_ERR_UNSUPPORTED, "AIR %u: constraint program too large for the interpreter", i);
+            continue;
+        }
+        jit::CheckJitArgs ja = check_jit_args(c);
+        ja.first = c.first; ja.failing_rows = c.failing_rows; ja.row0 = c.row0; ja.n_rows = c.n_rows;
+        try { kn->launch(ja, (unsigned)((c.n_rows + 127) / 128), 128, stream); }
+        catch (const std::exception& e) { fail(MDN_ERR_CUDA, "%s", e.what()); }
+        mk::count_launch();
+        jit_check_used[i] = 1;
+        if (kn->checked == 0) {
+            // first use of this kernel in the session: the interpreter checks the same rows into its own two words
+            mk::CheckArgs t = c;
+            t.first = (unsigned long long*)(res.p + twin + 2 * i); t.failing_rows = (unsigned long long*)(res.p + twin + 2 * i + 1);
+            if (mk::launch_check_rows(t, stream) != 0) fail(MDN_ERR_UNSUPPORTED, "AIR %u: constraint program too large for the interpreter", i);
+            first_use.push_back(i);
+        }
     }
-    CUDA_OK(cudaMemcpyAsync(host_res.data(), res.p, 2 * (size_t)k * sizeof(u64), cudaMemcpyDeviceToHost, stream));
+    CUDA_OK(cudaMemcpyAsync(host_res.data(), res.p, host_res.size() * sizeof(u64), cudaMemcpyDeviceToHost, stream));
     CUDA_OK(cudaStreamSynchronize(stream));
     CUDA_OK(cudaGetLastError());
+    for (u32 i : first_use) {
+        jit::Kernel& kn = *airs[i].check_jit;
+        if (host_res[2 * i] != host_res[twin + 2 * i] || host_res[2 * i + 1] != host_res[twin + 2 * i + 1]) {
+            // a compiler defect: the interpreter's words stand, the kernel is retired
+            host_res[2 * i] = host_res[twin + 2 * i]; host_res[2 * i + 1] = host_res[twin + 2 * i + 1];
+            kn.checked = -1; jit_check_used[i] = 0;
+            jit_note = "NVRTC check kernel disagreed with the interpreter on its first use; interpreter kept";
+        } else if (kn.checked == 0) kn.checked = 1;
+    }
 
     memset(out, 0, sizeof *out);
     for (u32 i = 0; i < k; i++) out->failing_rows += host_res[2 * i + 1];
@@ -1604,7 +1666,7 @@ void mdn_session::guard_constraints(const std::vector<u64>& flat_values) {
 // the external check's outcome.
 void mdn_session::prepare_check(const mdn_statement* st, const mdn_matrix* traces, const mdn_matrix* prep, const mdn_challenger* chal,
                                 mdn_aux_builder build_aux, void* aux_ctx, u32 flags, const void* out, CheckSetup& cs) {
-    const auto [cm, on_device, k] = start_check(st, traces, chal, flags, out);
+    const auto [cm, on_device, k] = start_check(st, traces, chal, flags, out, true);
     const bool dev_built = cm && dev_aux;   // aux traces from the device aux builder
     // the preprocessed traces come with the call (debug.rs re-materialises BaseAir::preprocessed_trace), not from the
     // session's committed bundle
@@ -1744,6 +1806,8 @@ void mdn_session::constraint_census(const mdn_statement* st, const mdn_matrix* t
     CUDA_OK(cudaMemsetAsync(words.p, 0, 2 * sizeof(u64), stream));
     u32* d_counts = reinterpret_cast<u32*>(counts.p);
     std::vector<mk::CensusArgs> ca(k);
+    jit_check_used.assign(k, 0);
+    u64 checked_rows = 0;   // failing rows of AIRs whose row pass was compared on first use (not in words[0])
     for (u32 i = 0; i < k; i++) {
         const u32 j = cs.pos[i];
         mk::CensusArgs& c = ca[i];
@@ -1754,7 +1818,49 @@ void mdn_session::constraint_census(const mdn_statement* st, const mdn_matrix* t
         c.tally = (unsigned long long*)(tally.p + tally_base[i]);
         c.failing_rows = (unsigned long long*)words.p;
         c.offsets = offsets.p + row_base[i];
-        if (mk::launch_census_rows(c, stream) != 0) fail(MDN_ERR_UNSUPPORTED, "AIR %u: constraint program too large for the interpreter", i);
+        std::shared_ptr<jit::Kernel>& kn = airs[i].census_jit;
+        if (kn && kn->checked < 0) kn.reset();   // failed its self-check earlier in this session
+        if (!kn) {
+            if (mk::launch_census_rows(c, stream) != 0) fail(MDN_ERR_UNSUPPORTED, "AIR %u: constraint program too large for the interpreter", i);
+            continue;
+        }
+        const size_t N = (size_t)1 << c.log_n, nt = 3 * (size_t)c.n_cons;
+        jit::CheckJitArgs ja = check_jit_args(c);
+        ja.failing_rows = c.failing_rows; ja.row_count = c.row_count; ja.tally = c.tally; ja.n_cons = c.n_cons;
+        // first use of this kernel in the session: the kernel's failing rows go to a word of their own, and the
+        // interpreter runs the same rows into its own counts, tally and word; all three must agree word for word
+        DevBuf twin;
+        if (kn->checked == 0) {
+            twin.alloc((N + 1) / 2 + nt + 2, stream);
+            CUDA_OK(cudaMemcpyAsync(twin.p + (N + 1) / 2, host_tally.data() + tally_base[i], nt * sizeof(u64), cudaMemcpyHostToDevice, stream));
+            CUDA_OK(cudaMemsetAsync(twin.p + (N + 1) / 2 + nt, 0, 2 * sizeof(u64), stream));
+            ja.failing_rows = (unsigned long long*)(twin.p + (N + 1) / 2 + nt);
+        }
+        try { kn->launch(ja, (unsigned)((N + 127) / 128), 128, stream); }
+        catch (const std::exception& e) { fail(MDN_ERR_CUDA, "%s", e.what()); }
+        mk::count_launch();
+        jit_check_used[i] = 1;
+        if (kn->checked != 0) continue;
+        mk::CensusArgs t = c;
+        t.row_count = reinterpret_cast<u32*>(twin.p); t.tally = (unsigned long long*)(twin.p + (N + 1) / 2);
+        t.failing_rows = (unsigned long long*)(twin.p + (N + 1) / 2 + nt + 1);
+        if (mk::launch_census_rows(t, stream) != 0) fail(MDN_ERR_UNSUPPORTED, "AIR %u: constraint program too large for the interpreter", i);
+        std::vector<u32> cnt_j(N), cnt_i(N);
+        std::vector<u64> tw(nt + 2), tj(std::max<size_t>(1, nt));
+        CUDA_OK(cudaMemcpyAsync(cnt_j.data(), c.row_count, N * sizeof(u32), cudaMemcpyDeviceToHost, stream));
+        CUDA_OK(cudaMemcpyAsync(cnt_i.data(), twin.p, N * sizeof(u32), cudaMemcpyDeviceToHost, stream));
+        if (nt) CUDA_OK(cudaMemcpyAsync(tj.data(), c.tally, nt * sizeof(u64), cudaMemcpyDeviceToHost, stream));
+        CUDA_OK(cudaMemcpyAsync(tw.data(), twin.p + (N + 1) / 2, (nt + 2) * sizeof(u64), cudaMemcpyDeviceToHost, stream));
+        CUDA_OK(cudaStreamSynchronize(stream));
+        CUDA_OK(cudaGetLastError());
+        if (cnt_j != cnt_i || !std::equal(tj.begin(), tj.begin() + nt, tw.begin()) || tw[nt] != tw[nt + 1]) {
+            // a compiler defect: the interpreter's counts and tally stand, the kernel is retired
+            CUDA_OK(cudaMemcpyAsync(c.row_count, twin.p, N * sizeof(u32), cudaMemcpyDeviceToDevice, stream));
+            if (nt) CUDA_OK(cudaMemcpyAsync(c.tally, twin.p + (N + 1) / 2, nt * sizeof(u64), cudaMemcpyDeviceToDevice, stream));
+            kn->checked = -1; jit_check_used[i] = 0;
+            jit_note = "NVRTC check kernel disagreed with the interpreter on its first use; interpreter kept";
+        } else kn->checked = 1;
+        checked_rows += tw[nt + 1];
     }
     mk::launch_count_exclusive_scan(d_counts, rows, offsets.p, words.p + 1, scratch.p, stream);
     u64 host_words[2];
@@ -1762,6 +1868,7 @@ void mdn_session::constraint_census(const mdn_statement* st, const mdn_matrix* t
     CUDA_OK(cudaMemcpyAsync(host_words, words.p, sizeof host_words, cudaMemcpyDeviceToHost, stream));
     CUDA_OK(cudaStreamSynchronize(stream));
     CUDA_OK(cudaGetLastError());
+    host_words[0] += checked_rows;
 
     // the failing (instance, constraint) pairs in order, and the least failure: the first failing instance's least
     // (first_row, constraint)
@@ -2899,7 +3006,7 @@ void mdn_session_destroy(mdn_session* s) {
     s->prep_c = Committed();
     s->d_publics.release(); s->d_randomness.release(); s->d_aux_values.release(); s->d_flag.release();
     s->ntt_plans.clear(); s->premul_plans.clear();
-    for (auto& a : s->airs) a.jit.reset();
+    for (auto& a : s->airs) { a.jit.reset(); a.check_jit.reset(); a.census_jit.reset(); }
     s->jit_kernels.clear();
     cudaStreamSynchronize(s->stream);
     s->arena.destroy();
@@ -3132,6 +3239,7 @@ long long mdn_get_info(mdn_session* s, mdn_info what, uint64_t* out, size_t cap)
         case MDN_INFO_FRI_ROOTS: v = s->dbg_fri_roots; break;
         case MDN_INFO_QUERY_INDICES: v = s->dbg_queries; break;
         case MDN_INFO_JIT: v = s->jit_used; break;
+        case MDN_INFO_JIT_CHECK: v = s->jit_check_used; break;
         case MDN_INFO_POOL: {
             cudaMemPool_t pool; uint64_t a[4] = {0, 0, 0, 0};
             if (cudaDeviceGetDefaultMemPool(&pool, s->device) == cudaSuccess) {
@@ -3278,7 +3386,7 @@ long long mdn_jit_compile_check(const uint32_t* program, uint32_t program_words,
                 if ((it[1] != 0xFFFFFFFFu && it[1] >= program[2]) || it[2] >= program[2] || it[3] >= program[2] || it[0] >= 16) { msg = "bad interaction"; if (err) *err = msg.c_str(); return MDN_ERR_INVALID_ARG; }
                 n_cols = std::max(n_cols, it[0] + 1);
             }
-            return (long long)jit::cubin_for(program, program_words, nullptr, true, n_cols).size();
+            return (long long)jit::cubin_for(program, program_words, nullptr, jit::MODE_LOOKUP, n_cols).size();
         }
         for (u32 q = 0; q < program[3]; q++) if (program[5 + 3 * (size_t)program[2] + q] >= program[2]) { msg = "bad constraint id"; if (err) *err = msg.c_str(); return MDN_ERR_INVALID_ARG; }
         return (long long)jit::cubin_for(program, program_words, nullptr).size();
