@@ -556,6 +556,56 @@ int mdn_check_lookup_folds(mdn_session* s, const mdn_statement* st, const mdn_ma
                            uint64_t* const* folds_out /* NULL, or per AIR NULL or rows x num_columns x 4 u64 */,
                            uint32_t flags, mdn_fold_report* out);
 
+/* ---- list every disagreement between an aux trace and its lookup program, without proving: the census of
+ * mdn_check_lookup_folds ----------------------------------------------------------------------------------------
+ * The same inputs, validation, messages, trace layouts and refusals as mdn_check_lookup_folds without folds_out (aux ==
+ * NULL: the device LogUp build of the same call, so that every row where a flag is not boolean or two flags of a group
+ * are set together is listed); the verdict of every (instance, row, column) is the one mdn_check_lookup_folds gives:
+ * kind 3 where U_c is zero, kind 1 for a fraction column that differs, kind 2 for column 0 when its delta differs and no
+ * U of that row is zero (a row with a zero U lists no column-0 entry).  Every one with kind != 0 is kept:
+ *   failures : host, room for max_failures (NULL iff max_failures == 0): the first max_failures disagreements in
+ *              (instance, row, column) order, instance order as in mdn_check_lookup_folds.
+ *   tallies  : host, room for max_tallies (NULL iff max_tallies == 0): each (instance, column) that disagrees on at least
+ *              one row, in (instance, column) order, truncated to max_tallies.
+ *   out      : the counts; out->first is field for field the report mdn_check_lookup_folds gives for the same call (the
+ *              first failing instance's least (first_row, column) of the tallies, its values probed at that row).
+ * A NULL list with a non-zero capacity, or a NULL out, is MDN_ERR_INVALID_ARG before any device work; a failure list
+ * whose device staging is larger than the free device memory MDN_ERR_UNSUPPORTED.  The outputs do not depend on the
+ * order in which device atomics ran: two calls on the same inputs give byte-identical outputs.  Refused, as
+ * mdn_check_lookup_folds, inside a staged proof and on a session split over ranks; uses and releases the proof arena;
+ * leaves mdn_get_info, mdn_get_timings and later proofs unchanged.  Interpreted whatever the program's size. */
+typedef struct {                 /* one (instance, row, column) where the aux trace departs from the fold */
+    uint32_t instance, column;
+    uint32_t kind;               /* 1, 2 or 3 exactly as mdn_fold_report.kind */
+    uint32_t reserved;
+    uint64_t row;
+    uint64_t fold[4];            /* (V c0, V c1, U c0, U c1) of that (row, column) */
+    uint64_t expected[2], actual[2];   /* as mdn_fold_report: the same conventions for every kind and column */
+} mdn_fold_failure;              /* 88 bytes */
+typedef struct {                 /* one (instance, column) that disagrees on at least one row */
+    uint32_t instance, column;
+    uint64_t failing_rows;       /* rows where this column has kind != 0 */
+    uint64_t zero_u_rows;        /* of those, rows of kind 3 (U_c == 0) */
+    uint64_t first_row, last_row;
+    uint32_t first_kind, reserved;
+    uint64_t first_expected[2], first_actual[2];   /* at first_row */
+} mdn_fold_tally;                /* 80 bytes */
+typedef struct {
+    mdn_fold_report first;       /* field for field what mdn_check_lookup_folds returns for the same call */
+    uint64_t disagreements;      /* (instance, row, column) triples with kind != 0 */
+    uint64_t n_failures;         /* = min(disagreements, max_failures) written to failures[] */
+    uint64_t failing_columns;    /* (instance, column) pairs with failing_rows > 0 */
+    uint64_t n_tallies;          /* = min(failing_columns, max_tallies) written to tallies[] */
+} mdn_fold_census_report;
+int mdn_lookup_fold_census(mdn_session* s, const mdn_statement* st, const mdn_matrix* traces /* instance order */,
+                           const uint64_t* randomness /* 2 * max num_randomness: alpha, beta, ... */,
+                           const uint32_t* const* fold_marks /* per AIR, NULL or one word per interaction; NULL = none */,
+                           const mdn_matrix* aux /* instance order, width 2 * aux_width; NULL: the device LogUp build */,
+                           const uint64_t* const* aux_finals /* per AIR 2 u64; NULL with aux == NULL */, uint32_t flags,
+                           mdn_fold_failure* failures, uint64_t max_failures,
+                           mdn_fold_tally* tallies, uint64_t max_tallies,
+                           mdn_fold_census_report* out);
+
 /* wincode/bincode-default layout of StarkProofData (prover/src/lib.rs:347-354): u64-LE length +
  * height bytes; u64-LE length + u64-LE felts; u64-LE length + 32-byte commitments.  Returns the
  * number of bytes needed; writes only if cap is large enough.  (Layout unpinned in-tree.) */
@@ -609,7 +659,8 @@ size_t mdn_abi_layout(uint32_t* out, size_t cap);
  * is absent) run on the op-list interpreter.  Both produce identical values.  Specialised: the proof's constraint
  * evaluation and LogUp row build (MDN_INFO_JIT), and the row pass of mdn_check_constraints, mdn_constraint_census and
  * the constraint guard (MDN_INFO_JIT_CHECK).  Interpreted whatever the size: the lookup checks
- * (mdn_check_trace_balance, mdn_check_lookup_folds), the census's failure listing and the checks' one-row probes.
+ * (mdn_check_trace_balance, mdn_check_lookup_folds, mdn_lookup_fold_census), the census's failure listing and the checks'
+ * one-row probes.
  * Each compiled kernel is compared word for word with the interpreter on its first use in a session. */
 int mdn_session_set_jit(mdn_session* s, uint32_t min_nodes);
 /* "nvrtc <version>" or why it is unavailable, plus the reason the last JIT attempt was dropped (compile error,

@@ -286,6 +286,47 @@ pub struct MdnFoldReport {
     pub reserved: u32,
 }
 
+/// `mdn_fold_failure`: one (instance, row, column) where the aux trace departs from the fold (kind as `MdnFoldReport`).
+#[repr(C)]
+#[derive(Clone, Copy, Debug, Default)]
+pub struct MdnFoldFailure {
+    pub instance: u32,
+    pub column: u32,
+    pub kind: u32,
+    pub reserved: u32,
+    pub row: u64,
+    pub fold: [u64; 4],
+    pub expected: [u64; 2],
+    pub actual: [u64; 2],
+}
+
+/// `mdn_fold_tally`: one (instance, column) that disagrees on at least one row.
+#[repr(C)]
+#[derive(Clone, Copy, Debug, Default)]
+pub struct MdnFoldTally {
+    pub instance: u32,
+    pub column: u32,
+    pub failing_rows: u64,
+    pub zero_u_rows: u64,
+    pub first_row: u64,
+    pub last_row: u64,
+    pub first_kind: u32,
+    pub reserved: u32,
+    pub first_expected: [u64; 2],
+    pub first_actual: [u64; 2],
+}
+
+/// `mdn_fold_census_report`: the counts of `mdn_lookup_fold_census`; `first` is what `mdn_check_lookup_folds` reports.
+#[repr(C)]
+#[derive(Clone, Copy, Debug, Default)]
+pub struct MdnFoldCensus {
+    pub first: MdnFoldReport,
+    pub disagreements: u64,
+    pub n_failures: u64,
+    pub failing_columns: u64,
+    pub n_tallies: u64,
+}
+
 pub enum MdnSession {}
 
 /// `mdn_hash_kind` (include/miden_b200.h): which `miden_air::config` constructor the session follows.
@@ -392,6 +433,22 @@ unsafe extern "C" {
         folds_out: *const *mut u64,
         flags: u32,
         out: *mut MdnFoldReport,
+    ) -> c_int;
+    /// Declared only; like the rest of the crate, not compiled yet.
+    pub fn mdn_lookup_fold_census(
+        s: *mut MdnSession,
+        st: *const MdnStatement,
+        traces: *const MdnMatrix,
+        randomness: *const u64,
+        fold_marks: *const *const u32,
+        aux: *const MdnMatrix,
+        aux_finals: *const *const u64,
+        flags: u32,
+        failures: *mut MdnFoldFailure,
+        max_failures: u64,
+        tallies: *mut MdnFoldTally,
+        max_tallies: u64,
+        out: *mut MdnFoldCensus,
     ) -> c_int;
     pub fn mdn_session_set_preprocessed(
         s: *mut MdnSession,

@@ -129,6 +129,25 @@ def fold_report_dict(rep: FoldReport) -> dict:
                 n_skipped_airs=rep.n_skipped_airs)
 
 
+class FoldFailure(C.Structure):
+    """`mdn_fold_failure`: one (instance, row, column) where the aux trace departs from the fold (kind as FoldReport)."""
+    _fields_ = [("instance", C.c_uint32), ("column", C.c_uint32), ("kind", C.c_uint32), ("reserved", C.c_uint32),
+                ("row", C.c_uint64), ("fold", C.c_uint64 * 4), ("expected", C.c_uint64 * 2), ("actual", C.c_uint64 * 2)]
+
+
+class FoldTally(C.Structure):
+    """`mdn_fold_tally`: one (instance, column) that disagrees on at least one row."""
+    _fields_ = [("instance", C.c_uint32), ("column", C.c_uint32), ("failing_rows", C.c_uint64), ("zero_u_rows", C.c_uint64),
+                ("first_row", C.c_uint64), ("last_row", C.c_uint64), ("first_kind", C.c_uint32), ("reserved", C.c_uint32),
+                ("first_expected", C.c_uint64 * 2), ("first_actual", C.c_uint64 * 2)]
+
+
+class FoldCensus(C.Structure):
+    """`mdn_fold_census_report`: the counts of mdn_lookup_fold_census; `first` is mdn_check_lookup_folds' report."""
+    _fields_ = [("first", FoldReport), ("disagreements", C.c_uint64), ("n_failures", C.c_uint64),
+                ("failing_columns", C.c_uint64), ("n_tallies", C.c_uint64)]
+
+
 BOUNDARY = 0xFFFFFFFF     # instance / column of a boundary emission in a balance report (row = 2^64 - 1)
 
 
@@ -164,6 +183,7 @@ EXPORTS = [
     "mdn_session_set_external_check", "mdn_session_set_hash", "mdn_session_set_hash_challenger",
     "mdn_check_constraints", "mdn_session_set_device_aux_builder", "mdn_check_trace_balance",
     "mdn_check_lookup_folds", "mdn_constraint_census", "mdn_session_set_constraint_guard", "mdn_last_constraint_report",
+    "mdn_lookup_fold_census",
 ]
 ERR_CONSTRAINT_VIOLATED = -8
 
@@ -214,6 +234,9 @@ def lib():
         L.mdn_check_lookup_folds.argtypes = [C.c_void_p, C.POINTER(Statement), C.POINTER(Matrix), u64p, C.POINTER(u32p),
                                              C.POINTER(Matrix), C.POINTER(u64p), C.POINTER(u64p), C.c_uint32,
                                              C.POINTER(FoldReport)]
+        L.mdn_lookup_fold_census.argtypes = [C.c_void_p, C.POINTER(Statement), C.POINTER(Matrix), u64p, C.POINTER(u32p),
+                                             C.POINTER(Matrix), C.POINTER(u64p), C.c_uint32, C.POINTER(FoldFailure), C.c_uint64,
+                                             C.POINTER(FoldTally), C.c_uint64, C.POINTER(FoldCensus)]
         L.mdn_prove_begin.argtypes = [C.c_void_p, C.POINTER(Statement), C.POINTER(Matrix), C.POINTER(Challenger),
                                       C.c_uint32, u64p, u64p]
         L.mdn_prove_commit_aux.argtypes = [C.c_void_p, C.POINTER(Matrix), C.POINTER(u64p), u64p]
@@ -451,21 +474,8 @@ class Session:
         aux: Matrix array in instance order (host row-major, or device as `flags` say) with aux_finals, per AIR None or
         (c0, c1) -- or None for the device LogUp build of the same call; folds_out: per AIR None, a uint64 numpy array of
         rows * num_columns * 4 words to fill, or a device address (int) with FLAG_DEVICE_TRACES.  Returns fold_report_dict."""
-        rnd = np.ascontiguousarray(np.asarray(randomness, dtype=np.uint64).reshape(-1))
-        n, keep = statement.n_airs, []
-        marks = fins = outs = None
-        if fold_marks is not None:
-            marks = (u32p * n)()
-            for i, m in enumerate(fold_marks):
-                if m is not None:
-                    keep.append(np.ascontiguousarray(m, dtype=np.uint32))
-                    marks[i] = keep[-1].ctypes.data_as(u32p)
-        if aux_finals is not None:
-            fins = (u64p * n)()
-            for i, f in enumerate(aux_finals):
-                if f is not None:
-                    keep.append(np.array([int(f[0]), int(f[1])], dtype=np.uint64))
-                    fins[i] = ptr(keep[-1])
+        rnd, marks, fins, keep = _fold_inputs(statement, randomness, fold_marks, aux_finals)
+        n, outs = statement.n_airs, None
         if folds_out is not None:
             outs = (u64p * n)()
             for i, o in enumerate(folds_out):
@@ -475,6 +485,21 @@ class Session:
         self._check(lib().mdn_check_lookup_folds(self._h, C.byref(statement), traces, ptr(rnd) if rnd.size else None, marks,
                                                  aux, fins, outs, flags, C.byref(rep)))
         return fold_report_dict(rep)
+
+    def lookup_fold_census(self, statement: Statement, traces, randomness, fold_marks=None, aux=None, aux_finals=None,
+                           flags=0, max_failures: int = 1 << 16, max_tallies: int = 1 << 16):
+        """check_lookup_folds without stopping at the first disagreement: every (instance, row, column) of non-zero kind.
+        The arguments are those of check_lookup_folds without folds_out.  Returns (FoldCensus, failures, tallies), with
+        `failures` the first min(disagreements, max_failures) FoldFailure in (instance, row, column) order and `tallies`
+        the first min(failing_columns, max_tallies) FoldTally in (instance, column) order."""
+        rnd, marks, fins, keep = _fold_inputs(statement, randomness, fold_marks, aux_finals)
+        out = FoldCensus()
+        fails = (FoldFailure * max(1, max_failures))()
+        tallies = (FoldTally * max(1, max_tallies))()
+        self._check(lib().mdn_lookup_fold_census(self._h, C.byref(statement), traces, ptr(rnd) if rnd.size else None, marks,
+                                                 aux, fins, flags, fails if max_failures else None, max_failures,
+                                                 tallies if max_tallies else None, max_tallies, C.byref(out)))
+        return out, list(fails[: out.n_failures]), list(tallies[: out.n_tallies])
 
     def info(self, what: int, cap: int = 0) -> np.ndarray:
         n = lib().mdn_get_info(self._h, what, None, 0)
@@ -489,6 +514,26 @@ class Session:
         t = Timings()
         self._check(lib().mdn_get_timings(self._h, C.byref(t)))
         return t
+
+
+def _fold_inputs(statement, randomness, fold_marks, aux_finals):
+    """(randomness, fold marks, aux finals, arrays to keep alive) as the two lookup fold checks take them."""
+    rnd = np.ascontiguousarray(np.asarray(randomness, dtype=np.uint64).reshape(-1))
+    n, keep = statement.n_airs, []
+    marks = fins = None
+    if fold_marks is not None:
+        marks = (u32p * n)()
+        for i, m in enumerate(fold_marks):
+            if m is not None:
+                keep.append(np.ascontiguousarray(m, dtype=np.uint32))
+                marks[i] = keep[-1].ctypes.data_as(u32p)
+    if aux_finals is not None:
+        fins = (u64p * n)()
+        for i, f in enumerate(aux_finals):
+            if f is not None:
+                keep.append(np.array([int(f[0]), int(f[1])], dtype=np.uint64))
+                fins[i] = ptr(keep[-1])
+    return rnd, marks, fins, keep
 
 
 def device_matrices(tensors):

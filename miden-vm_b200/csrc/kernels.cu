@@ -1239,15 +1239,13 @@ void launch_balance_finish(const BalanceTable& t, unsigned long long* counters, 
 // LogUp constraint-path folds (debug/trace collect_column_oracle_folds): the lookup program of k_logup_rows folded
 // batch by batch and group by group as DebugTraceBuilder folds it, compared with an aux trace (kernels.cuh LookupFoldArgs)
 // =============================================================================================
-template <int MAXS>
-__global__ void __launch_bounds__(128) k_fold_rows(LookupFoldArgs a) {
-    size_t N = (size_t)1 << a.log_n;
-    size_t r = a.row0 + (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (r >= a.row0 + a.n_rows) return;
+// The fold of row r shared by the fold kernels (k_fold_rows, k_fold_census_rows, k_fold_census_list), which name their
+// inputs alike (kernels.cuh LookupFoldArgs, FoldCensusArgs).  fold_walk: (V_c, U_c) of every column.
+template <int MAXS, class Args>
+__device__ __forceinline__ void fold_walk(const Args& a, size_t N, size_t r, E2* V, E2* U) {
     size_t rn = (r + 1) & (N - 1);
     size_t per_row = (r & (((size_t)1 << a.prog.log_max_period) - 1)) * a.prog.n_periodic;
     E2 slot[MAXS];
-    E2 V[LOGUP_MAX_COLS], U[LOGUP_MAX_COLS], F[LOGUP_MAX_COLS];
     for (u32 c = 0; c < a.n_cols; c++) { V[c] = gl::e2(0, 0); U[c] = gl::e2(1, 0); }
     const E2 zero = gl::e2(0, 0), one = gl::e2(1, 0);
     E2 bn = zero, bd = one, vg = zero, ug = one;   // the open batch (N, D) and the open group (V_g, U_g)
@@ -1285,6 +1283,49 @@ __global__ void __launch_bounds__(128) k_fold_rows(LookupFoldArgs a) {
     }
     close_batch();
     close_group();
+}
+// fold_divide: F[c] = V_c / U_c with one inversion (Montgomery's trick over the columns whose U is non-zero), F[c] = 0
+// where U_c is zero; returns the mask of those columns, `total` = the sum of the F[c]
+__device__ __forceinline__ u32 fold_divide(u32 n_cols, const E2* V, const E2* U, E2* F, E2& total) {
+    u32 zero_mask = 0;
+    E2 acc = gl::e2(1, 0);
+    for (u32 c = 0; c < n_cols; c++) {
+        F[c] = acc;
+        if ((U[c].a | U[c].b) == 0) zero_mask |= 1u << c; else acc = gl::e2_mul(acc, U[c]);
+    }
+    E2 inv = gl::e2_inv(acc);
+    total = gl::e2(0, 0);
+    for (u32 c = n_cols; c-- > 0;) {
+        if ((zero_mask >> c) & 1) { F[c] = gl::e2(0, 0); continue; }
+        F[c] = gl::e2_mul(V[c], gl::e2_mul(inv, F[c]));
+        inv = gl::e2_mul(inv, U[c]);
+        total = gl::e2_add(total, F[c]);
+    }
+    return zero_mask;
+}
+// fold_verdict: the kind of column c at row r (0 agrees, 1 fraction column, 2 accumulator, 3 zero U) with its expected
+// and actual values: column c >= 1 against aux[r][c]; column 0, when no U of the row is zero, the row's total against
+// aux[r + 1][0] - aux[r][0] (`final` closes the last row)
+template <class Args>
+__device__ __forceinline__ u32 fold_verdict(const Args& a, size_t N, size_t r, u32 c, const E2* F, E2 total, u32 zero_mask,
+                                            E2& expected, E2& actual) {
+    expected = F[c]; actual = gl::e2(a.aux_cm[(size_t)(2 * c) * N + r], a.aux_cm[(size_t)(2 * c + 1) * N + r]);
+    if (c == 0) {
+        E2 next = r == N - 1 ? a.final : gl::e2(a.aux_cm[r + 1], a.aux_cm[N + r + 1]);
+        expected = total; actual = gl::e2_sub(next, actual);
+    }
+    if ((zero_mask >> c) & 1) return 3;
+    if (c == 0 ? (zero_mask == 0 && !gl::e2_eq(expected, actual)) : !gl::e2_eq(expected, actual)) return c ? 1 : 2;
+    return 0;
+}
+
+template <int MAXS>
+__global__ void __launch_bounds__(128) k_fold_rows(LookupFoldArgs a) {
+    size_t N = (size_t)1 << a.log_n;
+    size_t r = a.row0 + (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= a.row0 + a.n_rows) return;
+    E2 V[LOGUP_MAX_COLS], U[LOGUP_MAX_COLS], F[LOGUP_MAX_COLS];
+    fold_walk<MAXS>(a, N, r, V, U);
 
     if (a.folds_out && a.folds_cm) {
         for (u32 c = 0; c < a.n_cols; c++) {
@@ -1296,30 +1337,13 @@ __global__ void __launch_bounds__(128) k_fold_rows(LookupFoldArgs a) {
         for (u32 c = 0; c < a.n_cols; c++) { o[2 * c] = make_ulonglong2(V[c].a, V[c].b); o[2 * c + 1] = make_ulonglong2(U[c].a, U[c].b); }
     }
 
-    // F[c] = V_c / U_c with one inversion (Montgomery's trick over the columns whose U is non-zero)
-    u32 zero_mask = 0, n_zero = 0;
-    E2 acc = one;
+    E2 total;
+    const u32 zero_mask = fold_divide(a.n_cols, V, U, F, total);
+    u32 first_c = 0xFFFFFFFFu, n_zero = 0;
     for (u32 c = 0; c < a.n_cols; c++) {
-        F[c] = acc;
-        if ((U[c].a | U[c].b) == 0) { zero_mask |= 1u << c; n_zero++; } else acc = gl::e2_mul(acc, U[c]);
-    }
-    E2 inv = gl::e2_inv(acc), total = zero;
-    for (u32 c = a.n_cols; c-- > 0;) {
-        if ((zero_mask >> c) & 1) { F[c] = zero; continue; }
-        F[c] = gl::e2_mul(V[c], gl::e2_mul(inv, F[c]));
-        inv = gl::e2_mul(inv, U[c]);
-        total = gl::e2_add(total, F[c]);
-    }
-    u32 first_c = 0xFFFFFFFFu;
-    for (u32 c = 0; c < a.n_cols; c++) {
-        E2 expected = F[c], actual = gl::e2(a.aux_cm[(size_t)(2 * c) * N + r], a.aux_cm[(size_t)(2 * c + 1) * N + r]);
-        u32 kind = 0;
-        if (c == 0) {
-            E2 next = r == N - 1 ? a.final : gl::e2(a.aux_cm[r + 1], a.aux_cm[N + r + 1]);
-            expected = total; actual = gl::e2_sub(next, actual);
-        }
-        if ((zero_mask >> c) & 1) kind = 3;
-        else if (c == 0 ? (zero_mask == 0 && !gl::e2_eq(expected, actual)) : !gl::e2_eq(expected, actual)) kind = c ? 1 : 2;
+        E2 expected, actual;
+        u32 kind = fold_verdict(a, N, r, c, F, total, zero_mask, expected, actual);
+        n_zero += kind == 3;
         if (kind && first_c == 0xFFFFFFFFu) first_c = c;
         if (a.probe && c == a.probe_col) {
             a.probe[0] = kind;
@@ -1341,6 +1365,115 @@ int launch_fold_rows(const LookupFoldArgs& a, cudaStream_t st) {
     else if (a.prog.n_slots <= 64) k_fold_rows<64><<<blocks, 128, 0, st>>>(a);
     else if (a.prog.n_slots <= 256) k_fold_rows<256><<<blocks, 128, 0, st>>>(a);
     else if (a.prog.n_slots <= 1024) k_fold_rows<1024><<<blocks, 128, 0, st>>>(a);
+    else return -1;
+    COUNT_LAUNCH();
+    return 0;
+}
+
+// =============================================================================================
+// LogUp fold census (every disagreement, not only the first): the fold and verdict of k_fold_rows counted per row and
+// tallied per column, then listed in (row, column) order from an exclusive scan of the per-row counts (kernels.cuh
+// FoldCensusArgs)
+// =============================================================================================
+template <int MAXS>
+__global__ void __launch_bounds__(128) k_fold_census_rows(FoldCensusArgs a) {
+    // per-block tally of each column: disagreeing rows, those with a zero U, least and greatest row (rows fit 32 bits)
+    __shared__ u32 s_cnt[LOGUP_MAX_COLS], s_zero[LOGUP_MAX_COLS], s_min[LOGUP_MAX_COLS], s_max[LOGUP_MAX_COLS];
+    __shared__ u32 s_rows;
+    for (u32 c = threadIdx.x; c < a.n_cols; c += blockDim.x) { s_cnt[c] = 0; s_zero[c] = 0; s_min[c] = 0xFFFFFFFFu; s_max[c] = 0; }
+    if (threadIdx.x == 0) s_rows = 0;
+    __syncthreads();
+    size_t N = (size_t)1 << a.log_n;
+    size_t r = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (r < N) {
+        E2 V[LOGUP_MAX_COLS], U[LOGUP_MAX_COLS], F[LOGUP_MAX_COLS];
+        fold_walk<MAXS>(a, N, r, V, U);
+        E2 total;
+        const u32 zero_mask = fold_divide(a.n_cols, V, U, F, total);
+        u32 n_fail = 0;
+        for (u32 c = 0; c < a.n_cols; c++) {
+            E2 expected, actual;
+            u32 kind = fold_verdict(a, N, r, c, F, total, zero_mask, expected, actual);
+            if (!kind) continue;
+            n_fail++;
+            atomicAdd(&s_cnt[c], 1u);
+            if (kind == 3) atomicAdd(&s_zero[c], 1u);
+            atomicMin(&s_min[c], (u32)r); census_max(&s_max[c], (u32)r);
+        }
+        a.row_count[r] = n_fail;
+        if (n_fail) atomicAdd(&s_rows, 1u);
+    }
+    __syncthreads();
+    // one global update per (block, disagreeing column)
+    for (u32 c = threadIdx.x; c < a.n_cols; c += blockDim.x) {
+        if (!s_cnt[c]) continue;
+        atomicAdd(&a.tally[4 * c], (unsigned long long)s_cnt[c]);
+        if (s_zero[c]) atomicAdd(&a.tally[4 * c + 1], (unsigned long long)s_zero[c]);
+        atomicMin(&a.tally[4 * c + 2], (unsigned long long)s_min[c]);
+        census_max(&a.tally[4 * c + 3], (unsigned long long)s_max[c]);
+    }
+    if (threadIdx.x == 0 && s_rows) atomicAdd(a.failing_rows, (unsigned long long)s_rows);
+}
+
+// list mode: rows with disagreements whose first slot is below max_failures write one record per disagreeing column in
+// ascending column order from slot offsets[r]; probe mode: thread p writes the record of (row, column) = probes[2p],
+// probes[2p + 1]
+template <int MAXS>
+__global__ void __launch_bounds__(128) k_fold_census_list(FoldCensusArgs a) {
+    size_t N = (size_t)1 << a.log_n;
+    size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    size_t r;
+    u32 want;             // the probed column, or 0xFFFFFFFF: every disagreeing one
+    u64 o, end;           // record slots [o, end) of this thread
+    if (a.probes) {
+        if (t >= a.n_probes) return;
+        r = a.probes[2 * t]; want = (u32)a.probes[2 * t + 1]; o = t; end = t + 1;
+    } else {
+        if (t >= N) return;
+        r = t;
+        u32 cnt = a.row_count[r];
+        if (!cnt) return;
+        o = a.offsets[r];
+        if (o >= a.max_failures) return;
+        want = 0xFFFFFFFFu; end = o + cnt < a.max_failures ? o + cnt : a.max_failures;
+    }
+    E2 V[LOGUP_MAX_COLS], U[LOGUP_MAX_COLS], F[LOGUP_MAX_COLS];
+    fold_walk<MAXS>(a, N, r, V, U);
+    E2 total;
+    const u32 zero_mask = fold_divide(a.n_cols, V, U, F, total);
+    for (u32 c = 0; c < a.n_cols; c++) {
+        E2 expected, actual;
+        u32 kind = fold_verdict(a, N, r, c, F, total, zero_mask, expected, actual);
+        if (want == 0xFFFFFFFFu ? kind == 0 : c != want) continue;
+        u64* rec = a.failures + (size_t)FOLD_RECORD_WORDS * o;
+        rec[0] = (u64)a.instance | ((u64)c << 32); rec[1] = kind; rec[2] = r;
+        rec[3] = V[c].a; rec[4] = V[c].b; rec[5] = U[c].a; rec[6] = U[c].b;
+        rec[7] = expected.a; rec[8] = expected.b; rec[9] = actual.a; rec[10] = actual.b;
+        if (++o == end) return;
+    }
+}
+
+int launch_fold_census_rows(const FoldCensusArgs& a, cudaStream_t st) {
+    if (a.n_cols == 0 || a.n_cols > LOGUP_MAX_COLS) return -1;
+    size_t N = (size_t)1 << a.log_n;
+    unsigned blocks = (unsigned)((N + 127) / 128);
+    if (a.prog.n_slots <= 16) k_fold_census_rows<16><<<blocks, 128, 0, st>>>(a);
+    else if (a.prog.n_slots <= 64) k_fold_census_rows<64><<<blocks, 128, 0, st>>>(a);
+    else if (a.prog.n_slots <= 256) k_fold_census_rows<256><<<blocks, 128, 0, st>>>(a);
+    else if (a.prog.n_slots <= 1024) k_fold_census_rows<1024><<<blocks, 128, 0, st>>>(a);
+    else return -1;
+    COUNT_LAUNCH();
+    return 0;
+}
+int launch_fold_census_list(const FoldCensusArgs& a, cudaStream_t st) {
+    if (a.n_cols == 0 || a.n_cols > LOGUP_MAX_COLS) return -1;
+    size_t n = a.probes ? a.n_probes : (size_t)1 << a.log_n;
+    if (n == 0) return 0;
+    unsigned blocks = (unsigned)((n + 127) / 128);
+    if (a.prog.n_slots <= 16) k_fold_census_list<16><<<blocks, 128, 0, st>>>(a);
+    else if (a.prog.n_slots <= 64) k_fold_census_list<64><<<blocks, 128, 0, st>>>(a);
+    else if (a.prog.n_slots <= 256) k_fold_census_list<256><<<blocks, 128, 0, st>>>(a);
+    else if (a.prog.n_slots <= 1024) k_fold_census_list<1024><<<blocks, 128, 0, st>>>(a);
     else return -1;
     COUNT_LAUNCH();
     return 0;

@@ -314,6 +314,39 @@ struct LookupFoldArgs {
 int launch_fold_rows(const LookupFoldArgs& a, cudaStream_t st);   // 0, or -1 when the program needs too many slots/columns
 
 // ---------------------------------------------------------------------------------------------
+// LogUp fold census: every disagreement, not only the first (mdn_lookup_fold_census)
+// ---------------------------------------------------------------------------------------------
+// The fold, division and verdict of k_fold_rows (the same inputs, named alike), one thread per row of the whole AIR.
+//   k_fold_census_rows: row_count[r] = the number of columns of row r whose kind is non-zero (every row is written); per
+//     column c tally[4c] += such rows, tally[4c + 1] += those of kind 3, tally[4c + 2] = min row (init ~0),
+//     tally[4c + 3] = max row (init 0), aggregated per block in shared memory (one global atomic of each kind per block
+//     and disagreeing column); failing_rows += rows with at least one disagreement.
+//   k_fold_census_list: with probes == NULL, a row whose count is non-zero and whose offsets[r] < max_failures writes its
+//     disagreements in ascending column to slots [offsets[r], min(offsets[r] + count, max_failures)); with probes,
+//     thread p writes the record of (row, column) = (probes[2p], probes[2p + 1]) to slot p.  A record is
+//     FOLD_RECORD_WORDS u64, the layout of mdn_fold_failure: instance | column << 32, kind, row, V c0, c1, U c0, c1,
+//     expected c0, c1, actual c0, c1.
+static constexpr u32 FOLD_RECORD_WORDS = 11;
+struct FoldCensusArgs {
+    const u64* main_cm; u32 log_n, n_cols;   // as LookupFoldArgs
+    AirDev prog;
+    const u64* publics; const u64* challenges;
+    const u32* marks;
+    const u64* aux_cm;
+    E2 final;
+    u32 instance;                        // written into every record
+    u32* row_count;                      // 2^log_n counts of this AIR
+    unsigned long long* tally;           // 4 * n_cols
+    unsigned long long* failing_rows;
+    const u64* offsets;                  // exclusive scan of row_count, offset by the disagreements of earlier AIRs
+    u64 max_failures;
+    u64* failures;                       // FOLD_RECORD_WORDS u64 per record
+    const u64* probes; size_t n_probes;  // probe mode, or NULL
+};
+int launch_fold_census_rows(const FoldCensusArgs& a, cudaStream_t st);   // 0, or -1 when the program needs too many slots/columns
+int launch_fold_census_list(const FoldCensusArgs& a, cudaStream_t st);   // list or probe mode; 0 or -1 as above
+
+// ---------------------------------------------------------------------------------------------
 // DEEP / FRI / misc
 // ---------------------------------------------------------------------------------------------
 // wvec[i] = y^(bitrev_n(p0 + i)) for i < cnt  (EF interleaved; p0 = 0, cnt = 2^n: the whole vector);

@@ -387,8 +387,30 @@ struct mdn_session {
                            mdn_constraint_tally* tallies, u64 max_tallies, mdn_constraint_census_report* out);
     void check_trace_balance(const mdn_statement* st, const mdn_matrix* traces, const u64* rnd, const u64* boundary, size_t n_boundary,
                              const uint32_t* const* mutex_sites, u64 max_contrib, u32 flags, mdn_balance_report* out);
+    // what prepare_folds leaves for the row passes of check_lookup_folds / lookup_fold_census
+    struct FoldSetup {
+        bool on_device = false, cm = false; u32 k = 0;
+        u32 skipped = 0;                        // AIRs without a lookup program
+        size_t staging_words = 0;               // the largest host fold buffer
+        std::vector<u64*> main_cm, aux_cm;      // raw column-major main and aux traces of the lookup AIRs
+        std::vector<DevBuf> marks;              // device fold marks, or empty
+        std::vector<E2> finals;                 // the value aux[N][0] would hold
+    };
+    void prepare_folds(const mdn_statement* st, const mdn_matrix* traces, const u64* rnd, const uint32_t* const* fold_marks,
+                       const mdn_matrix* aux, const u64* const* aux_finals, u64* const* folds_out, u32 flags, const void* out, FoldSetup& fs);
+    // the fold kernels' inputs of lookup AIR i (kernels.cuh LookupFoldArgs, FoldCensusArgs name them alike)
+    template <class Args> Args fold_args(u32 i, const FoldSetup& fs) const {
+        Args f{};
+        f.main_cm = fs.main_cm[i]; f.log_n = log_heights[i]; f.n_cols = airs[i].desc.aux_width; f.prog = airs[i].lookup_dev;
+        f.publics = d_publics.p; f.challenges = d_randomness.p; f.marks = (const u32*)fs.marks[i].p;
+        f.aux_cm = fs.aux_cm[i]; f.final = fs.finals[i];
+        return f;
+    }
     void check_lookup_folds(const mdn_statement* st, const mdn_matrix* traces, const u64* rnd, const uint32_t* const* fold_marks,
                             const mdn_matrix* aux, const u64* const* aux_finals, u64* const* folds_out, u32 flags, mdn_fold_report* out);
+    void lookup_fold_census(const mdn_statement* st, const mdn_matrix* traces, const u64* rnd, const uint32_t* const* fold_marks,
+                            const mdn_matrix* aux, const u64* const* aux_finals, u32 flags, mdn_fold_failure* failures, u64 max_failures,
+                            mdn_fold_tally* tallies, u64 max_tallies, mdn_fold_census_report* out);
     // the last balance report's lists (mdn_balance_report points into them)
     std::vector<mdn_unmatched> bal_unmatched;
     std::vector<mdn_balance_push> bal_contrib;
@@ -2141,16 +2163,19 @@ void mdn_session::check_trace_balance(const mdn_statement* st, const mdn_matrix*
 // with the call (host row-major through the transpose, column-major device read in place) or from build_logup_aux on
 // the same traces.  k_fold_rows runs once per AIR with a lowered lookup program; a second launch on the one failing row
 // fetches its fold, expected and actual values.
-void mdn_session::check_lookup_folds(const mdn_statement* st, const mdn_matrix* traces, const u64* rnd, const uint32_t* const* fold_marks,
-                                     const mdn_matrix* aux, const u64* const* aux_finals, u64* const* folds_out, u32 flags, mdn_fold_report* out) {
+// prepare_folds is everything before the row pass, shared with lookup_fold_census (which passes no folds_out).
+void mdn_session::prepare_folds(const mdn_statement* st, const mdn_matrix* traces, const u64* rnd, const uint32_t* const* fold_marks,
+                                const mdn_matrix* aux, const u64* const* aux_finals, u64* const* folds_out, u32 flags, const void* out,
+                                FoldSetup& fs) {
     const auto [cm, on_device, k] = start_check(st, traces, &no_challenger, flags, out);
+    fs.cm = cm; fs.on_device = on_device; fs.k = k;
     bind_order(st, false);
 
     // arguments: challenges, aux traces and their closing values, fold marks, fold buffers
     const u32 max_rand = check_randomness(rnd);
     if (!aux && aux_finals) fail(MDN_ERR_INVALID_ARG, "aux_finals given without aux: the device LogUp build supplies its own closing values");
-    u32 skipped = 0;
-    size_t staging_words = 0;
+    u32& skipped = fs.skipped;
+    size_t& staging_words = fs.staging_words;
     for (u32 i = 0; i < k; i++) {
         const uint32_t* marks = fold_marks ? fold_marks[i] : nullptr;
         if (!lookup_air(i, marks ? "fold marks" : folds_out && folds_out[i] ? "a fold buffer" : nullptr, skipped)) continue;
@@ -2182,8 +2207,9 @@ void mdn_session::check_lookup_folds(const mdn_statement* st, const mdn_matrix* 
     // caller keeps them)
     std::vector<u32> lookups;
     for (u32 i = 0; i < k; i++) if (airs[i].has_lookup) lookups.push_back(i);
-    const std::vector<u64*> main_cm = stage_main(traces, lookups, cm, on_device);
-    std::vector<u64*> aux_cm(k, nullptr);
+    fs.main_cm = stage_main(traces, lookups, cm, on_device);
+    fs.aux_cm.assign(k, nullptr);
+    std::vector<u64*>& aux_cm = fs.aux_cm;
     size_t aux_total = 0;
     if (!(aux && cm)) for (u32 i : lookups) aux_total += ((size_t)1 << log_heights[i]) * 2 * airs[i].desc.aux_width;
     aux_c.coef_buf.alloc(aux_total, stream);
@@ -2197,7 +2223,8 @@ void mdn_session::check_lookup_folds(const mdn_statement* st, const mdn_matrix* 
         check_input_flag("an aux trace");
     }
     upload_leaves(rnd, 2 * (size_t)max_rand);
-    std::vector<DevBuf> d_marks(k);
+    std::vector<DevBuf>& d_marks = fs.marks;
+    d_marks.resize(k);
     for (u32 i = 0; i < k; i++) {
         if (!airs[i].has_lookup || !fold_marks || !fold_marks[i]) continue;
         const u32 nc = LookupItems(*st->airs[i].lookup).n;
@@ -2206,19 +2233,28 @@ void mdn_session::check_lookup_folds(const mdn_statement* st, const mdn_matrix* 
         CUDA_OK(cudaMemcpyAsync(d_marks[i].p, fold_marks[i], nc * sizeof(u32), cudaMemcpyHostToDevice, stream));
     }
     // the prover path to check when no aux trace is given: k_logup_rows + the scan, as mdn_prove builds it
-    std::vector<E2> finals(k, gl::e2(0, 0));
+    fs.finals.assign(k, gl::e2(0, 0));
+    std::vector<E2>& finals = fs.finals;
     std::vector<u32> pos(k);
     for (u32 j = 0; j < k; j++) pos[order[j]] = j;
     for (u32 i = 0; i < k; i++) {
         if (!airs[i].has_lookup) continue;
         if (aux) { finals[i] = gl::e2(aux_finals[i][0], aux_finals[i][1]); continue; }
         u64 fin[2] = {0, 0};
-        build_logup_aux(pos[i], main_cm[i], aux_cm[i], fin);
+        build_logup_aux(pos[i], fs.main_cm[i], aux_cm[i], fin);
         finals[i] = gl::e2(fin[0], fin[1]);
     }
+}
+
+void mdn_session::check_lookup_folds(const mdn_statement* st, const mdn_matrix* traces, const u64* rnd, const uint32_t* const* fold_marks,
+                                     const mdn_matrix* aux, const u64* const* aux_finals, u64* const* folds_out, u32 flags, mdn_fold_report* out) {
+    FoldSetup fs;
+    prepare_folds(st, traces, rnd, fold_marks, aux, aux_finals, folds_out, flags, out, fs);
+    const u32 k = fs.k;
+    const bool on_device = fs.on_device, cm = fs.cm;
     // host fold buffers are filled through one device staging buffer, sized for the largest of them
     DevBuf staging;
-    if (staging_words) alloc_checked("the folds of the largest AIR need", {{&staging, staging_words}});
+    if (fs.staging_words) alloc_checked("the folds of the largest AIR need", {{&staging, fs.staging_words}});
 
     // per AIR: {first (row << 32 | column), failing rows, zero U}; then the probe's 9 words and its scratch counters
     DevBuf res; res.alloc(3 * (size_t)k + 12, stream);
@@ -2230,10 +2266,7 @@ void mdn_session::check_lookup_folds(const mdn_statement* st, const mdn_matrix* 
     for (u32 i = 0; i < k; i++) {
         if (!airs[i].has_lookup) continue;
         mk::LookupFoldArgs& f = fa[i];
-        f = mk::LookupFoldArgs{};
-        f.main_cm = main_cm[i]; f.log_n = log_heights[i]; f.n_cols = airs[i].desc.aux_width; f.prog = airs[i].lookup_dev;
-        f.publics = d_publics.p; f.challenges = d_randomness.p; f.marks = (const u32*)d_marks[i].p;
-        f.aux_cm = aux_cm[i]; f.final = finals[i];
+        f = fold_args<mk::LookupFoldArgs>(i, fs);
         u64* user = folds_out ? folds_out[i] : nullptr;
         f.folds_out = user && !on_device ? staging.p : user; f.folds_cm = cm;
         f.row0 = 0; f.n_rows = (size_t)1 << log_heights[i];
@@ -2250,7 +2283,7 @@ void mdn_session::check_lookup_folds(const mdn_statement* st, const mdn_matrix* 
     CUDA_OK(cudaGetLastError());
 
     memset(out, 0, sizeof *out);
-    out->n_skipped_airs = skipped;
+    out->n_skipped_airs = fs.skipped;
     for (u32 i = 0; i < k; i++) { out->failing_rows += host_res[3 * i + 1]; out->zero_u += host_res[3 * i + 2]; }
     for (u32 i = 0; i < k; i++) {
         u64 first = host_res[3 * i];
@@ -2270,6 +2303,146 @@ void mdn_session::check_lookup_folds(const mdn_statement* st, const mdn_matrix* 
         break;
     }
     out->holds = out->failing_rows == 0;
+}
+
+// ---------------------------------------------------------------------------------------------
+// lookup_fold_census: every disagreement of check_lookup_folds, per column and in row order, without a proof
+// ---------------------------------------------------------------------------------------------
+// prepare_folds as check_lookup_folds; then per lookup AIR (instance order) k_fold_census_rows fills that AIR's slice of
+// one per-row count array, concatenated in instance order, and its per-column tally; one exclusive scan of the counts
+// gives every disagreeing row its first record slot and the total.  k_fold_census_list then writes the first
+// max_failures records in (instance, row, column) order, and in probe mode the records at the reported tallies' first
+// rows (plus the least disagreement's, when truncation drops it).  Counts, minima, maxima and the scan do not depend on
+// the order the atomics ran in, so neither does anything reported.
+static_assert(sizeof(mdn_fold_failure) == mk::FOLD_RECORD_WORDS * sizeof(u64), "mdn_fold_failure is the kernel's record");
+static_assert(sizeof(mdn_fold_tally) == 10 * sizeof(u64), "mdn_fold_tally: 80 bytes");
+void mdn_session::lookup_fold_census(const mdn_statement* st, const mdn_matrix* traces, const u64* rnd, const uint32_t* const* fold_marks,
+                                     const mdn_matrix* aux, const u64* const* aux_finals, u32 flags, mdn_fold_failure* failures, u64 max_failures,
+                                     mdn_fold_tally* tallies, u64 max_tallies, mdn_fold_census_report* out) {
+    FoldSetup fs;
+    prepare_folds(st, traces, rnd, fold_marks, aux, aux_finals, nullptr, flags, out, fs);
+    const u32 k = fs.k;
+
+    // per-row counts of the lookup AIRs (u32, instance order), their offsets, one 4-word tally per column, two counters
+    std::vector<size_t> row_base(k + 1, 0), tally_base(k + 1, 0);
+    for (u32 i = 0; i < k; i++) {
+        const bool lk = airs[i].has_lookup;
+        row_base[i + 1] = row_base[i] + (lk ? (size_t)1 << log_heights[i] : 0);
+        tally_base[i + 1] = tally_base[i] + (lk ? 4 * (size_t)airs[i].desc.aux_width : 0);
+    }
+    const size_t rows = row_base[k];
+    DevBuf counts, offsets, tally, words, scratch;
+    counts.alloc(std::max<size_t>(1, (rows + 1) / 2), stream);
+    offsets.alloc(std::max<size_t>(1, rows), stream);
+    tally.alloc(std::max<size_t>(1, tally_base[k]), stream);
+    words.alloc(2, stream);                                             // rows with a disagreement, disagreements
+    scratch.alloc(std::max<size_t>(1, (rows + 2047) / 2048), stream);  // block sums of the scan
+    std::vector<u64> host_tally(std::max<size_t>(1, tally_base[k]), 0);
+    for (size_t q = 0; q < tally_base[k]; q += 4) host_tally[q + 2] = ~0ull;
+    CUDA_OK(cudaMemcpyAsync(tally.p, host_tally.data(), host_tally.size() * sizeof(u64), cudaMemcpyHostToDevice, stream));
+    CUDA_OK(cudaMemsetAsync(words.p, 0, 2 * sizeof(u64), stream));
+    u32* d_counts = reinterpret_cast<u32*>(counts.p);
+    std::vector<mk::FoldCensusArgs> fa(k);
+    for (u32 i = 0; i < k; i++) {
+        if (!airs[i].has_lookup) continue;
+        mk::FoldCensusArgs& f = fa[i];
+        f = fold_args<mk::FoldCensusArgs>(i, fs);
+        f.instance = i;
+        f.row_count = d_counts + row_base[i];
+        f.tally = (unsigned long long*)(tally.p + tally_base[i]);
+        f.failing_rows = (unsigned long long*)words.p;
+        f.offsets = offsets.p + row_base[i];
+        if (mk::launch_fold_census_rows(f, stream) != 0) fail(MDN_ERR_UNSUPPORTED, "AIR %u: lookup program too large for the interpreter", i);
+    }
+    if (rows) mk::launch_count_exclusive_scan(d_counts, rows, offsets.p, words.p + 1, scratch.p, stream);
+    u64 host_words[2];
+    CUDA_OK(cudaMemcpyAsync(host_tally.data(), tally.p, host_tally.size() * sizeof(u64), cudaMemcpyDeviceToHost, stream));
+    CUDA_OK(cudaMemcpyAsync(host_words, words.p, sizeof host_words, cudaMemcpyDeviceToHost, stream));
+    CUDA_OK(cudaStreamSynchronize(stream));
+    CUDA_OK(cudaGetLastError());
+
+    // the disagreeing (instance, column) pairs in order, and the least disagreement: the first failing instance's least
+    // (first_row, column)
+    std::vector<mdn_fold_tally> all;
+    size_t least = SIZE_MAX;
+    u64 zero_u = 0;
+    for (u32 i = 0; i < k; i++) {
+        if (!airs[i].has_lookup) continue;
+        for (u32 c = 0; c < airs[i].desc.aux_width; c++) {
+            const u64* t = host_tally.data() + tally_base[i] + 4 * (size_t)c;
+            if (!t[0]) continue;
+            mdn_fold_tally ft{};
+            ft.instance = i; ft.column = c; ft.failing_rows = t[0]; ft.zero_u_rows = t[1]; ft.first_row = t[2]; ft.last_row = t[3];
+            all.push_back(ft);
+            zero_u += t[1];
+            if (least == SIZE_MAX || (all[least].instance == i && t[2] < all[least].first_row)) least = all.size() - 1;
+        }
+    }
+    memset(out, 0, sizeof *out);
+    out->disagreements = host_words[1];
+    out->n_failures = std::min<u64>(out->disagreements, max_failures);
+    out->failing_columns = all.size();
+    out->n_tallies = std::min<u64>(all.size(), max_tallies);
+
+    // records at the first rows of the reported tallies and of the least disagreement: probe mode, one launch per instance
+    const size_t W = mk::FOLD_RECORD_WORDS;
+    std::vector<size_t> probed;
+    for (size_t q = 0; q < out->n_tallies; q++) probed.push_back(q);
+    if (least != SIZE_MAX && least >= out->n_tallies) probed.push_back(least);   // `all` is in instance order: still sorted
+    DevBuf d_probes, d_records, d_failures;
+    if (!probed.empty()) {
+        std::vector<u64> pr;
+        for (size_t q : probed) { pr.push_back(all[q].first_row); pr.push_back(all[q].column); }
+        d_probes.alloc(pr.size(), stream);
+        d_records.alloc(W * probed.size(), stream);
+        CUDA_OK(cudaMemcpyAsync(d_probes.p, pr.data(), pr.size() * sizeof(u64), cudaMemcpyHostToDevice, stream));
+        for (size_t b = 0; b < probed.size();) {
+            u32 i = all[probed[b]].instance;
+            size_t e = b;
+            while (e < probed.size() && all[probed[e]].instance == i) e++;
+            mk::FoldCensusArgs f = fa[i];
+            f.probes = d_probes.p + 2 * b; f.n_probes = e - b; f.failures = d_records.p + W * b;
+            if (mk::launch_fold_census_list(f, stream) != 0) fail(MDN_ERR_UNSUPPORTED, "AIR %u: lookup program too large for the interpreter", i);
+            b = e;
+        }
+    }
+    // the first n_failures records, every AIR with a disagreeing column writing its own slots
+    if (out->n_failures) {
+        alloc_checked("the list of " + std::to_string(out->n_failures) + " disagreements needs", {{&d_failures, W * out->n_failures}});
+        for (u32 i = 0; i < k; i++) {
+            if (!airs[i].has_lookup) continue;
+            bool any = false;
+            for (u32 c = 0; c < airs[i].desc.aux_width && !any; c++) any = host_tally[tally_base[i] + 4 * (size_t)c] != 0;
+            if (!any) continue;
+            mk::FoldCensusArgs f = fa[i];
+            f.max_failures = out->n_failures; f.failures = d_failures.p;
+            if (mk::launch_fold_census_list(f, stream) != 0) fail(MDN_ERR_UNSUPPORTED, "AIR %u: lookup program too large for the interpreter", i);
+        }
+    }
+    std::vector<mdn_fold_failure> records(probed.size());
+    if (!probed.empty()) CUDA_OK(cudaMemcpyAsync(records.data(), d_records.p, records.size() * sizeof(mdn_fold_failure), cudaMemcpyDeviceToHost, stream));
+    if (out->n_failures) CUDA_OK(cudaMemcpyAsync(failures, d_failures.p, out->n_failures * sizeof(mdn_fold_failure), cudaMemcpyDeviceToHost, stream));
+    CUDA_OK(cudaStreamSynchronize(stream));
+    CUDA_OK(cudaGetLastError());
+    for (size_t q = 0; q < probed.size(); q++) {
+        mdn_fold_tally& t = all[probed[q]];
+        t.first_kind = records[q].kind;
+        memcpy(t.first_expected, records[q].expected, sizeof t.first_expected); memcpy(t.first_actual, records[q].actual, sizeof t.first_actual);
+    }
+    for (size_t q = 0; q < out->n_tallies; q++) tallies[q] = all[q];
+
+    // `first`: what check_lookup_folds reports for the same call
+    mdn_fold_report& f = out->first;
+    f.n_skipped_airs = fs.skipped;
+    f.failing_rows = host_words[0];
+    f.zero_u = zero_u;
+    if (least != SIZE_MAX) {
+        const size_t q = std::find(probed.begin(), probed.end(), least) - probed.begin();
+        const mdn_fold_failure& r = records[q];
+        f.kind = r.kind; f.instance = r.instance; f.column = r.column; f.row = r.row;
+        memcpy(f.fold, r.fold, sizeof f.fold); memcpy(f.expected, r.expected, sizeof f.expected); memcpy(f.actual, r.actual, sizeof f.actual);
+    }
+    f.holds = f.failing_rows == 0;
 }
 
 // mdn_aux_builder_device for instance `inst`: the aux columns go straight into `aux_slot` (column-major, on the session's
@@ -3130,6 +3303,17 @@ int mdn_check_lookup_folds(mdn_session* s, const mdn_statement* st, const mdn_ma
                            uint64_t* const* folds_out, uint32_t flags, mdn_fold_report* out) {
     return run_check(s, "mdn_check_lookup_folds", nullptr, nullptr,
                      [&] { s->check_lookup_folds(st, traces, randomness, fold_marks, aux, aux_finals, folds_out, flags, out); });
+}
+
+int mdn_lookup_fold_census(mdn_session* s, const mdn_statement* st, const mdn_matrix* traces, const uint64_t* randomness,
+                           const uint32_t* const* fold_marks, const mdn_matrix* aux, const uint64_t* const* aux_finals, uint32_t flags,
+                           mdn_fold_failure* failures, uint64_t max_failures, mdn_fold_tally* tallies, uint64_t max_tallies,
+                           mdn_fold_census_report* out) {
+    const char* refused = !out ? "null argument"
+                        : !failures && max_failures ? "failures is NULL but max_failures is not 0"
+                        : !tallies && max_tallies ? "tallies is NULL but max_tallies is not 0" : nullptr;
+    return run_check(s, "mdn_lookup_fold_census", refused, nullptr,
+                     [&] { s->lookup_fold_census(st, traces, randomness, fold_marks, aux, aux_finals, flags, failures, max_failures, tallies, max_tallies, out); });
 }
 
 size_t mdn_proof_serialize(const mdn_proof* p, uint8_t* out, size_t cap) {
