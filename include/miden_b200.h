@@ -74,7 +74,10 @@ typedef struct {
  * sampled -- no host callback, no aux-trace upload for that AIR.
  *   program words[0..5) = { 0x504B4C4D ("MLKP"), 1, n_nodes, n_interactions, n_consts }
  *   nodes        : as in mdn_air.program, restricted to what a LookupBuilder exposes: MAIN, PUBLIC,
- *                  CHALLENGE (0 = alpha, 1 = beta), CONST, EXT_CONST, ADD, SUB, MUL, NEG, PERIODIC
+ *                  CHALLENGE (0 = alpha, 1 = beta), CONST, EXT_CONST, ADD, SUB, MUL, NEG, PERIODIC, and
+ *                  PREPROCESSED (a = row offset 0|1, b = column < preprocessed_width; an AIR without preprocessed
+ *                  columns is refused with MDN_ERR_INVALID_ARG) -- the `CombinedWindow` reads of a preprocessed
+ *                  lookup table.  AUX, AUX_VALUE and the selectors are refused.
  *   interactions : 4 words { aux column, flag node | 0xFFFFFFFF, multiplicity node, denominator node } --
  *                  one per `LookupGroup::insert` / `LookupBatch::insert` after `LookupMessage::encode`; it
  *                  contributes multiplicity/denominator to its column on every row where the (0/1) flag is
@@ -82,7 +85,15 @@ typedef struct {
  *   consts       : (lo, hi) word pairs
  * Output (aux_builder.rs:1-20,215-268): f_c(r) = sum of m/d over column c's active interactions at row r;
  * aux[r][c] = f_c(r) for c > 0; aux[r][0] = sum_{r' < r} sum_c f_c(r'); aux value 0 = the total over all rows.
- * Requires aux_width == num_columns (<= 16) and num_aux_values == 1; a zero denominator is an error. */
+ * Requires aux_width == num_columns (<= 16) and num_aux_values == 1; a zero denominator is an error.
+ * PREPROCESSED reads the raw preprocessed rows r and (r + 1) mod N of the trace domain, as mdn_check_constraints does.
+ * Where each call takes them from:
+ *   mdn_prove, mdn_prove_begin / commit_aux, the constraint guard : the installed bundle (mdn_session_set_preprocessed),
+ *       which such a proof requires anyway; one derivation serves the LogUp build and the guard
+ *   mdn_check_constraints, mdn_constraint_census                   : the call's own `preprocessed` argument
+ *   mdn_check_trace_balance, mdn_check_lookup_folds, mdn_lookup_fold_census : the installed bundle, which must hold
+ *       each AIR whose lookup program reads PREPROCESSED at that AIR's height and width (MDN_ERR_INVALID_ARG naming
+ *       the AIR otherwise, before any device work); calls whose lookup programs read none do not consult it. */
 typedef struct {
     uint32_t num_columns;           /* LookupAir::num_columns() */
     uint32_t program_words;
@@ -417,7 +428,8 @@ int mdn_constraint_census(mdn_session* s, const mdn_statement* st, const mdn_mat
  * AIRs without mdn_air.lookup are skipped and counted.  Per push, exactly as the reference's DebugTraceBuilder:
  * interaction k of the lookup program pushes (multiplicity, denominator) at row r when its flag is non-zero (or it has
  * none); the multiplicity is recorded as given, not multiplied by the flag; a zero denominator is an ordinary key (the
- * aux build refuses it); the next row wraps; periodic values are row r mod 2^log_max_period of periodic_values.
+ * aux build refuses it); the next row wraps; periodic values are row r mod 2^log_max_period of periodic_values;
+ * preprocessed columns are read from the installed bundle (see mdn_lookup).
  *   randomness : 2 * max num_randomness u64 (alpha, beta, ...: EF pairs), canonical -- e.g. the randomness_out of
  *                mdn_check_constraints or mdn_prove_begin.  Nothing is observed; no hash configuration is consulted.
  *   boundary   : n_boundary triples {denominator c0, c1, multiplicity}, canonical: the output of LookupAir::eval_boundary
@@ -494,7 +506,7 @@ int mdn_check_trace_balance(mdn_session* s, const mdn_statement* st, const mdn_m
  *   U_c(r) != 0                                                                (kind 3 otherwise: reported, not divided)
  * A column whose U is zero is left out of the kind 1 comparison, and a row with any zero U out of the kind 2 comparison.
  * Rows, the next-row wrap, periodic values, flags and the "multiplicity as given" rule are those of
- * mdn_check_trace_balance; nothing is observed and no hash configuration is consulted.  Boundary emissions do not enter
+ * mdn_check_trace_balance, preprocessed columns included; nothing is observed and no hash configuration is consulted.  Boundary emissions do not enter
  * the folds (mod.rs:194-195).  AIRs without mdn_air.lookup are skipped and counted.
  * The fold is the builder's, which (V, U) is compared with as a pair, not "sum m/d, then split":
  *   batch  : (N, D) <- (N * d + D * m, D * d) per interaction, from (0, 1)              (builder.rs:353-355,369-371)

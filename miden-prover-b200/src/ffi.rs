@@ -44,6 +44,9 @@ pub struct MdnChallenger {
     pub output_len: u32,
 }
 
+/// A lowered `LookupAir` (include/miden_b200.h `mdn_lookup`).  Its nodes may read PREPROCESSED (op 15) when the AIR
+/// declares preprocessed columns: from the installed bundle in a proof and in the three lookup checks, from the call's
+/// `preprocessed` argument in `mdn_check_constraints` / `mdn_constraint_census`.
 #[repr(C)]
 #[derive(Clone, Copy, Debug)]
 pub struct MdnLookup {

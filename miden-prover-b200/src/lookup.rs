@@ -4,8 +4,9 @@
 //!
 //! The recording builder below is the symbolic twin of the reference's two adapters:
 //!   * like `ConstraintLookupBuilder` (air/src/lookup/constraint.rs) it runs over the p3 symbolic types, so every flag,
-//!     multiplicity and encoded message is an expression tree over main / periodic / public leaves and the two
-//!     challenges alpha = CHALLENGE(0), beta = CHALLENGE(1) (`Challenges::new`, air/src/lookup/challenges.rs);
+//!     multiplicity and encoded message is an expression tree over main / preprocessed / periodic / public leaves and
+//!     the two challenges alpha = CHALLENGE(0), beta = CHALLENGE(1) (`Challenges::new`, air/src/lookup/challenges.rs);
+//!     a `CombinedWindow` read of the preprocessed part lowers to PREPROCESSED(offset, column) (op 15);
 //!   * like `ProverLookupBuilder` (air/src/lookup/prover.rs:230-444) it keeps one record per interaction -- the
 //!     `(multiplicity, encoded denominator)` pair the prover path pushes when the (boolean) flag is set -- instead of
 //!     folding them into the `(V, U)` constraint pair, and it runs only the `canonical` closure of

@@ -87,8 +87,9 @@ NO_FLAG = 0xFFFFFFFF
 
 class LookupProgramBuilder(ProgramBuilder):
     """Host-side lowering of `LookupAir::eval` (air/src/lookup/builder.rs) for the device aux build: the node
-    surface a `LookupBuilder` exposes (main window, periodic values, challenges alpha = challenge(0) and
-    beta = challenge(1), constants) and one record per interaction -- `insert(column, flag, multiplicity,
+    surface a `LookupBuilder` exposes (main window, preprocessed window `preprocessed(offset, col)` -- the AIR must
+    declare preprocessed columns --, periodic values, challenges alpha = challenge(0) and beta = challenge(1),
+    constants) and one record per interaction -- `insert(column, flag, multiplicity,
     denominator)` is `LookupGroup::insert` / `LookupBatch::insert` after `LookupMessage::encode`."""
 
     def __init__(self, num_columns: int):

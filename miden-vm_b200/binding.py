@@ -417,7 +417,8 @@ class Session:
     def check_constraints(self, statement: Statement, traces, challenger: Challenger, aux_builder=None, preprocessed=None,
                           flags=0):
         """`debug::check_constraints(prover_statement, challenger)` on the device: every constraint of every AIR on
-        every trace row, without proving.  `preprocessed` = Matrix array in instance order (width 0 = none) or None.
+        every trace row, without proving.  `preprocessed` = Matrix array in instance order (width 0 = none) or None; the
+        row checks and the device LogUp build both read it.
         Returns (ConstraintReport, randomness u64[2 * max num_randomness])."""
         rep = ConstraintReport()
         n_rand = max((statement.airs[i].num_randomness for i in range(statement.n_airs)), default=0)
@@ -449,7 +450,8 @@ class Session:
     def check_trace_balance(self, statement: Statement, traces, randomness, boundary=(), mutex_sites=None,
                             max_contributions: int = 1 << 16, flags=0) -> dict:
         """`check_trace_balance` (air/src/lookup/debug/trace/mod.rs:169) on the device, jointly over every AIR of the
-        statement with a lowered lookup program.  randomness: 2 * max num_randomness words (e.g. the randomness of
+        statement with a lowered lookup program; programs that read preprocessed columns read the installed bundle
+        (set_preprocessed).  randomness: 2 * max num_randomness words (e.g. the randomness of
         check_constraints); boundary: (c0, c1, multiplicity) triples of eval_boundary; mutex_sites: per AIR None or the
         annotation array of LookupProgramBuilder.mutex_sites().  Returns balance_report_dict of the report."""
         rnd = np.ascontiguousarray(np.asarray(randomness, dtype=np.uint64).reshape(-1))
@@ -472,7 +474,8 @@ class Session:
         """`collect_column_oracle_folds` (air/src/lookup/debug/trace/mod.rs:196) on the device, compared with an aux trace
         as `assert_prover_matches_oracle` compares them.  fold_marks: per AIR None or LookupProgramBuilder.fold_marks();
         aux: Matrix array in instance order (host row-major, or device as `flags` say) with aux_finals, per AIR None or
-        (c0, c1) -- or None for the device LogUp build of the same call; folds_out: per AIR None, a uint64 numpy array of
+        (c0, c1) -- or None for the device LogUp build of the same call; preprocessed columns come from the installed
+        bundle, as in check_trace_balance; folds_out: per AIR None, a uint64 numpy array of
         rows * num_columns * 4 words to fill, or a device address (int) with FLAG_DEVICE_TRACES.  Returns fold_report_dict."""
         rnd, marks, fins, keep = _fold_inputs(statement, randomness, fold_marks, aux_finals)
         n, outs = statement.n_airs, None

@@ -41,6 +41,7 @@ struct JitArgs {
 // Arguments of the generated LogUp row kernel (same member names as JitArgs where the leaf code is shared).
 struct LookupJitArgs {
     const uint64_t* main_lde;      // raw main trace, column-major [col][row]
+    const uint64_t* prep_lde;      // raw preprocessed trace, column-major [col][row], or NULL (the program reads none)
     const uint64_t* publics; const uint64_t* challenges; const uint64_t* periodic;   // periodic: raw row-major matrix
     uint64_t* aux_cm; uint64_t* totals;
     uint32_t* bad_flag;
@@ -122,7 +123,19 @@ __device__ __forceinline__ E2 esubf(E2 x, u64 s) { return mk(fsub(x.a, s), x.b);
 __device__ __forceinline__ E2 efsub(u64 s, E2 x) { return mk(fsub(s, x.a), fneg(x.b)); } // s - x
 __device__ __forceinline__ E2 ldapow(const u64* __restrict__ p, u32 k) { return mk(p[2 * k], p[2 * k + 1]); }
 __device__ E2 einv(E2 x) { u64 n = fsub(fmul(x.a, x.a), fmul7(fmul(x.b, x.b))); u64 ni = finv(n); return mk(fmul(x.a, ni), fneg(fmul(x.b, ni))); }
-struct LookupJitArgs {
+)CUDA";
+// the lookup mode's argument struct (host mirror: LookupJitArgs above)
+static const char PRELUDE_LOOKUP_ARGS[] = R"CUDA(struct LookupJitArgs {
+    const u64* main_lde; const u64* prep_lde; const u64* publics; const u64* challenges; const u64* periodic;
+    u64* aux_cm; u64* totals;
+    u32* bad_flag;
+    u32 log_n, n_periodic, log_max_period, pad;
+};
+)CUDA";
+// what the constraint and check modes emit in its place: the struct without prep_lde, which they do not use; kept so
+// that their generated source, and with it their cubins, stay exactly as they were before the lookup mode read
+// preprocessed columns
+static const char PRELUDE_LOOKUP_ARGS_UNUSED[] = R"CUDA(struct LookupJitArgs {
     const u64* main_lde; const u64* publics; const u64* challenges; const u64* periodic;
     u64* aux_cm; u64* totals;
     u32* bad_flag;
@@ -286,6 +299,7 @@ inline std::string generate(const uint32_t* w, GenInfo* info, Mode mode = MODE_C
     s += PRELUDE;
     s += PRELUDE_FMUL_G2;
     s += PRELUDE_B;
+    s += lookup ? PRELUDE_LOOKUP_ARGS : PRELUDE_LOOKUP_ARGS_UNUSED;
     if (check) {
         snprintf(buf, sizeof buf, "#define CENSUS_SHARED_K %uu\n", CENSUS_SHARED_K);
         s += buf;

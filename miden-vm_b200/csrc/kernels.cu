@@ -817,7 +817,8 @@ int launch_constraints(const ConstraintArgs& a, cudaStream_t st) {
 // LogUp aux trace (trace-domain interpreter + EF scan)
 // =============================================================================================
 // one instruction of a compiled lookup program that is not an EMIT: the leaves a LookupBuilder exposes and the arithmetic
-// ops, at trace row r (rn = the next row, wrapping).  Shared by the kernels that interpret lookup programs.
+// ops, at trace row r (rn = the next row, wrapping); PREPROCESSED reads the raw column-major preprocessed rows prep_cm.
+// Shared by the kernels that interpret lookup programs.
 #define LOOKUP_NODE_CASES(a, N, r, rn, per_row, slot, x, y, ext, v)                                                     \
     case 0: v = gl::e2((a).main_cm[(size_t)(y) * (N) + ((x) ? (rn) : (r))], 0); break;                                  \
     case 2: v = gl::e2((a).publics[x], 0); break;                                                                       \
@@ -828,7 +829,8 @@ int launch_constraints(const ConstraintArgs& a, cudaStream_t st) {
     case 11: v = (ext) ? gl::e2_sub(slot[x], slot[y]) : gl::e2(gl::sub(slot[x].a, slot[y].a), 0); break;                \
     case 12: v = (ext) ? gl::e2_mul(slot[x], slot[y]) : gl::e2(gl::mul(slot[x].a, slot[y].a), 0); break;                \
     case 13: v = (ext) ? gl::e2_neg(slot[x]) : gl::e2(gl::neg(slot[x].a), 0); break;                                    \
-    case 14: v = gl::e2((a).prog.periodic[(per_row) + (x)], 0); break;
+    case 14: v = gl::e2((a).prog.periodic[(per_row) + (x)], 0); break;                                                  \
+    case 16: v = gl::e2((a).prep_cm[(size_t)(y) * (N) + ((x) ? (rn) : (r))], 0); break;
 
 template <int MAXS>
 __global__ void __launch_bounds__(128) k_logup_rows(LogupArgs a) {

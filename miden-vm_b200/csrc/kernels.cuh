@@ -161,12 +161,13 @@ int launch_constraints(const ConstraintArgs& a, cudaStream_t st);   // returns 0
 // ---------------------------------------------------------------------------------------------
 // LogUp aux trace on the device (build_logup_aux_trace, reference air/src/lookup/aux_builder.rs:49-97)
 // ---------------------------------------------------------------------------------------------
-// Compiled lookup program: the constraint instruction format with MAIN/PERIODIC reading the TRACE domain and
+// Compiled lookup program: the constraint instruction format with MAIN/PERIODIC/PREPROCESSED reading the TRACE domain and
 // op 17 = EMIT {op, column, flag slot | multiplicity slot << 16, denominator slot} (flag slot 0xffff = none).
 // One thread per trace row keeps a rational (V_c, U_c) per aux column (V/U = sum of m/d over the row's
 // active interactions), inverts once per column, writes the fraction columns c > 0 and the row total.
 struct LogupArgs {
     const u64* main_cm;      // raw main trace, column-major [col][row]
+    const u64* prep_cm;      // raw preprocessed trace, column-major [col][row], or NULL (the program reads none)
     u32 log_n, n_cols;       // trace height, LookupAir::num_columns
     AirDev prog;             // periodic = RAW periodic matrix, row-major (max_period x n_periodic)
     const u64* publics; const u64* challenges;
@@ -266,6 +267,7 @@ __host__ __device__ inline u64 balance_key(u32 inst, u64 row, u32 k) { return ((
 static constexpr u32 BALANCE_MUTEX_MAX = 1024;   // annotated interactions per AIR
 struct BalanceArgs {
     const u64* main_cm; u32 log_n;       // raw main trace, column-major [col][row]
+    const u64* prep_cm;                   // as LogupArgs
     AirDev prog;                          // lookup program; periodic = RAW periodic matrix, row-major
     const u64* publics; const u64* challenges;
     u32 instance, mode;
@@ -299,6 +301,7 @@ void launch_balance_finish(const BalanceTable& t, unsigned long long* counters, 
 // With probe set, the thread stores {kind, V c0, c1, U c0, c1, expected c0, c1, actual c0, c1} of column probe_col.
 struct LookupFoldArgs {
     const u64* main_cm; u32 log_n, n_cols;   // raw main trace, column-major [col][row]; LookupAir::num_columns
+    const u64* prep_cm;                   // as LogupArgs
     AirDev prog;                          // lookup program; periodic = RAW periodic matrix, row-major
     const u64* publics; const u64* challenges;
     const u32* marks;                     // device, one word per interaction, or NULL
@@ -329,6 +332,7 @@ int launch_fold_rows(const LookupFoldArgs& a, cudaStream_t st);   // 0, or -1 wh
 static constexpr u32 FOLD_RECORD_WORDS = 11;
 struct FoldCensusArgs {
     const u64* main_cm; u32 log_n, n_cols;   // as LookupFoldArgs
+    const u64* prep_cm;
     AirDev prog;
     const u64* publics; const u64* challenges;
     const u32* marks;

@@ -186,6 +186,10 @@ struct AirHost {
     DevBuf lookup_program, raw_main, raw_periodic;
     const u64* raw_main_cm = nullptr;
     mk::AirDev lookup_dev;
+    // lookup_prep: the lookup program reads preprocessed columns (op 15).  raw_prep: the raw column-major rows of the
+    // installed bundle's preprocessed trace of this AIR, derived once per proof or check (mdn_session::bundle_prep_rows)
+    bool lookup_prep = false;
+    DevBuf raw_prep;
     // NVRTC-specialised constraint kernel (jit.hpp) for large programs; NULL = interpreter.  check_jit / census_jit:
     // the two entry points of the program's trace-check cubin (k_jit_check, k_jit_census), loaded for the checks and
     // for a guarded proof
@@ -323,7 +327,9 @@ struct mdn_session {
     void build_tree(Committed& c);
     void lde_matrix(CommittedMat& m);
     void keep_raw_main(u32 j, const u64* caller_cm);
-    void build_logup_aux(u32 j, const u64* main_cm, u64* aux_cm, u64 final_out[2]);
+    const u64* bundle_prep_rows(u32 i);
+    void check_bundle_prep(u32 i);
+    void build_logup_aux(u32 j, const u64* main_cm, const u64* prep_cm, u64* aux_cm, u64 final_out[2]);
     void lde_and_commit(Committed& c, float* t_lde, float* t_hash, bool lde_done = false);
     cudaStream_t copy_stream = nullptr;
     cudaEvent_t copy_ev[8];
@@ -401,7 +407,7 @@ struct mdn_session {
     // the fold kernels' inputs of lookup AIR i (kernels.cuh LookupFoldArgs, FoldCensusArgs name them alike)
     template <class Args> Args fold_args(u32 i, const FoldSetup& fs) const {
         Args f{};
-        f.main_cm = fs.main_cm[i]; f.log_n = log_heights[i]; f.n_cols = airs[i].desc.aux_width; f.prog = airs[i].lookup_dev;
+        f.main_cm = fs.main_cm[i]; f.prep_cm = airs[i].raw_prep.p; f.log_n = log_heights[i]; f.n_cols = airs[i].desc.aux_width; f.prog = airs[i].lookup_dev;
         f.publics = d_publics.p; f.challenges = d_randomness.p; f.marks = (const u32*)fs.marks[i].p;
         f.aux_cm = fs.aux_cm[i]; f.final = fs.finals[i];
         return f;
@@ -872,8 +878,9 @@ static Compiled compile_oplist(u32 i, const mdn_air& a, u32 n_publics, const u32
     for (u32 j = 0; j < nn; j++) {
         u32 op = w[5 + 3 * j], x = w[6 + 3 * j], y = w[7 + 3 * j];
         if (op > 15) fail(MDN_ERR_INVALID_ARG, "AIR %u: unknown op %u", i, op);
-        // a LookupBuilder exposes the main window, periodic values, public values, challenges and constants only
-        if (lookup && (op == 1 || (op >= 4 && op <= 7) || op == 15)) fail(MDN_ERR_INVALID_ARG, "AIR %u: op %u is not available to a lookup program", i, op);
+        // a LookupBuilder exposes the main and preprocessed windows, periodic values, public values, challenges and
+        // constants only
+        if (lookup && (op == 1 || (op >= 4 && op <= 7))) fail(MDN_ERR_INVALID_ARG, "AIR %u: op %u is not available to a lookup program", i, op);
         if (op == 15 && (x > 1 || y >= a.preprocessed_width)) fail(MDN_ERR_INVALID_ARG, "AIR %u: preprocessed column out of range", i);
         if (op >= 5 && op <= 7) out.uses_sel = true;
         if (op >= 10 && op <= 12 && (x >= j || y >= j)) fail(MDN_ERR_INVALID_ARG, "AIR %u: forward reference", i);
@@ -1173,6 +1180,8 @@ void mdn_session::bind_airs(const mdn_statement* st, const mdn_matrix* traces, b
             h.lookup_dev.periodic = np ? h.lookup_program.p + p_off : nullptr;
             h.lookup_dev.n_instr = (u32)(lc.code.size() / 4); h.lookup_dev.n_slots = std::max(1u, lc.n_slots);
             h.lookup_dev.log_max_period = a.log_max_period; h.lookup_dev.n_periodic = a.num_periodic_columns;
+            h.lookup_prep = false;
+            for (u32 j = 0; j < lk.program[2]; j++) h.lookup_prep |= lk.program[5 + 3 * (size_t)j] == 15;
             h.lookup_jit.reset();
             if (jit && jit_min_nodes && lk.program[2] >= jit_min_nodes) {
                 try {
@@ -1375,23 +1384,55 @@ void mdn_session::keep_raw_main(u32 j, const u64* caller_cm) {
     h.raw_main_cm = h.raw_main.p;
 }
 
+// The raw rows of AIR i's preprocessed trace in the installed bundle, column-major on the trace domain: re-derived from
+// the bundle's coefficients by a forward NTT with shift 1 (exact), once per proof or check, into airs[i].raw_prep, so
+// the bundle needs no raw copy.  The LogUp build and the constraint guard of one proof share the derivation.  The
+// bundle holds AIR i at its height and width (checked by prove_begin, or by check_bundle_prep for a lookup check).
+const u64* mdn_session::bundle_prep_rows(u32 i) {
+    AirHost& h = airs[i];
+    if (h.raw_prep.p) return h.raw_prep.p;
+    const u32 q = (u32)(std::find(prep_air.begin(), prep_air.end(), i) - prep_air.begin());
+    const CommittedMat& pm = prep_c.mats[q];
+    const size_t N = (size_t)1 << pm.log_n;
+    h.raw_prep.alloc(N * pm.width, stream);
+    std::vector<mk::FwdItem> items;
+    for (u32 c = 0; c < pm.width; c++) items.push_back(mk::FwdItem{pm.coef + (size_t)c * N, h.raw_prep.p + (size_t)c * N, 0, 0});
+    DevBuf d_items; d_items.alloc(items.size() * sizeof(mk::FwdItem) / sizeof(u64), stream);
+    CUDA_OK(cudaMemcpyAsync(d_items.p, items.data(), items.size() * sizeof(mk::FwdItem), cudaMemcpyHostToDevice, stream));
+    mk::launch_fwd_ntt((const mk::FwdItem*)d_items.p, pm.width, ntt(pm.log_n).T, premul_unshifted(pm.log_n).P, stream);
+    return h.raw_prep.p;
+}
+
+// The lookup checks take no preprocessed argument: an AIR whose lookup program reads preprocessed columns reads the
+// installed bundle, which must hold that AIR at its height and width.  Refused before any device work.
+void mdn_session::check_bundle_prep(u32 i) {
+    if (!airs[i].has_lookup || !airs[i].lookup_prep) return;
+    const u32 q = (u32)(std::find(prep_air.begin(), prep_air.end(), i) - prep_air.begin());
+    if (!has_prep || q == prep_air.size())
+        fail(MDN_ERR_INVALID_ARG, "AIR %u: its lookup program reads preprocessed columns, but the installed preprocessed bundle does not hold AIR %u (mdn_session_set_preprocessed)", i, i);
+    const CommittedMat& pm = prep_c.mats[q];
+    if (pm.log_n != log_heights[i] || pm.width != airs[i].desc.preprocessed_width)
+        fail(MDN_ERR_INVALID_ARG, "AIR %u: the installed preprocessed bundle holds it as 2^%u rows of %u columns, the call needs 2^%u rows of %u", i, pm.log_n, pm.width, log_heights[i], airs[i].desc.preprocessed_width);
+}
+
 // build_logup_aux_trace (air/src/lookup/aux_builder.rs:49-97) for proof position j: fraction collection and
 // per-row sums on the trace domain, exclusive EF prefix sum into column 0, committed final = the grand total.
-void mdn_session::build_logup_aux(u32 j, const u64* main_cm, u64* aux_cm, u64 final_out[2]) {
+// prep_cm: the raw column-major preprocessed rows the lookup program reads, or NULL when it reads none.
+void mdn_session::build_logup_aux(u32 j, const u64* main_cm, const u64* prep_cm, u64* aux_cm, u64 final_out[2]) {
     AirHost& h = airs[order[j]];
     u32 ln = log_heights[order[j]];
     size_t N = (size_t)1 << ln;
     DevBuf totals, scratch, fin;
     totals.alloc(2 * N, stream); scratch.alloc(2 * ((N + 2047) / 2048) + 2, stream); fin.alloc(2, stream);
     mk::LogupArgs la;
-    la.main_cm = main_cm; la.log_n = ln; la.n_cols = h.desc.aux_width; la.prog = h.lookup_dev;
+    la.main_cm = main_cm; la.prep_cm = prep_cm; la.log_n = ln; la.n_cols = h.desc.aux_width; la.prog = h.lookup_dev;
     la.publics = d_publics.p; la.challenges = d_randomness.p; la.aux_cm = aux_cm; la.totals = totals.p; la.bad_flag = (u32*)d_flag.p;
     {
         ProfScope ps(prof, PC_CONSTRAINTS);
         if (h.lookup_jit && h.lookup_jit->checked < 0) h.lookup_jit.reset();
         if (h.lookup_jit) {
             jit::LookupJitArgs ja{};
-            ja.main_lde = la.main_cm; ja.publics = la.publics; ja.challenges = la.challenges;
+            ja.main_lde = la.main_cm; ja.prep_lde = prep_cm; ja.publics = la.publics; ja.challenges = la.challenges;
             ja.periodic = h.lookup_dev.periodic; ja.aux_cm = aux_cm; ja.totals = totals.p; ja.bad_flag = la.bad_flag;
             ja.log_n = ln; ja.n_periodic = h.lookup_dev.n_periodic; ja.log_max_period = h.lookup_dev.log_max_period;
             try { h.lookup_jit->launch(ja, (unsigned)((N + 127) / 128), 128, stream); }
@@ -1647,31 +1688,19 @@ void mdn_session::check_rows(std::vector<mk::CheckArgs>& ca, bool locate, mdn_co
 // the external assertions hold, before the aux commitment: the row pass of check_constraints on what this proof is about
 // to commit.  Main rows: the raw copies of keep_raw_main (or the caller's column-major traces); aux rows: aux_c's
 // coefficient slots, still raw; `flat_values`: the aux values in proof order; challenges and publics: the proof's own.
-// Preprocessed rows are re-derived from the bundle's coefficients by a forward NTT with shift 1 -- exact, and the
-// bundle needs no raw copy whenever the guard was turned on.  Every rank of a split proof runs the whole check on its
-// own whole copies.  A non-zero constraint fails the proof with MDN_ERR_CONSTRAINT_VIOLATED.
+// Preprocessed rows: bundle_prep_rows, shared with the proof's LogUp build.  Every rank of a split proof runs the whole
+// check on its own whole copies.  A non-zero constraint fails the proof with MDN_ERR_CONSTRAINT_VIOLATED.
 void mdn_session::guard_constraints(const std::vector<u64>& flat_values) {
     const u32 k = (u32)airs.size();
     ProfScope ps(prof, PC_CONSTRAINTS);
     DevBuf values; values.alloc(std::max<size_t>(1, flat_values.size()), stream);
     if (!flat_values.empty()) CUDA_OK(cudaMemcpyAsync(values.p, flat_values.data(), flat_values.size() * sizeof(u64), cudaMemcpyHostToDevice, stream));
-    std::vector<DevBuf> prep_rows(k);
     std::vector<mk::CheckArgs> ca(k);
     for (u32 j = 0; j < k; j++) {
         const u32 i = order[j];
         AirHost& h = airs[i];
-        const size_t N = (size_t)1 << log_heights[i];
-        if (h.desc.preprocessed_width) {
-            const u32 q = (u32)(std::find(prep_air.begin(), prep_air.end(), i) - prep_air.begin());   // present: checked by prove_begin
-            const CommittedMat& pm = prep_c.mats[q];
-            prep_rows[i].alloc(N * pm.width, stream);
-            std::vector<mk::FwdItem> items;
-            for (u32 c = 0; c < pm.width; c++) items.push_back(mk::FwdItem{pm.coef + (size_t)c * N, prep_rows[i].p + (size_t)c * N, 0, 0});
-            DevBuf d_items; d_items.alloc(items.size() * sizeof(mk::FwdItem) / sizeof(u64), stream);
-            CUDA_OK(cudaMemcpyAsync(d_items.p, items.data(), items.size() * sizeof(mk::FwdItem), cudaMemcpyHostToDevice, stream));
-            mk::launch_fwd_ntt((const mk::FwdItem*)d_items.p, pm.width, ntt(pm.log_n).T, premul_unshifted(pm.log_n).P, stream);
-        }
-        ca[i] = row_args<mk::CheckArgs>(i, j, h.raw_main_cm, prep_rows[i].p, h.raw_periodic.p, values.p);
+        const u64* prep = h.desc.preprocessed_width ? bundle_prep_rows(i) : nullptr;   // present: checked by prove_begin
+        ca[i] = row_args<mk::CheckArgs>(i, j, h.raw_main_cm, prep, h.raw_periodic.p, values.p);
     }
     mdn_constraint_report rep;
     check_rows(ca, true, &rep);
@@ -1772,7 +1801,7 @@ void mdn_session::prepare_check(const mdn_statement* st, const mdn_matrix* trace
         u32 w = 2 * h.desc.aux_width;
         size_t N = (size_t)1 << log_heights[inst];
         u64 logup_final[2] = {0, 0};
-        if (h.has_lookup) build_logup_aux(j, main_c.mats[j].coef, aux_c.mats[j].coef, logup_final);   // no LDE: the buffer is raw
+        if (h.has_lookup) build_logup_aux(j, main_c.mats[j].coef, cs.prep_cm[inst].p, aux_c.mats[j].coef, logup_final);   // no LDE: the buffer is raw
         else if (w && dev_built) upload_matrix(mdn_matrix{aux_c.mats[j].coef, log_heights[inst], w}, true, aux_c.mats[j].coef, true);   // check only
         else if (w && build_aux) upload_matrix(mdn_matrix{aux_host[inst].data(), log_heights[inst], w}, false, aux_c.mats[j].coef);
         else if (w) CUDA_OK(cudaMemsetAsync(aux_c.mats[j].coef, 0, N * w * sizeof(u64), stream));
@@ -2007,6 +2036,7 @@ void mdn_session::check_trace_balance(const mdn_statement* st, const mdn_matrix*
         }
     }
 
+    for (u32 i = 0; i < k; i++) check_bundle_prep(i);
     std::vector<u32> lookups;
     for (u32 i = 0; i < k; i++) if (airs[i].has_lookup) lookups.push_back(i);
     const std::vector<u64*> main_cm = stage_main(traces, lookups, start.cm, start.on_device);
@@ -2037,7 +2067,7 @@ void mdn_session::check_trace_balance(const mdn_statement* st, const mdn_matrix*
         if (!airs[i].has_lookup) continue;
         mk::BalanceArgs& b = ba[i];
         b = mk::BalanceArgs{};
-        b.main_cm = main_cm[i]; b.log_n = log_heights[i]; b.prog = airs[i].lookup_dev;
+        b.main_cm = main_cm[i]; b.prep_cm = airs[i].lookup_prep ? bundle_prep_rows(i) : nullptr; b.log_n = log_heights[i]; b.prog = airs[i].lookup_dev;
         b.publics = d_publics.p; b.challenges = d_randomness.p; b.instance = i;
         const u32 nc = LookupItems(*st->airs[i].lookup).n, na = (u32)mx[i].group.size();
         if (na) {
@@ -2205,9 +2235,11 @@ void mdn_session::prepare_folds(const mdn_statement* st, const mdn_matrix* trace
 
     // raw main traces and aux slots of the lookup AIRs, column-major (column-major device aux traces are read where the
     // caller keeps them)
+    for (u32 i = 0; i < k; i++) check_bundle_prep(i);
     std::vector<u32> lookups;
     for (u32 i = 0; i < k; i++) if (airs[i].has_lookup) lookups.push_back(i);
     fs.main_cm = stage_main(traces, lookups, cm, on_device);
+    for (u32 i : lookups) if (airs[i].lookup_prep) bundle_prep_rows(i);
     fs.aux_cm.assign(k, nullptr);
     std::vector<u64*>& aux_cm = fs.aux_cm;
     size_t aux_total = 0;
@@ -2241,7 +2273,7 @@ void mdn_session::prepare_folds(const mdn_statement* st, const mdn_matrix* trace
         if (!airs[i].has_lookup) continue;
         if (aux) { finals[i] = gl::e2(aux_finals[i][0], aux_finals[i][1]); continue; }
         u64 fin[2] = {0, 0};
-        build_logup_aux(pos[i], fs.main_cm[i], aux_cm[i], fin);
+        build_logup_aux(pos[i], fs.main_cm[i], airs[i].raw_prep.p, aux_cm[i], fin);
         finals[i] = gl::e2(fin[0], fin[1]);
     }
 }
@@ -2507,7 +2539,7 @@ void mdn_session::commit_aux(const mdn_matrix* aux, const u64* const* aux_values
         CommittedMat& m = aux_c.mats[j];
         u64 logup_final[2] = {0, 0};
         const bool dev_aux = airs[inst].has_lookup;
-        if (dev_aux) build_logup_aux(j, airs[inst].raw_main_cm, m.coef, logup_final);
+        if (dev_aux) build_logup_aux(j, airs[inst].raw_main_cm, airs[inst].lookup_prep ? bundle_prep_rows(inst) : nullptr, m.coef, logup_final);
         else if (w) {
             if (zero_aux) CUDA_OK(cudaMemsetAsync(m.coef, 0, ((size_t)1 << m.log_n) * w * sizeof(u64), stream));
             else {
@@ -2535,10 +2567,8 @@ void mdn_session::commit_aux(const mdn_matrix* aux, const u64* const* aux_values
         if (rc > 0) fail(MDN_ERR_EXTERNAL_ASSERTION, "external assertion %u failed", failed);
         if (rc < 0) fail(MDN_ERR_EXTERNAL_ASSERTION, "eval_external reported a reduction error");
     }
-    if (constraint_guard) {
-        guard_constraints(flat_values);
-        for (AirHost& h : airs) h.raw_main.release();
-    }
+    if (constraint_guard) guard_constraints(flat_values);
+    for (AirHost& h : airs) { h.raw_main.release(); h.raw_prep.release(); }
     lde_and_commit(aux_c, nullptr, nullptr);
     tr.send_commitment(aux_c.root);
     memcpy(dbg_roots[1], aux_c.root, 32);
