@@ -93,7 +93,25 @@ typedef struct {
  *   mdn_check_constraints, mdn_constraint_census                   : the call's own `preprocessed` argument
  *   mdn_check_trace_balance, mdn_check_lookup_folds, mdn_lookup_fold_census : the installed bundle, which must hold
  *       each AIR whose lookup program reads PREPROCESSED at that AIR's height and width (MDN_ERR_INVALID_ARG naming
- *       the AIR otherwise, before any device work); calls whose lookup programs read none do not consult it. */
+ *       the AIR otherwise, before any device work); calls whose lookup programs read none do not consult it.
+ * Version 2 adds register columns after the LogUp ones (the uint chiplets' Schwartz-Zippel columns; the reference's
+ * `num_logup_cols` layout):
+ *   program words[0..6) = { 0x504B4C4D, 2, n_nodes, n_interactions, n_consts, n_registers }
+ *   nodes        : as version 1, plus AUX(a = 0, b = c) with num_columns <= c < aux_width: register c - num_columns's
+ *                  value on the current row
+ *   interactions : as version 1
+ *   registers    : n_registers words, the update node of register i; register i is aux column num_columns + i
+ *   consts       : (lo, hi) pairs
+ * reg_i[0] = 0 and reg_i[r+1] = U_i evaluated on row r (every register read at its row-r value); the LogUp columns and
+ * aux value 0 are what version 1 makes of the same interactions, and the registers take no part in them.  Refused with
+ * MDN_ERR_INVALID_ARG naming the AIR, before any device work: aux_width != num_columns + n_registers; n_registers
+ * outside 1..=4; num_aux_values != 1; an AUX leaf with offset 1 or on a LogUp column; an interaction whose flag,
+ * multiplicity or denominator reaches an AUX leaf; an update not syntactically affine in the registers (register degree:
+ * AUX 1, other leaves 0, ADD / SUB the max, MUL the sum, NEG the same; an update of degree > 1 is refused even where it
+ * cancels).  Version 1 still refuses AUX.  mdn_check_trace_balance runs the interactions only (registers push
+ * nothing); mdn_check_lookup_folds and mdn_lookup_fold_census compare the num_columns LogUp columns only (a given aux
+ * trace still has 2 * aux_width base columns; folds_out stays num_columns wide); the AIR's own constraints check the
+ * registers through mdn_check_constraints.  mdn_jit_compile_check compiles a version-2 program's interaction part. */
 typedef struct {
     uint32_t num_columns;           /* LookupAir::num_columns() */
     uint32_t program_words;

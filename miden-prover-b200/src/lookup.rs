@@ -200,6 +200,10 @@ impl<'b> LookupBatch for RecordingBatch<'b> {
 /// Lower the `LookupAir` of one AIR: `(num_columns, program words)` for `mdn_lookup`.
 /// The backend requires `aux_width == num_columns` (<= 16) and `num_aux_values == 1` -- the shape of every AIR whose
 /// `build_aux_trace` is `build_logup_aux_trace` (all three Miden AIRs, air/src/lib.rs:273-274, 671-685).
+/// This emits version-1 programs only.  AIRs whose aux trace is a LogUp trace followed by register columns (the uint
+/// chiplets' Schwartz-Zippel columns, precompiles-prover/src/uint/trace.rs) need a version-2 program: one update node
+/// per register after the interactions, AUX(0, num_columns + i) for register i's row value, every update affine in
+/// the registers (include/miden_b200.h `mdn_lookup`).  The recorder does not capture those updates yet.
 pub fn lower_lookup<A>(layout: AirLayout, air: &A) -> (u32, Vec<u32>)
 where
     A: LookupAir<RecordingLookupBuilder>,

@@ -90,11 +90,18 @@ class LookupProgramBuilder(ProgramBuilder):
     surface a `LookupBuilder` exposes (main window, preprocessed window `preprocessed(offset, col)` -- the AIR must
     declare preprocessed columns --, periodic values, challenges alpha = challenge(0) and beta = challenge(1),
     constants) and one record per interaction -- `insert(column, flag, multiplicity,
-    denominator)` is `LookupGroup::insert` / `LookupBatch::insert` after `LookupMessage::encode`."""
+    denominator)` is `LookupGroup::insert` / `LookupBatch::insert` after `LookupMessage::encode`.
 
-    def __init__(self, num_columns: int):
+    With `num_registers` > 0 the program also builds register columns after the LogUp ones (a version-2 program, as
+    the uint chiplets' Schwartz-Zippel columns): aux column num_columns + i is register i, 0 on row 0 and
+    `update(i, expr)` evaluated on row r at row r + 1.  `register(i)` is register i's row-r value, readable by updates
+    only, and every update must be affine in the registers."""
+
+    def __init__(self, num_columns: int, num_registers: int = 0):
         super().__init__()
         self.num_columns = num_columns
+        self.num_registers = num_registers
+        self.updates: list[int | None] = [None] * num_registers
         self.interactions: list[tuple[int, int, int, int]] = []
         # mutual-exclusion annotation of every interaction (mdn_check_trace_balance): NO_FLAG, or group << 16 | site
         self.sites: list[int] = []
@@ -187,15 +194,29 @@ class LookupProgramBuilder(ProgramBuilder):
         site = self._batch_site if self._batch_site is not None else self._new_site()
         self.sites.append((g[1] << 16) | site)
 
+    def register(self, i: int) -> Expr:
+        """Register i's value on the current row (the AUX leaf of aux column num_columns + i, offset 0)."""
+        return self._node(OP_AUX, 0, self.num_columns + i)
+
+    def update(self, i: int, e: Expr):
+        """Register i on the next row = `e` evaluated on the current row."""
+        self.updates[i] = e.id
+
     def assert_zero(self, e):  # pragma: no cover - a lookup description emits no constraints
         raise TypeError("LookupBuilder has no assert_* surface")
 
     def serialize(self) -> np.ndarray:
-        w = [LOOKUP_MAGIC, 1, len(self.nodes), len(self.interactions), len(self.consts)]
+        """Version 1 without registers; version 2 (an update node per register after the interactions) with them."""
+        if self.num_registers:
+            assert None not in self.updates, "every register needs an update"
+            w = [LOOKUP_MAGIC, 2, len(self.nodes), len(self.interactions), len(self.consts), self.num_registers]
+        else:
+            w = [LOOKUP_MAGIC, 1, len(self.nodes), len(self.interactions), len(self.consts)]
         for n in self.nodes:
             w += list(n)
         for it in self.interactions:
             w += list(it)
+        w += self.updates
         for c in self.consts:
             w += [c & 0xFFFFFFFF, c >> 32]
         return np.array(w, dtype=np.uint32)

@@ -476,7 +476,9 @@ class Session:
         aux: Matrix array in instance order (host row-major, or device as `flags` say) with aux_finals, per AIR None or
         (c0, c1) -- or None for the device LogUp build of the same call; preprocessed columns come from the installed
         bundle, as in check_trace_balance; folds_out: per AIR None, a uint64 numpy array of
-        rows * num_columns * 4 words to fill, or a device address (int) with FLAG_DEVICE_TRACES.  Returns fold_report_dict."""
+        rows * num_columns * 4 words to fill, or a device address (int) with FLAG_DEVICE_TRACES.  A lookup program with
+        registers (LookupProgramBuilder(num_columns, num_registers)) is compared on its num_columns LogUp columns only: its
+        aux trace keeps every aux column, and check_constraints checks the registers.  Returns fold_report_dict."""
         rnd, marks, fins, keep = _fold_inputs(statement, randomness, fold_marks, aux_finals)
         n, outs = statement.n_airs, None
         if folds_out is not None:

@@ -884,6 +884,208 @@ int launch_logup_rows(const LogupArgs& a, cudaStream_t st) {
     return 0;
 }
 
+// ---------------------------------------------------------------------------------------------
+// Register columns of a version-2 lookup program (kernels.cuh RegisterArgs): affine row maps scanned in row order
+// ---------------------------------------------------------------------------------------------
+// reg[r+1] = A reg[r] + b; composition (A2, b2) o (A1, b1) = (A2 A1, A2 b1 + b2): associative, not commutative
+template <int K> struct RegMap { E2 A[K][K]; E2 b[K]; };
+template <int K> __device__ __forceinline__ RegMap<K> reg_identity() {
+    RegMap<K> m;
+#pragma unroll
+    for (int i = 0; i < K; i++) {
+        m.b[i] = gl::e2(0, 0);
+#pragma unroll
+        for (int j = 0; j < K; j++) m.A[i][j] = gl::e2(i == j, 0);
+    }
+    return m;
+}
+// dst = hi o lo, all three in shared memory
+template <int K> __device__ __forceinline__ void reg_compose(RegMap<K>& dst, const RegMap<K>& hi, const RegMap<K>& lo) {
+#pragma unroll
+    for (int i = 0; i < K; i++) {
+#pragma unroll
+        for (int j = 0; j < K; j++) {
+            E2 s = gl::e2(0, 0);
+#pragma unroll
+            for (int q = 0; q < K; q++) s = gl::e2_add(s, gl::e2_mul(hi.A[i][q], lo.A[q][j]));
+            dst.A[i][j] = s;
+        }
+        E2 bi = hi.b[i];
+#pragma unroll
+        for (int q = 0; q < K; q++) bi = gl::e2_add(bi, gl::e2_mul(hi.A[i][q], lo.b[q]));
+        dst.b[i] = bi;
+    }
+}
+// inclusive scan of the block's maps sm[0 .. blockDim) in thread order, double-buffered in sm[0 .. 2 blockDim): returns
+// the buffer whose entry t is M_t o ... o M_0
+template <int K> __device__ __forceinline__ const RegMap<K>* reg_block_scan(RegMap<K>* sm) {
+    const u32 t = threadIdx.x;
+    RegMap<K>* src = sm;
+    RegMap<K>* dst = sm + blockDim.x;
+    __syncthreads();
+    for (u32 d = 1; d < blockDim.x; d <<= 1) {
+        if (t >= d) reg_compose<K>(dst[t], src[t], src[t - d]);
+        else dst[t] = src[t];
+        __syncthreads();
+        RegMap<K>* x = src; src = dst; dst = x;
+    }
+    return src;
+}
+// registers after the map p: p applied to v
+template <int K> __device__ __forceinline__ void reg_apply(const RegMap<K>& p, E2 (&v)[K]) {
+    E2 w[K];
+#pragma unroll
+    for (int i = 0; i < K; i++) {
+        w[i] = p.b[i];
+#pragma unroll
+        for (int j = 0; j < K; j++) w[i] = gl::e2_add(w[i], gl::e2_mul(p.A[i][j], v[j]));
+    }
+#pragma unroll
+    for (int i = 0; i < K; i++) v[i] = w[i];
+}
+// M_r into m (shared memory): the register program evaluated k + 1 times on row r, the registers set to 0 (b_r) and
+// then to each unit vector (b_r + A_r e_j).  The updates are affine in the registers (validated on the host), so this
+// is exact.
+template <int K, int MAXS> __device__ __forceinline__ void reg_row_map(const RegisterArgs& a, size_t r, RegMap<K>& m) {
+    const size_t N = (size_t)1 << a.log_n, rn = (r + 1) & (N - 1);
+    const size_t per_row = (r & (((size_t)1 << a.prog.log_max_period) - 1)) * a.prog.n_periodic;
+    E2 slot[MAXS];
+    const uint4* code = reinterpret_cast<const uint4*>(a.prog.code);
+    for (u32 e = 0; e <= (u32)K; e++) {
+        for (u32 i = 0; i < a.prog.n_instr; i++) {
+            uint4 ins = code[i];
+            u32 op = ins.x & 0xff, ext = ins.x >> 8, x = ins.z, y = ins.w;
+            E2 v;
+            switch (op) {
+                LOOKUP_NODE_CASES(a, N, r, rn, per_row, slot, x, y, ext, v)
+                case 1: v = gl::e2(y + 1 == e, 0); break;   // REGISTER: the basis value of this evaluation
+                default:                                     // 15 STORE update ins.y
+                    if (e == 0) m.b[ins.y] = slot[x];
+                    else m.A[ins.y][e - 1] = gl::e2_sub(slot[x], m.b[ins.y]);
+                    continue;
+            }
+            slot[ins.y] = v;
+        }
+    }
+}
+template <int K> __device__ __forceinline__ void reg_store(u64* p, const RegMap<K>& m) {
+#pragma unroll
+    for (int i = 0; i < K; i++) {
+#pragma unroll
+        for (int j = 0; j < K; j++) { p[2 * (i * K + j)] = m.A[i][j].a; p[2 * (i * K + j) + 1] = m.A[i][j].b; }
+        p[2 * (K * K + i)] = m.b[i].a; p[2 * (K * K + i) + 1] = m.b[i].b;
+    }
+}
+template <int K> __device__ __forceinline__ RegMap<K> reg_load(const u64* p) {
+    RegMap<K> m;
+#pragma unroll
+    for (int i = 0; i < K; i++) {
+#pragma unroll
+        for (int j = 0; j < K; j++) m.A[i][j] = gl::e2(p[2 * (i * K + j)], p[2 * (i * K + j) + 1]);
+        m.b[i] = gl::e2(p[2 * (K * K + i)], p[2 * (K * K + i) + 1]);
+    }
+    return m;
+}
+static constexpr size_t reg_map_words(u32 k) { return 2 * (size_t)k * (k + 1); }
+size_t register_scratch_words(u32 log_n, u32 n_regs) {
+    size_t nb = (((size_t)1 << log_n) + REG_BLOCK - 1) / REG_BLOCK;
+    return nb * (reg_map_words(n_regs) + 2 * n_regs);   // block aggregates, then each block's incoming registers
+}
+// phase 1: the composition of each block's row maps
+template <int K, int MAXS>
+__global__ void __launch_bounds__(REG_BLOCK) k_reg_block_maps(RegisterArgs a) {
+    extern __shared__ u64 reg_smem[];
+    RegMap<K>* sm = reinterpret_cast<RegMap<K>*>(reg_smem);
+    reg_row_map<K, MAXS>(a, (size_t)blockIdx.x * blockDim.x + threadIdx.x, sm[threadIdx.x]);
+    const RegMap<K>* res = reg_block_scan<K>(sm);
+    if (threadIdx.x == blockDim.x - 1) reg_store<K>(a.scratch + reg_map_words(K) * blockIdx.x, res[threadIdx.x]);
+}
+// phase 2 (one block): the aggregates scanned in chunks of REG_BLOCK; carry[blk] = the registers at block blk's first row
+template <int K>
+__global__ void __launch_bounds__(REG_BLOCK) k_reg_block_carry(RegisterArgs a, u32 n_blocks) {
+    extern __shared__ u64 reg_smem[];
+    RegMap<K>* sm = reinterpret_cast<RegMap<K>*>(reg_smem);
+    __shared__ E2 v_sh[K];
+    const u32 t = threadIdx.x;
+    const u64* agg = a.scratch;
+    u64* carry = a.scratch + reg_map_words(K) * n_blocks;
+    if (t < K) v_sh[t] = gl::e2(0, 0);
+    __syncthreads();
+    for (u32 c0 = 0; c0 < n_blocks; c0 += REG_BLOCK) {
+        E2 v[K];
+#pragma unroll
+        for (int i = 0; i < K; i++) v[i] = v_sh[i];
+        sm[t] = c0 + t < n_blocks ? reg_load<K>(agg + reg_map_words(K) * (c0 + t)) : reg_identity<K>();
+        const RegMap<K>* res = reg_block_scan<K>(sm);
+        if (t == 0) for (int i = 0; i < K; i++) { carry[2 * (K * (size_t)c0 + i)] = v[i].a; carry[2 * (K * (size_t)c0 + i) + 1] = v[i].b; }
+        reg_apply<K>(res[t], v);   // the registers after block c0 + t
+        if (c0 + t + 1 < n_blocks)
+            for (int i = 0; i < K; i++) { carry[2 * (K * (size_t)(c0 + t + 1) + i)] = v[i].a; carry[2 * (K * (size_t)(c0 + t + 1) + i) + 1] = v[i].b; }
+        __syncthreads();
+        if (t == REG_BLOCK - 1) for (int i = 0; i < K; i++) v_sh[i] = v[i];
+        __syncthreads();
+    }
+}
+// phase 3: each block recomputes and scans its row maps, applies its incoming registers and writes the register planes
+template <int K, int MAXS>
+__global__ void __launch_bounds__(REG_BLOCK) k_reg_apply(RegisterArgs a, u32 n_blocks) {
+    extern __shared__ u64 reg_smem[];
+    RegMap<K>* sm = reinterpret_cast<RegMap<K>*>(reg_smem);
+    const size_t N = (size_t)1 << a.log_n, r = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    reg_row_map<K, MAXS>(a, r, sm[threadIdx.x]);
+    const RegMap<K>* res = reg_block_scan<K>(sm);
+    const u64* carry = a.scratch + reg_map_words(K) * n_blocks + 2 * (size_t)K * blockIdx.x;
+    E2 v[K];
+#pragma unroll
+    for (int i = 0; i < K; i++) v[i] = gl::e2(carry[2 * i], carry[2 * i + 1]);
+    // reg[r] = (M_{r-1} o ... o M_base) applied to the registers at the block's first row
+    if (threadIdx.x > 0) reg_apply<K>(res[threadIdx.x - 1], v);
+    bool bad = false;
+#pragma unroll
+    for (int i = 0; i < K; i++) {
+        bad |= v[i].a >= gl::P || v[i].b >= gl::P;
+        a.aux_cm[(size_t)(2 * (a.col0 + i)) * N + r] = v[i].a;
+        a.aux_cm[(size_t)(2 * (a.col0 + i) + 1) * N + r] = v[i].b;
+    }
+    if (bad) atomicOr(a.bad_flag, 1u);
+}
+template <int K, int MAXS> static int launch_registers_k(const RegisterArgs& a, cudaStream_t st) {
+    const size_t N = (size_t)1 << a.log_n;
+    const unsigned threads = (unsigned)std::min<size_t>(N, REG_BLOCK), nb = (unsigned)(N / threads);
+    // two buffers of maps per block: 80 KiB at k = 4, above the default 48 KiB
+    const size_t smem = 2 * sizeof(RegMap<K>) * threads, smem2 = 2 * sizeof(RegMap<K>) * REG_BLOCK;
+    cudaError_t e = cudaFuncSetAttribute(k_reg_block_maps<K, MAXS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(k_reg_block_carry<K>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem2);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(k_reg_apply<K, MAXS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return (int)e;
+    // a launch configuration error is not sticky: check after each launch
+    k_reg_block_maps<K, MAXS><<<nb, threads, smem, st>>>(a);
+    COUNT_LAUNCH();
+    if ((e = cudaGetLastError()) != cudaSuccess) return (int)e;
+    k_reg_block_carry<K><<<1, REG_BLOCK, smem2, st>>>(a, nb);
+    COUNT_LAUNCH();
+    if ((e = cudaGetLastError()) != cudaSuccess) return (int)e;
+    k_reg_apply<K, MAXS><<<nb, threads, smem, st>>>(a, nb);
+    COUNT_LAUNCH();
+    return (int)cudaGetLastError();
+}
+template <int K> static int launch_registers_slots(const RegisterArgs& a, cudaStream_t st) {
+    if (a.prog.n_slots <= 16) return launch_registers_k<K, 16>(a, st);
+    if (a.prog.n_slots <= 64) return launch_registers_k<K, 64>(a, st);
+    if (a.prog.n_slots <= 256) return launch_registers_k<K, 256>(a, st);
+    if (a.prog.n_slots <= 1024) return launch_registers_k<K, 1024>(a, st);
+    return -1;
+}
+int launch_register_columns(const RegisterArgs& a, cudaStream_t st) {
+    switch (a.n_regs) {
+        case 1: return launch_registers_slots<1>(a, st);
+        case 2: return launch_registers_slots<2>(a, st);
+        case 3: return launch_registers_slots<3>(a, st);
+        case 4: return launch_registers_slots<4>(a, st);
+        default: return -1;
+    }
+}
+
 // =============================================================================================
 // Constraint check on the trace domain (debug.rs check_constraints): the constraint program of k_constraints, read
 // on raw rows with exact 0/1 selectors; FOLD k tests constraint k instead of folding it

@@ -181,6 +181,28 @@ int launch_logup_rows(const LogupArgs& a, cudaStream_t st);   // 0, or -1 when t
 void launch_ef_exclusive_scan(const u64* totals, size_t n, u64* acc0, u64* acc1, u64* final2, u64* scratch, cudaStream_t st);
 static constexpr u32 LOGUP_MAX_COLS = 16;
 
+// Register columns of a version-2 lookup program: reg_i[0] = 0, reg_i[r+1] = U_i(row r, reg[r]), every U_i affine in the
+// registers.  The compiled register program is the lookup instruction format plus op 1 = REGISTER {op, dst, 0, register
+// index} (the row-r value of that register) and op 15 = STORE {op, update index, slot, 0}.  Each row's map
+// M_r = (A_r, b_r), reg[r+1] = A_r reg[r] + b_r, comes from k + 1 evaluations (registers 0, then each unit vector); the
+// maps are composed in row order by a three-phase scan over 128-row blocks (aggregates, scan of the aggregates,
+// recompute and apply), so scratch is O(N / 128) maps.
+static constexpr u32 REG_MAX = 4, REG_BLOCK = 128;
+struct RegisterArgs {
+    const u64* main_cm;      // raw main trace, column-major [col][row]
+    const u64* prep_cm;      // raw preprocessed trace, column-major, or NULL
+    u32 log_n, n_regs;       // trace height, registers (1..REG_MAX)
+    u32 col0;                // aux column of register 0 (LookupAir::num_columns)
+    AirDev prog;             // periodic = RAW periodic matrix, row-major (max_period x n_periodic)
+    const u64* publics; const u64* challenges;
+    u64* aux_cm;             // aux trace, column-major planes [2c + coord][row]; planes 2(col0 + i), +1 are written
+    u64* scratch;            // register_scratch_words(log_n, n_regs) u64
+    u32* bad_flag;           // bit 0: a non-canonical register value (never expected: the field ops are canonical)
+};
+size_t register_scratch_words(u32 log_n, u32 n_regs);
+// 0; -1 when the program needs too many slots or registers; otherwise the cudaError_t of a failed attribute call or launch
+int launch_register_columns(const RegisterArgs& a, cudaStream_t st);
+
 // ---------------------------------------------------------------------------------------------
 // Constraint check without proving (mdn_check_constraints; reference crates/lifted-stark/src/debug.rs:70-214)
 // ---------------------------------------------------------------------------------------------

@@ -186,10 +186,20 @@ struct AirHost {
     DevBuf lookup_program, raw_main, raw_periodic;
     const u64* raw_main_cm = nullptr;
     mk::AirDev lookup_dev;
-    // lookup_prep: the lookup program reads preprocessed columns (op 15).  raw_prep: the raw column-major rows of the
+    // lookup_prep: the lookup program's interaction part reads preprocessed columns (op 15); reg_prep: its register
+    // updates do (a proof's LogUp build then needs the rows; the lookup checks, which build no registers, do not).  raw_prep: the raw column-major rows of the
     // installed bundle's preprocessed trace of this AIR, derived once per proof or check (mdn_session::bundle_prep_rows)
-    bool lookup_prep = false;
+    bool lookup_prep = false, reg_prep = false;
     DevBuf raw_prep;
+    // lookup_v1: the lookup program's interaction part as a version-1 program, which the LogUp build and the three
+    // lookup checks run (the caller's words for a version-1 program, lookup_words for a version-2 one).
+    // lookup_cols: its LogUp columns.  A version-2 program's n_regs register columns follow them, built from the
+    // compiled register program reg_dev (kernels.cuh RegisterArgs; it shares lookup_dev's periodic matrix).
+    mdn_lookup lookup_v1{};
+    std::vector<u32> lookup_words;
+    u32 lookup_cols = 0, n_regs = 0;
+    DevBuf reg_program;
+    mk::AirDev reg_dev{};
     // NVRTC-specialised constraint kernel (jit.hpp) for large programs; NULL = interpreter.  check_jit / census_jit:
     // the two entry points of the program's trace-check cubin (k_jit_check, k_jit_census), loaded for the checks and
     // for a guarded proof
@@ -329,7 +339,8 @@ struct mdn_session {
     void keep_raw_main(u32 j, const u64* caller_cm);
     const u64* bundle_prep_rows(u32 i);
     void check_bundle_prep(u32 i);
-    void build_logup_aux(u32 j, const u64* main_cm, const u64* prep_cm, u64* aux_cm, u64 final_out[2]);
+    // registers == false: the LogUp columns only (the lookup checks, which compare no register column)
+    void build_logup_aux(u32 j, const u64* main_cm, const u64* prep_cm, u64* aux_cm, u64 final_out[2], bool registers = true);
     void lde_and_commit(Committed& c, float* t_lde, float* t_hash, bool lde_done = false);
     cudaStream_t copy_stream = nullptr;
     cudaEvent_t copy_ev[8];
@@ -407,7 +418,7 @@ struct mdn_session {
     // the fold kernels' inputs of lookup AIR i (kernels.cuh LookupFoldArgs, FoldCensusArgs name them alike)
     template <class Args> Args fold_args(u32 i, const FoldSetup& fs) const {
         Args f{};
-        f.main_cm = fs.main_cm[i]; f.prep_cm = airs[i].raw_prep.p; f.log_n = log_heights[i]; f.n_cols = airs[i].desc.aux_width; f.prog = airs[i].lookup_dev;
+        f.main_cm = fs.main_cm[i]; f.prep_cm = airs[i].raw_prep.p; f.log_n = log_heights[i]; f.n_cols = airs[i].lookup_cols; f.prog = airs[i].lookup_dev;
         f.publics = d_publics.p; f.challenges = d_randomness.p; f.marks = (const u32*)fs.marks[i].p;
         f.aux_cm = fs.aux_cm[i]; f.final = fs.finals[i];
         return f;
@@ -863,6 +874,24 @@ u64 mdn_session::grind(u32 bits) {
 // op-list compiler: validation, liveness, slot assignment (shared by constraint and lookup programs)
 // ---------------------------------------------------------------------------------------------
 struct Compiled { std::vector<u32> code; std::vector<u64> consts; u32 n_slots = 0; bool uses_sel = false; };
+// node j = (op, x, y) of AIR i's program with nk constants: op and operands in range, operands defined before j
+static void check_node(u32 i, const mdn_air& a, u32 n_publics, u32 nk, bool lookup, u32 j, u32 op, u32 x, u32 y) {
+    if (op > 15) fail(MDN_ERR_INVALID_ARG, "AIR %u: unknown op %u", i, op);
+    // a LookupBuilder exposes the main and preprocessed windows, periodic values, public values, challenges and
+    // constants only
+    if (lookup && (op == 1 || (op >= 4 && op <= 7))) fail(MDN_ERR_INVALID_ARG, "AIR %u: op %u is not available to a lookup program", i, op);
+    if (op == 15 && (x > 1 || y >= a.preprocessed_width)) fail(MDN_ERR_INVALID_ARG, "AIR %u: preprocessed column out of range", i);
+    if (op >= 10 && op <= 12 && (x >= j || y >= j)) fail(MDN_ERR_INVALID_ARG, "AIR %u: forward reference", i);
+    if (op == 13 && x >= j) fail(MDN_ERR_INVALID_ARG, "AIR %u: forward reference", i);
+    if (op == 0 && (x > 1 || y >= a.width)) fail(MDN_ERR_INVALID_ARG, "AIR %u: main column out of range", i);
+    if (op == 1 && (x > 1 || y >= a.aux_width)) fail(MDN_ERR_INVALID_ARG, "AIR %u: aux column out of range", i);
+    if (op == 2 && x >= n_publics) fail(MDN_ERR_INVALID_ARG, "AIR %u: public value out of range", i);
+    if (op == 3 && x >= a.num_randomness) fail(MDN_ERR_INVALID_ARG, "AIR %u: challenge out of range", i);
+    if (op == 4 && x >= a.num_aux_values) fail(MDN_ERR_INVALID_ARG, "AIR %u: aux value out of range", i);
+    if (op == 8 && x >= nk) fail(MDN_ERR_INVALID_ARG, "AIR %u: constant out of range", i);
+    if (op == 9 && x + 1 >= nk) fail(MDN_ERR_INVALID_ARG, "AIR %u: constant out of range", i);
+    if (op == 14 && x >= a.num_periodic_columns) fail(MDN_ERR_INVALID_ARG, "AIR %u: periodic column out of range", i);
+}
 // lookup == false: words = [MAIR, 1, n_nodes, n_constraints, n_consts | nodes | constraint node ids | consts];
 //                  a FOLD instruction (15) is placed right after the node it folds, in emission order.
 // lookup == true : words = [MLKP, 1, n_nodes, n_interactions, n_consts | nodes | {column, flag, mult, denom} | consts];
@@ -877,22 +906,8 @@ static Compiled compile_oplist(u32 i, const mdn_air& a, u32 n_publics, const u32
     const u32* items = w + 5 + 3 * (size_t)nn;
     for (u32 j = 0; j < nn; j++) {
         u32 op = w[5 + 3 * j], x = w[6 + 3 * j], y = w[7 + 3 * j];
-        if (op > 15) fail(MDN_ERR_INVALID_ARG, "AIR %u: unknown op %u", i, op);
-        // a LookupBuilder exposes the main and preprocessed windows, periodic values, public values, challenges and
-        // constants only
-        if (lookup && (op == 1 || (op >= 4 && op <= 7))) fail(MDN_ERR_INVALID_ARG, "AIR %u: op %u is not available to a lookup program", i, op);
-        if (op == 15 && (x > 1 || y >= a.preprocessed_width)) fail(MDN_ERR_INVALID_ARG, "AIR %u: preprocessed column out of range", i);
+        check_node(i, a, n_publics, nk, lookup, j, op, x, y);
         if (op >= 5 && op <= 7) out.uses_sel = true;
-        if (op >= 10 && op <= 12 && (x >= j || y >= j)) fail(MDN_ERR_INVALID_ARG, "AIR %u: forward reference", i);
-        if (op == 13 && x >= j) fail(MDN_ERR_INVALID_ARG, "AIR %u: forward reference", i);
-        if (op == 0 && (x > 1 || y >= a.width)) fail(MDN_ERR_INVALID_ARG, "AIR %u: main column out of range", i);
-        if (op == 1 && (x > 1 || y >= a.aux_width)) fail(MDN_ERR_INVALID_ARG, "AIR %u: aux column out of range", i);
-        if (op == 2 && x >= n_publics) fail(MDN_ERR_INVALID_ARG, "AIR %u: public value out of range", i);
-        if (op == 3 && x >= a.num_randomness) fail(MDN_ERR_INVALID_ARG, "AIR %u: challenge out of range", i);
-        if (op == 4 && x >= a.num_aux_values) fail(MDN_ERR_INVALID_ARG, "AIR %u: aux value out of range", i);
-        if (op == 8 && x >= nk) fail(MDN_ERR_INVALID_ARG, "AIR %u: constant out of range", i);
-        if (op == 9 && x + 1 >= nk) fail(MDN_ERR_INVALID_ARG, "AIR %u: constant out of range", i);
-        if (op == 14 && x >= a.num_periodic_columns) fail(MDN_ERR_INVALID_ARG, "AIR %u: periodic column out of range", i);
     }
     // event stream: node definitions, each followed by the folds / emits that became ready
     struct Ev { u32 kind; u32 node; };   // kind 0: define node; 1: fold node / emit interaction `node`
@@ -983,6 +998,98 @@ static Compiled compile_oplist(u32 i, const mdn_air& a, u32 n_publics, const u32
         out.consts.push_back(v);
     }
     return out;
+}
+
+// A version-2 lookup program of AIR i (words = [MLKP, 2, n_nodes, n_interactions, n_consts, n_registers | nodes |
+// {column, flag, mult, denom} | update node per register | consts]), validated and split in two:
+//   v1   : the interaction part, a version-1 program of the nodes the interactions reach (renumbered in order), which
+//          every consumer of version-1 programs takes as it is;
+//   regs : the register part in the constraint-program format, its "constraints" being the update nodes, over the nodes
+//          the updates reach; AUX(0, num_columns + i) reads register i.
+struct LookupSplit { std::vector<u32> v1, regs; u32 n_regs = 0; };
+static LookupSplit split_lookup_v2(u32 i, const mdn_air& a, u32 n_publics, const mdn_lookup& lk) {
+    const u32* w = lk.program;
+    const u32 n_words = lk.program_words;
+    if (n_words < 6) fail(MDN_ERR_INVALID_ARG, "AIR %u: bad lookup program header", i);
+    const u32 nn = w[2], nc = w[3], nk = w[4], nr = w[5];
+    if ((size_t)n_words != 6 + 3 * (size_t)nn + 4 * (size_t)nc + nr + 2 * (size_t)nk) fail(MDN_ERR_INVALID_ARG, "AIR %u: bad lookup program length", i);
+    if (nr < 1 || nr > mk::REG_MAX) fail(MDN_ERR_INVALID_ARG, "AIR %u: a version-2 lookup program has 1..=%u registers, not %u", i, mk::REG_MAX, nr);
+    if (a.aux_width != lk.num_columns + nr || a.num_aux_values != 1)
+        fail(MDN_ERR_INVALID_ARG, "AIR %u: a lookup program with registers needs aux_width == num_columns + n_registers and num_aux_values == 1", i);
+    const u32* nodes = w + 6;
+    const u32* items = nodes + 3 * (size_t)nn;
+    const u32* upd = items + 4 * (size_t)nc;
+    const u32* kw = upd + nr;
+    // vocabulary and ranges; the AUX leaf is a register's row-r value; register degree of every node
+    std::vector<uint8_t> deg(nn, 0);
+    for (u32 j = 0; j < nn; j++) {
+        const u32 op = nodes[3 * j], x = nodes[3 * j + 1], y = nodes[3 * j + 2];
+        if (op == 1) {
+            if (x != 0 || y < lk.num_columns || y >= a.aux_width) fail(MDN_ERR_INVALID_ARG, "AIR %u: node %u: an AUX leaf must read a register column at offset 0", i, j);
+            deg[j] = 1;
+            continue;
+        }
+        check_node(i, a, n_publics, nk, true, j, op, x, y);
+        if (op == 10 || op == 11) deg[j] = std::max(deg[x], deg[y]);
+        else if (op == 12) deg[j] = (uint8_t)std::min(2, deg[x] + deg[y]);
+        else if (op == 13) deg[j] = deg[x];
+    }
+    for (u32 q = 0; q < nr; q++) {
+        if (upd[q] >= nn) fail(MDN_ERR_INVALID_ARG, "AIR %u: bad register update node", i);
+        if (deg[upd[q]] > 1) fail(MDN_ERR_INVALID_ARG, "AIR %u: the update of register %u is not affine in the registers", i, q);
+    }
+    for (u32 q = 0; q < nc; q++) {
+        const u32* it = items + 4 * (size_t)q;
+        if ((it[1] != 0xFFFFFFFFu && it[1] >= nn) || it[2] >= nn || it[3] >= nn) fail(MDN_ERR_INVALID_ARG, "AIR %u: bad lookup interaction", i);
+    }
+    // the nodes each part reaches (operands precede their node, so one backward pass)
+    auto reach = [&](std::vector<uint8_t>& m) {
+        for (u32 j = nn; j-- > 0;) {
+            if (!m[j]) continue;
+            const u32 op = nodes[3 * j];
+            if (op >= 10 && op <= 12) { m[nodes[3 * j + 1]] = 1; m[nodes[3 * j + 2]] = 1; }
+            else if (op == 13) m[nodes[3 * j + 1]] = 1;
+        }
+    };
+    std::vector<uint8_t> in_v1(nn, 0), in_regs(nn, 0);
+    for (u32 q = 0; q < nc; q++) {
+        const u32* it = items + 4 * (size_t)q;
+        if (it[1] != 0xFFFFFFFFu) in_v1[it[1]] = 1;
+        in_v1[it[2]] = 1; in_v1[it[3]] = 1;
+    }
+    for (u32 q = 0; q < nr; q++) in_regs[upd[q]] = 1;
+    reach(in_v1); reach(in_regs);
+    for (u32 j = 0; j < nn; j++)
+        if (in_v1[j] && deg[j]) fail(MDN_ERR_INVALID_ARG, "AIR %u: a lookup interaction reads a register (node %u); registers are read by register updates only", i, j);
+    // one part: the kept nodes renumbered, then its items, then every constant
+    auto part = [&](const std::vector<uint8_t>& keep, u32 magic, u32 n_items, auto&& emit_items) {
+        std::vector<u32> id(nn, 0), out = {magic, 1, 0, n_items, nk};
+        u32 m = 0;
+        for (u32 j = 0; j < nn; j++) {
+            if (!keep[j]) continue;
+            u32 op = nodes[3 * j], x = nodes[3 * j + 1], y = nodes[3 * j + 2];
+            if (op >= 10 && op <= 12) { x = id[x]; y = id[y]; }
+            else if (op == 13) x = id[x];
+            out.insert(out.end(), {op, x, y});
+            id[j] = m++;
+        }
+        out[2] = m;
+        emit_items(out, id);
+        out.insert(out.end(), kw, kw + 2 * (size_t)nk);
+        return out;
+    };
+    LookupSplit s;
+    s.n_regs = nr;
+    s.v1 = part(in_v1, 0x504B4C4Du, nc, [&](std::vector<u32>& out, const std::vector<u32>& id) {
+        for (u32 q = 0; q < nc; q++) {
+            const u32* it = items + 4 * (size_t)q;
+            out.insert(out.end(), {it[0], it[1] == 0xFFFFFFFFu ? it[1] : id[it[1]], id[it[2]], id[it[3]]});
+        }
+    });
+    s.regs = part(in_regs, 0x5249414Du, nr, [&](std::vector<u32>& out, const std::vector<u32>& id) {
+        for (u32 q = 0; q < nr; q++) out.push_back(id[upd[q]]);
+    });
+    return s;
 }
 
 
@@ -1162,26 +1269,52 @@ void mdn_session::bind_airs(const mdn_statement* st, const mdn_matrix* traces, b
         // lowered LookupAir -> the aux trace of this AIR is built on the device (commit_aux)
         h.has_lookup = a.lookup != nullptr;
         if (h.has_lookup) {
-            const mdn_lookup& lk = *a.lookup;
-            if (lk.num_columns != a.aux_width || a.num_aux_values != 1) fail(MDN_ERR_INVALID_ARG, "AIR %u: a lookup program needs aux_width == num_columns and num_aux_values == 1", i);
+            const bool v2 = a.lookup->program && a.lookup->program_words >= 2 && a.lookup->program[0] == 0x504B4C4Du && a.lookup->program[1] == 2;
+            h.lookup_words.clear(); h.n_regs = 0;
+            LookupSplit split;
+            if (v2) {
+                split = split_lookup_v2(i, a, st->n_public_values, *a.lookup);
+                h.lookup_words = std::move(split.v1); h.n_regs = split.n_regs;
+                h.lookup_v1 = mdn_lookup{a.lookup->num_columns, (u32)h.lookup_words.size(), h.lookup_words.data()};
+            } else h.lookup_v1 = *a.lookup;
+            const mdn_lookup& lk = h.lookup_v1;
+            h.lookup_cols = lk.num_columns;
+            if (!v2 && (lk.num_columns != a.aux_width || a.num_aux_values != 1)) fail(MDN_ERR_INVALID_ARG, "AIR %u: a lookup program needs aux_width == num_columns and num_aux_values == 1", i);
             if (lk.num_columns == 0 || lk.num_columns > mk::LOGUP_MAX_COLS) fail(MDN_ERR_UNSUPPORTED, "AIR %u: at most %u lookup columns", i, mk::LOGUP_MAX_COLS);
             Compiled lc = compile_oplist(i, a, st->n_public_values, lk.program, lk.program_words, true, lk.num_columns);
-            size_t c_off = (lc.code.size() + 1) / 2, p_off = c_off + lc.consts.size() + 2;
-            size_t np = a.num_periodic_columns, mp = (size_t)1 << a.log_max_period;
-            std::vector<u64> hp(p_off + np * mp, 0);
-            memcpy(hp.data(), lc.code.data(), lc.code.size() * sizeof(u32));
-            for (size_t j = 0; j < lc.consts.size(); j++) hp[c_off + j] = lc.consts[j];
-            for (size_t q = 0; q < np * mp; q++) hp[p_off + q] = a.periodic_values[q];   // canonical: checked above
-            h.lookup_program.alloc(hp.size(), stream);
-            CUDA_OK(cudaMemcpyAsync(h.lookup_program.p, hp.data(), hp.size() * sizeof(u64), cudaMemcpyHostToDevice, stream));
-            CUDA_OK(cudaStreamSynchronize(stream));
-            h.lookup_dev = mk::AirDev{};
-            h.lookup_dev.code = (const u32*)h.lookup_program.p; h.lookup_dev.consts = h.lookup_program.p + c_off;
-            h.lookup_dev.periodic = np ? h.lookup_program.p + p_off : nullptr;
-            h.lookup_dev.n_instr = (u32)(lc.code.size() / 4); h.lookup_dev.n_slots = std::max(1u, lc.n_slots);
-            h.lookup_dev.log_max_period = a.log_max_period; h.lookup_dev.n_periodic = a.num_periodic_columns;
-            h.lookup_prep = false;
+            // code | consts | raw periodic matrix, on the device
+            auto upload = [&](const Compiled& c, DevBuf& buf, mk::AirDev& d) {
+                size_t c_off = (c.code.size() + 1) / 2, p_off = c_off + c.consts.size() + 2;
+                size_t np = a.num_periodic_columns, mp = (size_t)1 << a.log_max_period;
+                std::vector<u64> hp(p_off + np * mp, 0);
+                memcpy(hp.data(), c.code.data(), c.code.size() * sizeof(u32));
+                for (size_t j = 0; j < c.consts.size(); j++) hp[c_off + j] = c.consts[j];
+                for (size_t q = 0; q < np * mp; q++) hp[p_off + q] = a.periodic_values[q];   // canonical: checked above
+                buf.alloc(hp.size(), stream);
+                CUDA_OK(cudaMemcpyAsync(buf.p, hp.data(), hp.size() * sizeof(u64), cudaMemcpyHostToDevice, stream));
+                CUDA_OK(cudaStreamSynchronize(stream));
+                d = mk::AirDev{};
+                d.code = (const u32*)buf.p; d.consts = buf.p + c_off;
+                d.periodic = np ? buf.p + p_off : nullptr;
+                d.n_instr = (u32)(c.code.size() / 4); d.n_slots = std::max(1u, c.n_slots);
+                d.log_max_period = a.log_max_period; d.n_periodic = a.num_periodic_columns;
+            };
+            upload(lc, h.lookup_program, h.lookup_dev);
+            if (v2) {
+                // the register updates as constraints: the m-th FOLD (emitted in constraint order) becomes STORE m, and
+                // AUX(0, num_columns + q) becomes REGISTER q
+                Compiled rc = compile_oplist(i, a, st->n_public_values, split.regs.data(), (u32)split.regs.size(), false, 0);
+                u32 m = 0;
+                for (size_t q = 0; q < rc.code.size(); q += 4) {
+                    const u32 op = rc.code[q] & 0xff;
+                    if (op == 15) rc.code[q + 1] = m++;
+                    else if (op == 1) rc.code[q + 3] -= lk.num_columns;
+                }
+                upload(rc, h.reg_program, h.reg_dev);
+            }
+            h.lookup_prep = h.reg_prep = false;
             for (u32 j = 0; j < lk.program[2]; j++) h.lookup_prep |= lk.program[5 + 3 * (size_t)j] == 15;
+            for (u32 j = 0; v2 && j < split.regs[2]; j++) h.reg_prep |= split.regs[5 + 3 * (size_t)j] == 15;
             h.lookup_jit.reset();
             if (jit && jit_min_nodes && lk.program[2] >= jit_min_nodes) {
                 try {
@@ -1418,14 +1551,14 @@ void mdn_session::check_bundle_prep(u32 i) {
 // build_logup_aux_trace (air/src/lookup/aux_builder.rs:49-97) for proof position j: fraction collection and
 // per-row sums on the trace domain, exclusive EF prefix sum into column 0, committed final = the grand total.
 // prep_cm: the raw column-major preprocessed rows the lookup program reads, or NULL when it reads none.
-void mdn_session::build_logup_aux(u32 j, const u64* main_cm, const u64* prep_cm, u64* aux_cm, u64 final_out[2]) {
+void mdn_session::build_logup_aux(u32 j, const u64* main_cm, const u64* prep_cm, u64* aux_cm, u64 final_out[2], bool registers) {
     AirHost& h = airs[order[j]];
     u32 ln = log_heights[order[j]];
     size_t N = (size_t)1 << ln;
     DevBuf totals, scratch, fin;
     totals.alloc(2 * N, stream); scratch.alloc(2 * ((N + 2047) / 2048) + 2, stream); fin.alloc(2, stream);
     mk::LogupArgs la;
-    la.main_cm = main_cm; la.prep_cm = prep_cm; la.log_n = ln; la.n_cols = h.desc.aux_width; la.prog = h.lookup_dev;
+    la.main_cm = main_cm; la.prep_cm = prep_cm; la.log_n = ln; la.n_cols = h.lookup_cols; la.prog = h.lookup_dev;
     la.publics = d_publics.p; la.challenges = d_randomness.p; la.aux_cm = aux_cm; la.totals = totals.p; la.bad_flag = (u32*)d_flag.p;
     {
         ProfScope ps(prof, PC_CONSTRAINTS);
@@ -1442,7 +1575,7 @@ void mdn_session::build_logup_aux(u32 j, const u64* main_cm, const u64* prep_cm,
                 // first use: the interpreter builds the same rows into scratch buffers; fraction columns and row totals
                 // must agree word for word, otherwise the interpreter's result is kept and the kernel is retired
                 DevBuf aux2, tot2;
-                u32 C = h.desc.aux_width;
+                u32 C = h.lookup_cols;
                 aux2.alloc(2 * (size_t)C * N, stream); tot2.alloc(2 * N, stream);
                 mk::LogupArgs lb2 = la; lb2.aux_cm = aux2.p; lb2.totals = tot2.p;
                 if (mk::launch_logup_rows(lb2, stream) != 0) fail(MDN_ERR_UNSUPPORTED, "lookup program too large for the interpreter");
@@ -1465,6 +1598,16 @@ void mdn_session::build_logup_aux(u32 j, const u64* main_cm, const u64* prep_cm,
             }
         } else if (mk::launch_logup_rows(la, stream) != 0) fail(MDN_ERR_UNSUPPORTED, "lookup program too large for the interpreter");
         mk::launch_ef_exclusive_scan(totals.p, N, aux_cm, aux_cm + N, fin.p, scratch.p, stream);
+        if (h.n_regs && registers) {   // a version-2 program's register columns, after the LogUp columns
+            DevBuf reg_scratch;
+            reg_scratch.alloc(mk::register_scratch_words(ln, h.n_regs), stream);
+            mk::RegisterArgs ra{};
+            ra.main_cm = main_cm; ra.prep_cm = prep_cm; ra.log_n = ln; ra.n_regs = h.n_regs; ra.col0 = h.lookup_cols; ra.prog = h.reg_dev;
+            ra.publics = d_publics.p; ra.challenges = d_randomness.p; ra.aux_cm = aux_cm; ra.scratch = reg_scratch.p; ra.bad_flag = (u32*)d_flag.p;
+            const int rc = mk::launch_register_columns(ra, stream);
+            if (rc < 0) fail(MDN_ERR_UNSUPPORTED, "register program too large for the interpreter");
+            if (rc > 0) fail(MDN_ERR_CUDA, "AIR %u: register column kernels: %s", order[j], cudaGetErrorString((cudaError_t)rc));
+        }
     }
     CUDA_OK(cudaMemcpyAsync(final_out, fin.p, 2 * sizeof(u64), cudaMemcpyDeviceToHost, stream));
     u32 flag = 0;
@@ -2017,7 +2160,7 @@ void mdn_session::check_trace_balance(const mdn_statement* st, const mdn_matrix*
     for (u32 i = 0; i < k; i++) {
         const uint32_t* ann = mutex_sites ? mutex_sites[i] : nullptr;
         if (!lookup_air(i, ann ? "mutex sites" : nullptr, skipped)) continue;
-        const LookupItems items(*st->airs[i].lookup);
+        const LookupItems items(airs[i].lookup_v1);
         if (items.n >= (1u << 24)) fail(MDN_ERR_UNSUPPORTED, "AIR %u: at most 2^24 - 1 lookup interactions", i);
         if (!ann) continue;
         std::vector<u32> ids;
@@ -2069,7 +2212,7 @@ void mdn_session::check_trace_balance(const mdn_statement* st, const mdn_matrix*
         b = mk::BalanceArgs{};
         b.main_cm = main_cm[i]; b.prep_cm = airs[i].lookup_prep ? bundle_prep_rows(i) : nullptr; b.log_n = log_heights[i]; b.prog = airs[i].lookup_dev;
         b.publics = d_publics.p; b.challenges = d_randomness.p; b.instance = i;
-        const u32 nc = LookupItems(*st->airs[i].lookup).n, na = (u32)mx[i].group.size();
+        const u32 nc = LookupItems(airs[i].lookup_v1).n, na = (u32)mx[i].group.size();
         if (na) {
             const u32* w = (const u32*)d_mx[i].p;
             b.mutex_pos = w; b.mutex_group = w + nc; b.mutex_site = w + nc + na; b.n_mutex = na;
@@ -2161,7 +2304,7 @@ void mdn_session::check_trace_balance(const mdn_statement* st, const mdn_matrix*
             u32 inst = (u32)(r.key >> 48), q = (u32)(r.key & 0xFFFFFFu);
             p.multiplicity = r.m; p.interaction = q;
             if (inst == mk::BALANCE_BOUNDARY) { p.instance = 0xFFFFFFFFu; p.row = ~0ull; p.column = 0xFFFFFFFFu; }
-            else { p.instance = inst; p.row = (r.key >> 24) & 0xFFFFFFu; p.column = LookupItems(*st->airs[inst].lookup).column(q); }
+            else { p.instance = inst; p.row = (r.key >> 24) & 0xFFFFFFu; p.column = LookupItems(airs[inst].lookup_v1).column(q); }
             bal_contrib.push_back(p);
         }
     }
@@ -2209,9 +2352,10 @@ void mdn_session::prepare_folds(const mdn_statement* st, const mdn_matrix* trace
     for (u32 i = 0; i < k; i++) {
         const uint32_t* marks = fold_marks ? fold_marks[i] : nullptr;
         if (!lookup_air(i, marks ? "fold marks" : folds_out && folds_out[i] ? "a fold buffer" : nullptr, skipped)) continue;
-        const u32 C = airs[i].desc.aux_width;
+        const u32 C = airs[i].lookup_cols;   // the folds cover the LogUp columns; an aux trace has every aux column
         if (aux) {
-            if (aux[i].width != 2 * C || aux[i].log_height != log_heights[i]) fail(MDN_ERR_INVALID_ARG, "AIR %u: the aux trace must be 2^%u rows of %u base columns", i, log_heights[i], 2 * C);
+            const u32 aw = airs[i].desc.aux_width;
+            if (aux[i].width != 2 * aw || aux[i].log_height != log_heights[i]) fail(MDN_ERR_INVALID_ARG, "AIR %u: the aux trace must be 2^%u rows of %u base columns", i, log_heights[i], 2 * aw);
             if (!aux[i].values) fail(MDN_ERR_INVALID_ARG, "aux trace %u is NULL", i);
             if (cm) check_column_major(aux[i], "aux trace", i);
             if (!aux_finals || !aux_finals[i]) fail(MDN_ERR_INVALID_ARG, "AIR %u: aux_finals is NULL", i);
@@ -2222,7 +2366,7 @@ void mdn_session::prepare_folds(const mdn_statement* st, const mdn_matrix* trace
             if (!on_device) staging_words = std::max(staging_words, ((size_t)4 * C) << log_heights[i]);
         }
         if (!marks) continue;
-        const LookupItems items(*st->airs[i].lookup);
+        const LookupItems items(airs[i].lookup_v1);
         for (u32 q = 0; q < items.n; q++) {
             const u32 m = marks[q];
             if (m != 0 && m != 1 && m != 3) fail(MDN_ERR_INVALID_ARG, "AIR %u: fold mark %u of interaction %u (0, 1 or 3)", i, m, q);
@@ -2259,7 +2403,7 @@ void mdn_session::prepare_folds(const mdn_statement* st, const mdn_matrix* trace
     d_marks.resize(k);
     for (u32 i = 0; i < k; i++) {
         if (!airs[i].has_lookup || !fold_marks || !fold_marks[i]) continue;
-        const u32 nc = LookupItems(*st->airs[i].lookup).n;
+        const u32 nc = LookupItems(airs[i].lookup_v1).n;
         if (!nc) continue;
         d_marks[i].alloc(((size_t)nc + 1) / 2, stream);
         CUDA_OK(cudaMemcpyAsync(d_marks[i].p, fold_marks[i], nc * sizeof(u32), cudaMemcpyHostToDevice, stream));
@@ -2273,7 +2417,7 @@ void mdn_session::prepare_folds(const mdn_statement* st, const mdn_matrix* trace
         if (!airs[i].has_lookup) continue;
         if (aux) { finals[i] = gl::e2(aux_finals[i][0], aux_finals[i][1]); continue; }
         u64 fin[2] = {0, 0};
-        build_logup_aux(pos[i], fs.main_cm[i], airs[i].raw_prep.p, aux_cm[i], fin);
+        build_logup_aux(pos[i], fs.main_cm[i], airs[i].raw_prep.p, aux_cm[i], fin, false);
         finals[i] = gl::e2(fin[0], fin[1]);
     }
 }
@@ -2360,7 +2504,7 @@ void mdn_session::lookup_fold_census(const mdn_statement* st, const mdn_matrix* 
     for (u32 i = 0; i < k; i++) {
         const bool lk = airs[i].has_lookup;
         row_base[i + 1] = row_base[i] + (lk ? (size_t)1 << log_heights[i] : 0);
-        tally_base[i + 1] = tally_base[i] + (lk ? 4 * (size_t)airs[i].desc.aux_width : 0);
+        tally_base[i + 1] = tally_base[i] + (lk ? 4 * (size_t)airs[i].lookup_cols : 0);
     }
     const size_t rows = row_base[k];
     DevBuf counts, offsets, tally, words, scratch;
@@ -2400,7 +2544,7 @@ void mdn_session::lookup_fold_census(const mdn_statement* st, const mdn_matrix* 
     u64 zero_u = 0;
     for (u32 i = 0; i < k; i++) {
         if (!airs[i].has_lookup) continue;
-        for (u32 c = 0; c < airs[i].desc.aux_width; c++) {
+        for (u32 c = 0; c < airs[i].lookup_cols; c++) {
             const u64* t = host_tally.data() + tally_base[i] + 4 * (size_t)c;
             if (!t[0]) continue;
             mdn_fold_tally ft{};
@@ -2444,7 +2588,7 @@ void mdn_session::lookup_fold_census(const mdn_statement* st, const mdn_matrix* 
         for (u32 i = 0; i < k; i++) {
             if (!airs[i].has_lookup) continue;
             bool any = false;
-            for (u32 c = 0; c < airs[i].desc.aux_width && !any; c++) any = host_tally[tally_base[i] + 4 * (size_t)c] != 0;
+            for (u32 c = 0; c < airs[i].lookup_cols && !any; c++) any = host_tally[tally_base[i] + 4 * (size_t)c] != 0;
             if (!any) continue;
             mk::FoldCensusArgs f = fa[i];
             f.max_failures = out->n_failures; f.failures = d_failures.p;
@@ -2539,7 +2683,7 @@ void mdn_session::commit_aux(const mdn_matrix* aux, const u64* const* aux_values
         CommittedMat& m = aux_c.mats[j];
         u64 logup_final[2] = {0, 0};
         const bool dev_aux = airs[inst].has_lookup;
-        if (dev_aux) build_logup_aux(j, airs[inst].raw_main_cm, airs[inst].lookup_prep ? bundle_prep_rows(inst) : nullptr, m.coef, logup_final);
+        if (dev_aux) build_logup_aux(j, airs[inst].raw_main_cm, airs[inst].lookup_prep || airs[inst].reg_prep ? bundle_prep_rows(inst) : nullptr, m.coef, logup_final);
         else if (w) {
             if (zero_aux) CUDA_OK(cudaMemsetAsync(m.coef, 0, ((size_t)1 << m.log_n) * w * sizeof(u64), stream));
             else {
@@ -3586,6 +3730,19 @@ int mdn_session_set_jit(mdn_session* s, uint32_t min_nodes) {
 long long mdn_jit_compile_check(const uint32_t* program, uint32_t program_words, const char** err) {
     static thread_local std::string msg;
     try {
+        std::vector<u32> v1;
+        if (program && program_words >= 6 && program[0] == 0x504B4C4Du && program[1] == 2) {
+            // a version-2 lookup program: its interaction part, split with every range the program itself can satisfy
+            const u32 nn = program[2], nc = program[3], nr = program[5];
+            u32 n_cols = 1;
+            for (u32 q = 0; q < nc && (size_t)6 + 3 * (size_t)nn + 4 * (size_t)q < program_words; q++) n_cols = std::max(n_cols, program[6 + 3 * (size_t)nn + 4 * (size_t)q] + 1);
+            mdn_air a{};
+            a.width = a.num_randomness = a.num_periodic_columns = a.preprocessed_width = ~0u;
+            a.aux_width = n_cols + nr; a.num_aux_values = 1;
+            try { v1 = split_lookup_v2(0, a, ~0u, mdn_lookup{n_cols, program_words, program}).v1; }
+            catch (const MdnError& e) { msg = e.what(); if (err) *err = msg.c_str(); return MDN_ERR_INVALID_ARG; }
+            program = v1.data(); program_words = (u32)v1.size();
+        }
         const bool lookup = program && program_words >= 5 && program[0] == 0x504B4C4Du;
         if (!program || program_words < 5 || (program[0] != 0x5249414Du && !lookup) || program[1] != 1 ||
             (size_t)program_words != 5 + 3 * (size_t)program[2] + (lookup ? 4 : 1) * (size_t)program[3] + 2 * (size_t)program[4]) { msg = "bad program"; if (err) *err = msg.c_str(); return MDN_ERR_INVALID_ARG; }
