@@ -471,7 +471,12 @@ int mdn_constraint_census(mdn_session* s, const mdn_statement* st, const mdn_mat
  * mdn_prove_begin and mdn_prove_finish (MDN_ERR_INVALID_ARG) and a session split over ranks (MDN_ERR_UNSUPPORTED).
  * Malformed or non-canonical randomness, boundary triples or annotations: MDN_ERR_INVALID_ARG; a table larger than the
  * free device memory: MDN_ERR_UNSUPPORTED.  The report's memory is owned by the session and valid until the next call
- * on it.  Nothing mdn_get_info / mdn_get_timings report about the last proof changes, and later proofs are unchanged. */
+ * on it.  Nothing mdn_get_info / mdn_get_timings report about the last proof changes, and later proofs are unchanged.
+ * The three row passes (count, insert, collect) of a lookup program at or above the mdn_session_set_jit threshold run
+ * on the NVRTC kernel k_jit_balance; on its first use in a session the interpreter repeats every pass into a second
+ * table and lists of its own, which must agree (when that table does not fit in free device memory the call runs the
+ * interpreter and the kernel stays unchecked).  MDN_INFO_JIT_LOOKUP_CHECK says which AIRs used it; the same holds for
+ * mdn_check_lookup_folds (k_jit_fold) and mdn_lookup_fold_census (k_jit_fold_census). */
 typedef struct {
     uint64_t denom[2];               /* encoded denominator (c0, c1) */
     uint64_t net_multiplicity;       /* sum of its multiplicities mod p, non-zero */
@@ -603,7 +608,10 @@ int mdn_check_lookup_folds(mdn_session* s, const mdn_statement* st, const mdn_ma
  * whose device staging is larger than the free device memory MDN_ERR_UNSUPPORTED.  The outputs do not depend on the
  * order in which device atomics ran: two calls on the same inputs give byte-identical outputs.  Refused, as
  * mdn_check_lookup_folds, inside a staged proof and on a session split over ranks; uses and releases the proof arena;
- * leaves mdn_get_info, mdn_get_timings and later proofs unchanged.  Interpreted whatever the program's size. */
+ * leaves mdn_get_info (but for MDN_INFO_JIT_LOOKUP_CHECK), mdn_get_timings and later proofs unchanged.  The per-row count
+ * and tally pass runs on the NVRTC kernel k_jit_fold_census for lookup programs at or above the mdn_session_set_jit
+ * threshold (self-checked against k_fold_census_rows on its first use); the failure listing and its probes stay on the
+ * interpreter. */
 typedef struct {                 /* one (instance, row, column) where the aux trace departs from the fold */
     uint32_t instance, column;
     uint32_t kind;               /* 1, 2 or 3 exactly as mdn_fold_report.kind */
@@ -675,6 +683,7 @@ typedef enum {
     MDN_INFO_POOL = 9,             /* cudaMallocAsync pool reserved now / high, used now / high (bytes); proof arena capacity (bytes), slabs, driver allocations so far, live blocks */
     MDN_INFO_BUILD = 10,           /* { generation of the field arithmetic, generation of the NTT kernels }: always { 2, 2 } (poseidon2_fast2.cuh, ntt2.cuh) */
     MDN_INFO_JIT_CHECK = 11,       /* per AIR (instance order) of the last mdn_check_constraints / mdn_constraint_census call or constraint-guard run: 1 = NVRTC row kernel, 0 = interpreter */
+    MDN_INFO_JIT_LOOKUP_CHECK = 12, /* per AIR (instance order) of the last mdn_check_trace_balance / mdn_check_lookup_folds / mdn_lookup_fold_census call: 1 = NVRTC row kernel, 0 = interpreter (also for an AIR without mdn_air.lookup) */
 } mdn_info;
 /* QUOTIENT_ACC / DEEP_EVALS are only recorded (extra device->host copies) after mdn_set_debug(s, 1). */
 int mdn_set_debug(mdn_session* s, int enable);
@@ -687,11 +696,13 @@ size_t mdn_abi_layout(uint32_t* out, size_t cap);
  * AIR programs with at least `min_nodes` nodes (default 256; 0 = never) are lowered to straight-line CUDA,
  * compiled once per program with NVRTC for sm_90a and cached; smaller ones (and all of them when libnvrtc
  * is absent) run on the op-list interpreter.  Both produce identical values.  Specialised: the proof's constraint
- * evaluation and LogUp row build (MDN_INFO_JIT), and the row pass of mdn_check_constraints, mdn_constraint_census and
- * the constraint guard (MDN_INFO_JIT_CHECK).  Interpreted whatever the size: the lookup checks
- * (mdn_check_trace_balance, mdn_check_lookup_folds, mdn_lookup_fold_census), the census's failure listing and the checks'
- * one-row probes.
- * Each compiled kernel is compared word for word with the interpreter on its first use in a session. */
+ * evaluation and LogUp row build (MDN_INFO_JIT), the row pass of mdn_check_constraints, mdn_constraint_census and
+ * the constraint guard (MDN_INFO_JIT_CHECK), and the row passes of the lookup checks mdn_check_trace_balance,
+ * mdn_check_lookup_folds and mdn_lookup_fold_census (MDN_INFO_JIT_LOOKUP_CHECK; the lookup program's node count decides,
+ * and only these three calls compile or load its kernels).  Interpreted whatever the size: the censuses' failure
+ * listings, the checks' one-row probes and the register program of a version-2 lookup program.
+ * Each compiled kernel is compared with the interpreter on its first use in a session: word for word, and for the
+ * balance table slot by slot (slot placement follows the order of the atomics). */
 int mdn_session_set_jit(mdn_session* s, uint32_t min_nodes);
 /* "nvrtc <version>" or why it is unavailable, plus the reason the last JIT attempt was dropped (compile error,
  * or the first-use comparison against the interpreter failed -- the interpreter's result is then kept). */

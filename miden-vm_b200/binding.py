@@ -42,6 +42,9 @@ class HashChallenger(C.Structure):
 
 
 HASH_POSEIDON2, HASH_BLAKE3, HASH_KECCAK, HASH_RPO, HASH_RPX = 0, 1, 2, 3, 4
+# Session.info(INFO_JIT_LOOKUP_CHECK): per AIR (instance order) of the last check_trace_balance / check_lookup_folds /
+# lookup_fold_census call, 1 where the row passes ran on the NVRTC kernel, 0 on the interpreter (mdn_get_info 12)
+INFO_JIT_LOOKUP_CHECK = 12
 
 
 class Matrix(C.Structure):

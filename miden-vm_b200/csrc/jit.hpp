@@ -9,7 +9,8 @@
 // cubin through the driver API.  Field arithmetic is exact, so the result is bit-identical to the interpreter
 // (asserted in tests/test_gpu_parity.py).  libnvrtc / libcuda are dlopen'ed on first use; when NVRTC is
 // missing the session keeps using the interpreter and says so in mdn_get_info(MDN_INFO_JIT).  The same lowering also
-// gives the LogUp row kernel (MODE_LOOKUP) and the trace-check row kernels (MODE_CHECK, MDN_INFO_JIT_CHECK).
+// gives the LogUp row kernel (MODE_LOOKUP), the trace-check row kernels (MODE_CHECK, MDN_INFO_JIT_CHECK) and the
+// lookup-check row kernels (MODE_LOOKUP_CHECK, MDN_INFO_JIT_LOOKUP_CHECK).
 #pragma once
 #include <cuda_runtime.h>
 #include <dlfcn.h>
@@ -62,8 +63,30 @@ struct CheckJitArgs {
 // per-block shared tallies of k_jit_census up to this many constraints (kernels.cuh CENSUS_SHARED_K)
 static constexpr uint32_t CENSUS_SHARED_K = 256;
 
-// what generate() emits: the proof's constraint kernel, the LogUp row kernel, or the two trace-check kernels
-enum Mode : uint32_t { MODE_CONSTRAINTS = 0, MODE_LOOKUP = 1, MODE_CHECK = 2 };
+// Arguments of the generated lookup-check kernels k_jit_balance / k_jit_fold / k_jit_fold_census (the semantics of
+// k_balance_rows / k_fold_rows / k_fold_census_rows, kernels.cuh BalanceArgs / LookupFoldArgs / FoldCensusArgs); one
+// struct for the three, each reading its own members.  Layout must equal `struct LookupCheckJitArgs` in
+// PRELUDE_LOOKUP_CHECK below.
+struct LookupCheckJitArgs {
+    const uint64_t* main_lde; const uint64_t* prep_lde;   // raw column-major traces (L = N); prep: NULL when unread
+    const uint64_t* publics; const uint64_t* challenges; const uint64_t* periodic;   // periodic: raw row-major matrix
+    // k_jit_balance: mutex annotation, the table (BalanceTable), counters and lists
+    const uint32_t* mutex_pos; const uint32_t* mutex_group; const uint32_t* mutex_site;
+    uint64_t* t_keys; uint64_t* t_sums; unsigned long long* t_count; unsigned long long* t_first;
+    unsigned long long* counters; uint64_t* mutex_out; uint64_t* contrib_out;
+    // k_jit_fold / k_jit_fold_census
+    const uint32_t* marks; const uint64_t* aux_cm; uint64_t* folds_out;
+    unsigned long long* first; unsigned long long* failing_rows; unsigned long long* zero_u;
+    uint32_t* row_count; unsigned long long* tally;
+    uint64_t t_mask, final_a, final_b, row0, n_rows;   // k_jit_fold: rows [row0, row0 + n_rows)
+    uint32_t log_n, n_periodic, log_max_period, n_cols, instance, mode, n_mutex, folds_cm;
+};
+// activity words of the mutex sites per row (kernels.cuh BALANCE_MUTEX_MAX / 64)
+static constexpr uint32_t LOOKUP_CHECK_MUTEX_WORDS = 16;
+
+// what generate() emits: the proof's constraint kernel, the LogUp row kernel, the two trace-check kernels, or the three
+// lookup-check kernels
+enum Mode : uint32_t { MODE_CONSTRAINTS = 0, MODE_LOOKUP = 1, MODE_CHECK = 2, MODE_LOOKUP_CHECK = 3 };
 
 static const char PRELUDE[] = R"CUDA(
 typedef unsigned long long u64;
@@ -164,6 +187,235 @@ __device__ __noinline__ void tally(const CheckJitArgs& a, u32* sh, u32 r, u32 k)
     }
 }
 )CUDA";
+// lookup-check mode only, after `#define LK_NC <columns>` and `#define LK_MUTEX_WORDS <words>`: the argument struct, the
+// per-row state every chunk carries by reference, the balance table of kernels.cu (the same hash, probe order and
+// atomics; the 128-bit compare-and-swap in PTX, which every NVRTC that targets sm_90 accepts), the fold steps of
+// fold_walk / fold_divide / fold_verdict in the same operation order, and lk_hook, which the chunks call once per
+// interaction in interaction order.  Field results are exact, so every word equals the interpreter's.
+static const char PRELUDE_LOOKUP_CHECK[] = R"CUDA(struct LookupCheckJitArgs {
+    const u64* main_lde; const u64* prep_lde;
+    const u64* publics; const u64* challenges; const u64* periodic;
+    const u32* mutex_pos; const u32* mutex_group; const u32* mutex_site;
+    u64* t_keys; u64* t_sums; unsigned long long* t_count; unsigned long long* t_first;
+    unsigned long long* counters; u64* mutex_out; u64* contrib_out;
+    const u32* marks; const u64* aux_cm; u64* folds_out;
+    unsigned long long* first; unsigned long long* failing_rows; unsigned long long* zero_u;
+    u32* row_count; unsigned long long* tally;
+    u64 t_mask, final_a, final_b, row0, n_rows;
+    u32 log_n, n_periodic, log_max_period, n_cols, instance, mode, n_mutex, folds_cm;
+};
+// mode 0 / 1 / 2: the balance pass of that mode; 3: the fold
+struct LkRow {
+    E2 V[LK_NC], U[LK_NC];                 // the columns' folds
+    E2 bn, bd, vg, ug; u64 bf; u32 cur;    // the open batch (N, D) and its flag, the open group (V_g, U_g) and its column
+    u32 mode;
+    u64 act[LK_MUTEX_WORDS];               // activity of the annotated interactions (bit mutex_pos[k])
+    unsigned long long pushes;
+};
+template <class T> __device__ __forceinline__ T census_max(T* p, T v) { return atomicMax(p, v); }
+struct alignas(16) K2 { u64 x, y; };
+__device__ __forceinline__ u64 balance_hash(u64 c0, u64 c1) {
+    u64 h = c0 * 0x9E3779B97F4A7C15ull ^ (c1 + 0x632BE59BD9B4E019ull) * 0xC2B2AE3D27D4EB4Full;
+    return h ^ (h >> 29) ^ (h >> 47);
+}
+__device__ __forceinline__ u64 balance_key(u32 inst, u64 row, u32 k) { return ((u64)inst << 48) | (row << 24) | k; }
+__device__ __forceinline__ K2 cas128(u64* p, u64 c0, u64 c1, u64 n0, u64 n1) {
+    K2 o;
+    asm volatile("{\n\t.reg .b128 d, b, c;\n\tmov.b128 b, {%2, %3};\n\tmov.b128 c, {%4, %5};\n\t"
+                 "atom.global.cas.b128 d, [%6], b, c;\n\tmov.b128 {%0, %1}, d;\n\t}"
+                 : "=l"(o.x), "=l"(o.y) : "l"(c0), "l"(c1), "l"(n0), "l"(n1), "l"(p) : "memory");
+    return o;
+}
+__device__ __forceinline__ u64 balance_insert(const LookupCheckJitArgs& a, u64 c0, u64 c1) {
+    K2* keys = reinterpret_cast<K2*>(a.t_keys);
+    for (u64 s = balance_hash(c0, c1) & a.t_mask;; s = (s + 1) & a.t_mask) {
+        K2 cur = keys[s];
+        if (cur.x == c0 && cur.y == c1) return s;
+        if (cur.x != ~0ull && cur.y != ~0ull) continue;
+        K2 old = cas128(a.t_keys + 2 * s, ~0ull, ~0ull, c0, c1);
+        if ((old.x == ~0ull && old.y == ~0ull) || (old.x == c0 && old.y == c1)) return s;
+    }
+}
+__device__ __forceinline__ u64 balance_find(const LookupCheckJitArgs& a, u64 c0, u64 c1) {
+    const K2* keys = reinterpret_cast<const K2*>(a.t_keys);
+    u64 s = balance_hash(c0, c1) & a.t_mask;
+    for (;; s = (s + 1) & a.t_mask) { K2 cur = keys[s]; if (cur.x == c0 && cur.y == c1) return s; }
+}
+__device__ __forceinline__ void balance_add(const LookupCheckJitArgs& a, u64 s, u64 m, u64 key) {
+    unsigned long long* sum = reinterpret_cast<unsigned long long*>(a.t_sums) + 2 * s;
+    unsigned long long old = atomicAdd(sum, (unsigned long long)m);
+    if (old + m < old) atomicAdd(sum + 1, 1ull);
+    atomicAdd(a.t_count + s, 1ull);
+    atomicMin(a.t_first + s, (unsigned long long)key);
+}
+__device__ __forceinline__ void lk_close_batch(LkRow& st) {
+    st.ug = eadd(st.ug, emulf(esub(st.bd, mk(1ull, 0ull)), st.bf));
+    st.vg = eadd(st.vg, emulf(st.bn, st.bf));
+    st.bn = mk(0ull, 0ull); st.bd = mk(1ull, 0ull);
+}
+__device__ __forceinline__ void lk_close_group(LkRow& st) {
+    st.V[st.cur] = eadd(emul(st.V[st.cur], st.ug), emul(st.vg, st.U[st.cur]));
+    st.U[st.cur] = emul(st.U[st.cur], st.ug);
+    st.vg = mk(0ull, 0ull); st.ug = mk(1ull, 0ull);
+}
+// interaction k of column col at row r, its flag (1 when it has none), multiplicity and denominator
+__device__ __noinline__ void lk_hook(const LookupCheckJitArgs& a, size_t r, LkRow& st, u32 k, u32 col, u64 flag, u64 m, E2 d) {
+    if (st.mode == 3) {   // fold_walk: every interaction takes part whatever its flag
+        const u32 mark = a.marks ? a.marks[k] : 3u;
+        if (mark & 1) lk_close_batch(st);
+        if (mark & 2) { lk_close_group(st); st.cur = col; }
+        if (mark & 1) st.bf = flag;
+        st.bn = eadd(emul(st.bn, d), emulf(st.bd, m));
+        st.bd = emul(st.bd, d);
+        return;
+    }
+    if (flag == 0ull) return;   // a zero flag skips the push
+    if (a.n_mutex) { const u32 b = a.mutex_pos[k]; if (b != 0xFFFFFFFFu) st.act[b >> 6] |= 1ull << (b & 63); }
+    if (st.mode == 0) { st.pushes++; return; }
+    const u64 key = balance_key(a.instance, r, k);   // a zero denominator is an ordinary key
+    if (st.mode == 1) { balance_add(a, balance_insert(a, d.a, d.b), m, key); return; }
+    const u64 s = balance_find(a, d.a, d.b);
+    if (a.t_sums[2 * s + 1]) {
+        const unsigned long long p = atomicAdd(a.counters + 2, 1ull);
+        a.contrib_out[3 * p] = s; a.contrib_out[3 * p + 1] = key; a.contrib_out[3 * p + 2] = m;
+    }
+}
+__device__ __forceinline__ void lk_fold_init(LkRow& st) {
+    for (u32 c = 0; c < LK_NC; c++) { st.V[c] = mk(0ull, 0ull); st.U[c] = mk(1ull, 0ull); }
+    st.bn = st.vg = mk(0ull, 0ull); st.bd = st.ug = mk(1ull, 0ull); st.bf = 0; st.cur = 0; st.mode = 3;
+}
+// fold_divide: F[c] = V_c / U_c with one inversion, F[c] = 0 where U_c is zero; the mask of those columns
+__device__ __forceinline__ u32 lk_fold_divide(const LkRow& st, E2* F, E2& total) {
+    u32 zero_mask = 0;
+    E2 acc = mk(1ull, 0ull);
+    for (u32 c = 0; c < LK_NC; c++) {
+        F[c] = acc;
+        if ((st.U[c].a | st.U[c].b) == 0ull) zero_mask |= 1u << c; else acc = emul(acc, st.U[c]);
+    }
+    E2 inv = einv(acc);
+    total = mk(0ull, 0ull);
+    for (u32 c = LK_NC; c-- > 0;) {
+        if ((zero_mask >> c) & 1) { F[c] = mk(0ull, 0ull); continue; }
+        F[c] = emul(st.V[c], emul(inv, F[c]));
+        inv = emul(inv, st.U[c]);
+        total = eadd(total, F[c]);
+    }
+    return zero_mask;
+}
+// fold_verdict: 0 agrees, 1 fraction column, 2 accumulator, 3 zero U
+__device__ __forceinline__ u32 lk_fold_verdict(const LookupCheckJitArgs& a, size_t N, size_t r, u32 c, const E2* F, E2 total, u32 zero_mask) {
+    E2 expected = F[c], actual = mk(a.aux_cm[(size_t)(2 * c) * N + r], a.aux_cm[(size_t)(2 * c + 1) * N + r]);
+    if (c == 0) {
+        E2 next = r == N - 1 ? mk(a.final_a, a.final_b) : mk(a.aux_cm[r + 1], a.aux_cm[N + r + 1]);
+        expected = total; actual = esub(next, actual);
+    }
+    const bool eq = expected.a == actual.a && expected.b == actual.b;
+    if ((zero_mask >> c) & 1) return 3;
+    if (c == 0 ? (zero_mask == 0 && !eq) : !eq) return c ? 1 : 2;
+    return 0;
+}
+)CUDA";
+// lookup-check mode: the three entry points, after lk_row (the chunks on one row)
+static const char LOOKUP_CHECK_ENTRIES[] = R"CUDA(// k_balance_rows: the pushes of row r by mode, then the row's mutex groups in (column, group) order
+extern "C" __global__ void __launch_bounds__(128) k_jit_balance(const KArgs a) {
+  const size_t N = (size_t)1 << a.log_n, r = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= N) return;
+  LkRow st;
+  st.mode = a.mode; st.pushes = 0;
+  for (u32 w = 0; w < (a.n_mutex + 63) / 64; w++) st.act[w] = 0;
+  lk_row(a, r, st);
+  if (st.pushes) atomicAdd(a.counters, st.pushes);
+  if (!a.n_mutex || a.mode == 2) return;
+  u32 cur_g = a.mutex_group[0], cur_s = a.mutex_site[0], cnt = 0;
+  bool counted = false;
+  for (u32 b = 0;; b++) {
+    const bool end = b == a.n_mutex;
+    u32 g = end ? 0xFFFFFFFFu : a.mutex_group[b], s = end ? 0xFFFFFFFFu : a.mutex_site[b];
+    if (end || g != cur_g) {
+      if (cnt > 1) {
+        unsigned long long p = atomicAdd(a.counters + 1, 1ull);
+        if (a.mode == 1) {
+          a.mutex_out[3 * p] = ((u64)a.instance << 32) | r;
+          a.mutex_out[3 * p + 1] = ((u64)(cur_g >> 16) << 32) | (cur_g & 0xffffu);
+          a.mutex_out[3 * p + 2] = cnt;
+        }
+      }
+      if (end) break;
+      cur_g = g; cur_s = s; cnt = 0; counted = false;
+    } else if (s != cur_s) { cur_s = s; counted = false; }
+    if (!counted && ((st.act[b >> 6] >> (b & 63)) & 1)) { cnt++; counted = true; }
+  }
+}
+// k_fold_rows on rows [row0, row0 + n_rows)
+extern "C" __global__ void __launch_bounds__(128) k_jit_fold(const KArgs a) {
+  const size_t N = (size_t)1 << a.log_n, r = a.row0 + (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= a.row0 + a.n_rows) return;
+  LkRow st;
+  lk_fold_init(st);
+  lk_row(a, r, st);
+  lk_close_batch(st); lk_close_group(st);
+  if (a.folds_out && a.folds_cm) {
+    for (u32 c = 0; c < LK_NC; c++) {
+      u64* o = a.folds_out + (size_t)(4 * c) * N + r;
+      o[0] = st.V[c].a; o[N] = st.V[c].b; o[2 * N] = st.U[c].a; o[3 * N] = st.U[c].b;
+    }
+  } else if (a.folds_out) {
+    K2* o = reinterpret_cast<K2*>(a.folds_out) + 2 * r * LK_NC;
+    for (u32 c = 0; c < LK_NC; c++) { o[2 * c].x = st.V[c].a; o[2 * c].y = st.V[c].b; o[2 * c + 1].x = st.U[c].a; o[2 * c + 1].y = st.U[c].b; }
+  }
+  E2 F[LK_NC], total;
+  const u32 zero_mask = lk_fold_divide(st, F, total);
+  u32 first_c = 0xFFFFFFFFu, n_zero = 0;
+  for (u32 c = 0; c < LK_NC; c++) {
+    const u32 kind = lk_fold_verdict(a, N, r, c, F, total, zero_mask);
+    n_zero += kind == 3;
+    if (kind && first_c == 0xFFFFFFFFu) first_c = c;
+  }
+  if (first_c != 0xFFFFFFFFu) {
+    atomicMin(a.first, (unsigned long long)(((u64)r << 32) | first_c));
+    atomicAdd(a.failing_rows, 1ull);
+  }
+  if (n_zero) atomicAdd(a.zero_u, (unsigned long long)n_zero);
+}
+// k_fold_census_rows: every row's count of disagreeing columns; per column the block's tallies in shared memory, one
+// global atomic of each kind per (block, disagreeing column)
+extern "C" __global__ void __launch_bounds__(128) k_jit_fold_census(const KArgs a) {
+  __shared__ u32 s_cnt[LK_NC], s_zero[LK_NC], s_min[LK_NC], s_max[LK_NC];
+  __shared__ u32 s_rows;
+  for (u32 c = threadIdx.x; c < LK_NC; c += blockDim.x) { s_cnt[c] = 0; s_zero[c] = 0; s_min[c] = 0xFFFFFFFFu; s_max[c] = 0; }
+  if (threadIdx.x == 0) s_rows = 0;
+  __syncthreads();
+  const size_t N = (size_t)1 << a.log_n, r = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (r < N) {
+    LkRow st;
+    lk_fold_init(st);
+    lk_row(a, r, st);
+    lk_close_batch(st); lk_close_group(st);
+    E2 F[LK_NC], total;
+    const u32 zero_mask = lk_fold_divide(st, F, total);
+    u32 n_fail = 0;
+    for (u32 c = 0; c < LK_NC; c++) {
+      const u32 kind = lk_fold_verdict(a, N, r, c, F, total, zero_mask);
+      if (!kind) continue;
+      n_fail++;
+      atomicAdd(&s_cnt[c], 1u);
+      if (kind == 3) atomicAdd(&s_zero[c], 1u);
+      atomicMin(&s_min[c], (u32)r); census_max(&s_max[c], (u32)r);
+    }
+    a.row_count[r] = n_fail;
+    if (n_fail) atomicAdd(&s_rows, 1u);
+  }
+  __syncthreads();
+  for (u32 c = threadIdx.x; c < LK_NC; c += blockDim.x) {
+    if (!s_cnt[c]) continue;
+    atomicAdd(&a.tally[4 * c], (unsigned long long)s_cnt[c]);
+    if (s_zero[c]) atomicAdd(&a.tally[4 * c + 1], (unsigned long long)s_zero[c]);
+    atomicMin(&a.tally[4 * c + 2], (unsigned long long)s_min[c]);
+    census_max(&a.tally[4 * c + 3], (unsigned long long)s_max[c]);
+  }
+  if (threadIdx.x == 0 && s_rows) atomicAdd(a.failing_rows, (unsigned long long)s_rows);
+}
+)CUDA";
 
 // ---------------------------------------------------------------------------------------------
 // code generation
@@ -186,15 +438,21 @@ inline uint32_t chunk_nodes() { const char* e = getenv("MDN_JIT_CHUNK"); uint32_
 // tested instead of folded; a chunk returns its failures' count and least constraint index, so the row's result does
 // not depend on the order the chunks visit the constraints in.  Two entry points share the chunks: k_jit_check (the
 // semantics of k_check_rows) and k_jit_census (those of k_census_rows).
+// MODE_LOOKUP_CHECK: `w` is a lowered LookupAir with `n_cols` columns, read on the trace domain as MODE_LOOKUP reads it.
+// Every interaction calls lk_hook (PRELUDE_LOOKUP_CHECK) with its literal index once its operands are defined, in
+// interaction order (an interaction never runs in an earlier chunk than the one before it), with one LkRow of per-row
+// state passed by reference through the chunks.  Three entry points share the chunks: k_jit_balance (the semantics of
+// k_balance_rows, all three modes), k_jit_fold (k_fold_rows) and k_jit_fold_census (k_fold_census_rows).
 inline std::string generate(const uint32_t* w, GenInfo* info, Mode mode = MODE_CONSTRAINTS, uint32_t n_cols = 0) {
-    const bool lookup = mode == MODE_LOOKUP, check = mode == MODE_CHECK;
+    const bool lookup = mode == MODE_LOOKUP, check = mode == MODE_CHECK, lkc = mode == MODE_LOOKUP_CHECK;
+    const bool interactions = lookup || lkc;   // 4-word interaction items instead of constraint node ids
     const uint32_t nn = w[2], nc = w[3];
     const uint32_t* cons = w + 5 + 3 * (size_t)nn;
-    const uint32_t* kw = cons + (lookup ? 4 : 1) * (size_t)nc;
+    const uint32_t* kw = cons + (interactions ? 4 : 1) * (size_t)nc;
     const uint32_t NOFLAG = 0xFFFFFFFFu;
     // operand nodes of item k (constraint: the node itself; interaction: flag?, multiplicity, denominator)
     auto item_ops = [&](uint32_t k, uint32_t out[3]) -> int {
-        if (!lookup) { out[0] = cons[k]; return 1; }
+        if (!interactions) { out[0] = cons[k]; return 1; }
         const uint32_t* it = cons + 4 * (size_t)k;
         int n = 0;
         if (it[1] != NOFLAG) out[n++] = it[1];
@@ -236,6 +494,7 @@ inline std::string generate(const uint32_t* w, GenInfo* info, Mode mode = MODE_C
     for (uint32_t k = 0; k < nc; k++) {
         uint32_t o[3]; int n = item_ops(k, o);
         for (int q = 0; q < n; q++) if (chunk_of[o[q]] != NONE) item_chunk[k] = std::max(item_chunk[k], chunk_of[o[q]]);
+        if (lkc && k) item_chunk[k] = std::max(item_chunk[k], item_chunk[k - 1]);   // the folds walk interactions in order
         for (int q = 0; q < n; q++) if (chunk_of[o[q]] != NONE) last_chunk[o[q]] = std::max(last_chunk[o[q]], item_chunk[k]);
     }
     // slots for values that cross a chunk boundary
@@ -305,12 +564,18 @@ inline std::string generate(const uint32_t* w, GenInfo* info, Mode mode = MODE_C
         s += buf;
         s += PRELUDE_CHECK;
     }
-    s += lookup ? "typedef LookupJitArgs KArgs;\n" : check ? "typedef CheckJitArgs KArgs;\n" : "typedef JitArgs KArgs;\n";
+    if (lkc) {
+        snprintf(buf, sizeof buf, "#define LK_NC %uu\n#define LK_MUTEX_WORDS %uu\n", std::max(1u, n_cols), LOOKUP_CHECK_MUTEX_WORDS);
+        s += buf;
+        s += PRELUDE_LOOKUP_CHECK;
+    }
+    s += lookup ? "typedef LookupJitArgs KArgs;\n" : check ? "typedef CheckJitArgs KArgs;\n" : lkc ? "typedef LookupCheckJitArgs KArgs;\n" : "typedef JitArgs KArgs;\n";
     s += "struct Ctx { size_t L, pos, pn, per_idx, per_stride; u64 is_first, is_last, is_trans; };\n";
     std::vector<uint8_t> seen(nn, 0);
     for (uint32_t c = 0; c < n_chunks; c++) {
         if (lookup) snprintf(buf, sizeof buf, "__device__ __noinline__ void chunk%u(const KArgs& a, const Ctx& c, u64* __restrict__ Sb, E2* __restrict__ Se, E2* __restrict__ V, E2* __restrict__ U) {\n", c);
         else if (check) snprintf(buf, sizeof buf, "__device__ __noinline__ u64 chunk%u(const KArgs& a, const Ctx& c, u64* __restrict__ Sb, E2* __restrict__ Se, u32* sh) {\n", c);
+        else if (lkc) snprintf(buf, sizeof buf, "__device__ __noinline__ void chunk%u(const KArgs& a, const Ctx& c, u64* __restrict__ Sb, E2* __restrict__ Se, LkRow& st) {\n", c);
         else snprintf(buf, sizeof buf, "__device__ __noinline__ void chunk%u(const KArgs& a, const Ctx& c, u64* __restrict__ Sb, E2* __restrict__ Se, E2& acc) {\n", c);
         s += buf;
         s += "  const size_t L = c.L, pos = c.pos, pn = c.pn, per_idx = c.per_idx, per_stride = c.per_stride;\n"
@@ -336,6 +601,15 @@ inline std::string generate(const uint32_t* w, GenInfo* info, Mode mode = MODE_C
                 uint32_t cn = cons[k];
                 std::string nz = ext[cn] ? "(" + nm(cn) + ".a | " + nm(cn) + ".b) != 0ull" : nm(cn) + " != 0ull";
                 snprintf(buf, sizeof buf, "  if (%s) { n++; f = f < %uu ? f : %uu; if (a.tally) tally(a, sh, (u32)pos, %uu); }\n", nz.c_str(), k, k, k);
+                s += buf;
+                continue;
+            }
+            if (lkc) {
+                const uint32_t* it = cons + 4 * (size_t)k;
+                auto base = [&](uint32_t j) { return ext[j] ? nm(j) + ".a" : nm(j); };
+                const std::string den = ext[it[3]] ? nm(it[3]) : "mk(" + nm(it[3]) + ", 0ull)";
+                const std::string flag = it[1] == NOFLAG ? "1ull" : base(it[1]);
+                snprintf(buf, sizeof buf, "  lk_hook(a, pos, st, %uu, %uu, %s, %s, %s);\n", k, it[0], flag.c_str(), base(it[2]).c_str(), den.c_str());
                 s += buf;
                 continue;
             }
@@ -410,6 +684,24 @@ inline std::string generate(const uint32_t* w, GenInfo* info, Mode mode = MODE_C
              "  if (threadIdx.x == 0 && s_rows) atomicAdd(a.failing_rows, (unsigned long long)s_rows);\n"
              "}\n";
         if (info) { info->n_constraints = nc; info->uses_sel = uses_sel; info->n_chunks = n_chunks; info->spill_base = nb; info->spill_ext = ne; }
+        return s;
+    }
+    if (lkc) {
+        // row r of the trace domain, the chunks in order on one LkRow
+        s += "__device__ __forceinline__ void lk_row(const KArgs& a, size_t r, LkRow& st) {\n"
+             "  Ctx c;\n"
+             "  c.L = (size_t)1 << a.log_n;\n"
+             "  c.pos = r;\n"
+             "  c.pn = (r + 1) & (c.L - 1);\n"
+             "  c.per_idx = (r & (((size_t)1 << a.log_max_period) - 1)) * a.n_periodic;\n"
+             "  c.per_stride = 1;\n"
+             "  c.is_first = c.is_last = c.is_trans = 0ull;\n";
+        snprintf(buf, sizeof buf, "  u64 Sb[%u]; E2 Se[%u];\n", std::max(1u, nb), std::max(1u, ne));
+        s += buf;
+        for (uint32_t c = 0; c < n_chunks; c++) { snprintf(buf, sizeof buf, "  chunk%u(a, c, Sb, Se, st);\n", c); s += buf; }
+        s += "}\n";
+        s += LOOKUP_CHECK_ENTRIES;
+        if (info) { info->n_constraints = nc; info->uses_sel = false; info->n_chunks = n_chunks; info->spill_base = nb; info->spill_ext = ne; }
         return s;
     }
     if (lookup) {

@@ -1438,6 +1438,31 @@ void launch_balance_finish(const BalanceTable& t, unsigned long long* counters, 
     k_balance_finish<<<(unsigned)((slots + 255) / 256), 256, 0, st>>>(t, counters, out);
     COUNT_LAUNCH();
 }
+// every occupied slot of `a` looked up in `b` (a bounded probe: the key may be missing there)
+__global__ void __launch_bounds__(256) k_balance_compare(BalanceTable a, BalanceTable b, unsigned long long* words) {
+    size_t s = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (s > a.mask) return;
+    if (b.keys[2 * s] != ~0ull || b.keys[2 * s + 1] != ~0ull) atomicAdd(words + 1, 1ull);
+    u64 c0 = a.keys[2 * s], c1 = a.keys[2 * s + 1];
+    if (c0 == ~0ull && c1 == ~0ull) return;
+    atomicAdd(words, 1ull);
+    u64 q = balance_hash(c0, c1) & b.mask;
+    for (u64 n = 0; n <= b.mask; n++, q = (q + 1) & b.mask) {
+        u64 k0 = b.keys[2 * q], k1 = b.keys[2 * q + 1];
+        if (k0 == c0 && k1 == c1) {
+            if (a.sums[2 * s] != b.sums[2 * q] || a.sums[2 * s + 1] != b.sums[2 * q + 1] || a.count[s] != b.count[q] || a.first[s] != b.first[q])
+                atomicAdd(words + 2, 1ull);
+            return;
+        }
+        if (k0 == ~0ull && k1 == ~0ull) break;
+    }
+    atomicAdd(words + 2, 1ull);
+}
+void launch_balance_compare(const BalanceTable& a, const BalanceTable& b, unsigned long long* words, cudaStream_t st) {
+    size_t slots = (size_t)a.mask + 1;
+    k_balance_compare<<<(unsigned)((slots + 255) / 256), 256, 0, st>>>(a, b, words);
+    COUNT_LAUNCH();
+}
 
 // =============================================================================================
 // LogUp constraint-path folds (debug/trace collect_column_oracle_folds): the lookup program of k_logup_rows folded

@@ -305,6 +305,10 @@ void launch_balance_boundary(const BalanceTable& t, const u64* triples, u32 n, c
 // every occupied slot: counters[3] += 1; the net reduced mod p; an unmatched slot s appends
 // {c0, c1, net, count, first, s} to out (6 u64 each) at counters[4]
 void launch_balance_finish(const BalanceTable& t, unsigned long long* counters, u64* out, cudaStream_t st);
+// first-use check of an NVRTC balance kernel (two tables of the same size, filled with the same pushes in any order):
+// words[0] += occupied slots of a, words[1] += occupied slots of b, words[2] += occupied slots of a whose key is missing
+// from b or whose sum, count or least key differ there; the tables agree when words[0] == words[1] and words[2] == 0
+void launch_balance_compare(const BalanceTable& a, const BalanceTable& b, unsigned long long* words, cudaStream_t st);
 
 // ---------------------------------------------------------------------------------------------
 // LogUp constraint-path folds without proving (mdn_check_lookup_folds; reference air/src/lookup/debug/trace/mod.rs:191-207)

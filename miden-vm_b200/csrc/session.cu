@@ -9,6 +9,7 @@
 #include "kernels.cuh"
 #include "ntt_tables.hpp"
 #include "jit.hpp"
+#include <array>
 #include <cstddef>
 
 #include <cstdarg>
@@ -204,6 +205,9 @@ struct AirHost {
     // the two entry points of the program's trace-check cubin (k_jit_check, k_jit_census), loaded for the checks and
     // for a guarded proof
     std::shared_ptr<jit::Kernel> jit, lookup_jit, check_jit, census_jit;
+    // lkc_balance / lkc_fold / lkc_census: the three entry points of the lookup program's lookup-check cubin
+    // (k_jit_balance, k_jit_fold, k_jit_fold_census), loaded by the lookup checks only (load_lookup_check_jit)
+    std::shared_ptr<jit::Kernel> lkc_balance, lkc_fold, lkc_census;
     u32 n_constraints = 0;
 };
 
@@ -309,6 +313,9 @@ struct mdn_session {
     std::map<u64, std::shared_ptr<jit::Kernel>> jit_kernels;   // loaded modules by program hash
     std::vector<u64> jit_used;       // per AIR of the last proof: 1 = JIT kernel, 0 = interpreter
     std::vector<u64> jit_check_used; // per AIR (instance order) of the last constraint check, census or guard run: the same
+    std::vector<u64> jit_lookup_check_used;   // per AIR (instance order) of the last lookup check: the same
+    void load_lookup_check_jit();
+    bool alloc_if_free(std::initializer_list<std::pair<DevBuf*, size_t>> bufs);
     std::string jit_note;            // why the JIT was not used, if it was wanted
     Committed prep_c; bool has_prep = false;
     std::vector<u32> prep_air, prep_log_h;
@@ -385,6 +392,27 @@ struct mdn_session {
         ja.main_lde = c.main_cm; ja.aux_lde = c.aux_cm; ja.prep_lde = c.prep_cm;
         ja.publics = c.publics; ja.challenges = c.challenges; ja.aux_values = c.aux_values; ja.periodic = c.prog.periodic;
         ja.log_n = c.log_n; ja.n_periodic = c.prog.n_periodic; ja.log_max_period = c.prog.log_max_period;
+        return ja;
+    }
+    // the same inputs for the NVRTC lookup-check kernels (jit.hpp LookupCheckJitArgs), one per interpreter struct
+    template <class Args> static jit::LookupCheckJitArgs lookup_check_args(const Args& b) {
+        jit::LookupCheckJitArgs ja{};
+        ja.main_lde = b.main_cm; ja.prep_lde = b.prep_cm; ja.publics = b.publics; ja.challenges = b.challenges;
+        ja.periodic = b.prog.periodic; ja.log_n = b.log_n; ja.n_periodic = b.prog.n_periodic; ja.log_max_period = b.prog.log_max_period;
+        return ja;
+    }
+    static jit::LookupCheckJitArgs balance_jit_args(const mk::BalanceArgs& b) {
+        jit::LookupCheckJitArgs ja = lookup_check_args(b);
+        ja.mutex_pos = b.mutex_pos; ja.mutex_group = b.mutex_group; ja.mutex_site = b.mutex_site; ja.n_mutex = b.n_mutex;
+        ja.t_keys = b.t.keys; ja.t_sums = b.t.sums; ja.t_count = b.t.count; ja.t_first = b.t.first; ja.t_mask = b.t.mask;
+        ja.counters = b.counters; ja.mutex_out = b.mutex_out; ja.contrib_out = b.contrib_out;
+        ja.instance = b.instance; ja.mode = b.mode;
+        return ja;
+    }
+    template <class Args> static jit::LookupCheckJitArgs fold_jit_args(const Args& f) {   // LookupFoldArgs, FoldCensusArgs
+        jit::LookupCheckJitArgs ja = lookup_check_args(f);
+        ja.n_cols = f.n_cols; ja.marks = f.marks; ja.aux_cm = f.aux_cm; ja.final_a = f.final.a; ja.final_b = f.final.b;
+        ja.failing_rows = f.failing_rows;
         return ja;
     }
     void check_constraints(const mdn_statement* st, const mdn_matrix* traces, const mdn_matrix* prep, const mdn_challenger* ch,
@@ -1733,6 +1761,58 @@ bool mdn_session::lookup_air(u32 i, const char* given, u32& skipped) {
     return false;
 }
 
+// The lookup checks' NVRTC kernels (jit.hpp MODE_LOOKUP_CHECK) of every AIR whose lookup program -- its interaction
+// part, for a version-2 program -- has at least jit_min_nodes nodes: one cubin per program and column count, cached in
+// jit_kernels with the keys "LKCB" / "LKCF" / "LKCC" (one per entry point, each with its own first-use state).  Proofs
+// and the constraint checks never call this.  A compile or load failure leaves the AIR on the interpreter and says why
+// in jit_note; the emulator build never specialises.
+void mdn_session::load_lookup_check_jit() {
+    jit_lookup_check_used.assign(airs.size(), 0);
+    for (AirHost& h : airs) {
+        h.lkc_balance.reset(); h.lkc_fold.reset(); h.lkc_census.reset();
+#ifndef MDN_EMULATED
+        const mdn_lookup& lk = h.lookup_v1;
+        if (!h.has_lookup || !jit_min_nodes || lk.program[2] < jit_min_nodes) continue;
+        try {
+            const u64 key = jit::fnv1a(lk.program, lk.program_words) ^ ((u64)lk.program_words << 40) ^ ((u64)lk.num_columns << 32);
+            const u64 kb = key ^ 0x4C4B4342ull, kf = key ^ 0x4C4B4346ull, kc = key ^ 0x4C4B4343ull;   // "LKCB", "LKCF", "LKCC"
+            if (!jit_kernels.count(kb) || !jit_kernels.count(kf) || !jit_kernels.count(kc)) {
+                const std::vector<char>& cubin = jit::cubin_for(lk.program, lk.program_words, nullptr, jit::MODE_LOOKUP_CHECK, lk.num_columns);
+                auto b = std::make_shared<jit::Kernel>(), f = std::make_shared<jit::Kernel>(), c = std::make_shared<jit::Kernel>();
+                b->load(cubin, "k_jit_balance");
+                f->load(*b, "k_jit_fold");
+                c->load(*b, "k_jit_fold_census");
+                jit_kernels[kb] = b; jit_kernels[kf] = f; jit_kernels[kc] = c;
+            }
+            h.lkc_balance = jit_kernels[kb]; h.lkc_fold = jit_kernels[kf]; h.lkc_census = jit_kernels[kc];
+        } catch (const std::exception& e) { jit_note = e.what(); }
+#endif
+    }
+}
+
+// Allocates buffers that are optional to the caller: false, with nothing allocated, when the device's and the arena's
+// free memory cannot hold them or an allocation fails.
+bool mdn_session::alloc_if_free(std::initializer_list<std::pair<DevBuf*, size_t>> bufs) {
+    size_t need = 0;
+    for (auto& b : bufs) need += b.second * sizeof(u64);
+#ifndef MDN_EMULATED
+    size_t arena_b = 0, free_b = 0, total_b = 0;
+    for (auto& sl : arena.slabs) arena_b += sl.size - sl.used;
+    CUDA_OK(cudaMemGetInfo(&free_b, &total_b));
+    if (need > free_b + arena_b) return false;
+#endif
+    try {
+        for (auto& b : bufs) b.first->alloc(b.second, stream);
+    } catch (const MdnError&) {
+        cudaGetLastError();
+        for (auto& b : bufs) b.first->release();
+        return false;
+    }
+    return true;
+}
+
+static const char LOOKUP_CHECK_DISAGREED[] = "NVRTC lookup-check kernel disagreed with the interpreter on its first use; interpreter kept";
+
 // ---------------------------------------------------------------------------------------------
 // check_constraints: every constraint of every AIR on every trace row, without a proof  (debug.rs:70-214)
 // ---------------------------------------------------------------------------------------------
@@ -2198,13 +2278,59 @@ void mdn_session::check_trace_balance(const mdn_statement* st, const mdn_matrix*
     CUDA_OK(cudaMemsetAsync(ctr.p, 0, 5 * sizeof(u64), stream));
     unsigned long long* counters = (unsigned long long*)ctr.p;
     std::vector<mk::BalanceArgs> ba(k);
+    // k_jit_balance where the AIR has it.  `twin`: one of them is on its first use in the session, so every pass runs
+    // the interpreter a second time, on every lookup AIR, into a table, counters and lists of its own (tw); the passes
+    // compare the two and, on a disagreement, keep the interpreter's and retire the kernels on their first use.
+    load_lookup_check_jit();
+    std::vector<std::shared_ptr<jit::Kernel>> bk(k);
+    bool twin = false;
+    for (u32 i = 0; i < k; i++) {
+        std::shared_ptr<jit::Kernel>& kn = airs[i].lkc_balance;
+        if (kn && kn->checked < 0) kn.reset();   // failed its self-check earlier in this session
+        bk[i] = kn;
+        if (kn) { jit_lookup_check_used[i] = 1; twin |= kn->checked == 0; }
+    }
+    DevBuf tw_ctr, tw_table, tw_mut, tw_con;
+    mk::BalanceTable tw_t{};
+    if (twin) { tw_ctr.alloc(5, stream); CUDA_OK(cudaMemsetAsync(tw_ctr.p, 0, 5 * sizeof(u64), stream)); }
+    auto drop_jit = [&](bool disagreed) {   // the interpreter's results stand from here on
+        for (u32 i = 0; i < k; i++) {
+            if (!bk[i]) continue;
+            if (disagreed && bk[i]->checked == 0) bk[i]->checked = -1;
+            bk[i].reset(); jit_lookup_check_used[i] = 0;
+        }
+        if (disagreed) jit_note = LOOKUP_CHECK_DISAGREED;
+        twin = false;
+    };
     auto run_rows = [&](u32 mode) {
         for (u32 i = 0; i < k; i++) {
             if (!airs[i].has_lookup) continue;
             mk::BalanceArgs& b = ba[i];
             b.mode = mode;
-            if (mk::launch_balance_rows(b, stream) != 0) fail(MDN_ERR_UNSUPPORTED, "AIR %u: lookup program too large for the interpreter", i);
+            if (bk[i]) {
+                const jit::LookupCheckJitArgs ja = balance_jit_args(b);
+                try { bk[i]->launch(ja, (unsigned)((((size_t)1 << b.log_n) + 127) / 128), 128, stream); }
+                catch (const std::exception& e) { fail(MDN_ERR_CUDA, "%s", e.what()); }
+                mk::count_launch();
+            } else if (mk::launch_balance_rows(b, stream) != 0) fail(MDN_ERR_UNSUPPORTED, "AIR %u: lookup program too large for the interpreter", i);
+            if (!twin) continue;
+            mk::BalanceArgs c = b;
+            c.t = tw_t; c.counters = (unsigned long long*)tw_ctr.p; c.mutex_out = tw_mut.p; c.contrib_out = tw_con.p;
+            if (mk::launch_balance_rows(c, stream) != 0) fail(MDN_ERR_UNSUPPORTED, "AIR %u: lookup program too large for the interpreter", i);
         }
+    };
+    // the twin's counters (after the stream's work so far)
+    auto twin_counters = [&](u64 c2[5]) {
+        CUDA_OK(cudaMemcpyAsync(c2, tw_ctr.p, 5 * sizeof(u64), cudaMemcpyDeviceToHost, stream));
+        CUDA_OK(cudaStreamSynchronize(stream));
+    };
+    // n triples of a list, sorted: the lists are written in the order the atomics ran
+    auto sorted_triples = [&](const u64* d, u64 n) {
+        std::vector<std::array<u64, 3>> v(n);
+        if (n) CUDA_OK(cudaMemcpyAsync(v.data(), d, 3 * n * sizeof(u64), cudaMemcpyDeviceToHost, stream));
+        CUDA_OK(cudaStreamSynchronize(stream));
+        std::sort(v.begin(), v.end());
+        return v;
     };
     for (u32 i = 0; i < k; i++) {
         if (!airs[i].has_lookup) continue;
@@ -2225,6 +2351,11 @@ void mdn_session::check_trace_balance(const mdn_statement* st, const mdn_matrix*
     u64 cnt[5];
     CUDA_OK(cudaMemcpyAsync(cnt, ctr.p, sizeof cnt, cudaMemcpyDeviceToHost, stream));
     CUDA_OK(cudaStreamSynchronize(stream));
+    if (twin) {
+        u64 c2[5];
+        twin_counters(c2);
+        if (c2[0] != cnt[0] || c2[1] != cnt[1]) { cnt[0] = c2[0]; cnt[1] = c2[1]; drop_jit(true); }
+    }
     const u64 n_push = cnt[0] + n_boundary, n_mutex = cnt[1];
     u64 slots = 1024;
     while (slots < 2 * n_push) slots <<= 1;
@@ -2238,10 +2369,38 @@ void mdn_session::check_trace_balance(const mdn_statement* st, const mdn_matrix*
     CUDA_OK(cudaMemsetAsync(t.sums, 0, 3 * slots * sizeof(u64), stream));
     CUDA_OK(cudaMemsetAsync(t.first, 0xFF, slots * sizeof(u64), stream));
     CUDA_OK(cudaMemsetAsync(ctr.p, 0, 5 * sizeof(u64), stream));
+    // the twin's table of the same size; without the room for it this call runs the interpreter, the kernels unchecked
+    if (twin && !alloc_if_free({{&tw_table, 6 * slots}, {&tw_mut, 3 * std::max<u64>(1, n_mutex)}})) drop_jit(false);
+    if (twin) {
+        tw_t.keys = tw_table.p; tw_t.sums = tw_table.p + 2 * slots;
+        tw_t.count = (unsigned long long*)(tw_table.p + 4 * slots); tw_t.first = (unsigned long long*)(tw_table.p + 5 * slots); tw_t.mask = slots - 1;
+        CUDA_OK(cudaMemsetAsync(tw_t.keys, 0xFF, 2 * slots * sizeof(u64), stream));
+        CUDA_OK(cudaMemsetAsync(tw_t.sums, 0, 3 * slots * sizeof(u64), stream));
+        CUDA_OK(cudaMemsetAsync(tw_t.first, 0xFF, slots * sizeof(u64), stream));
+        CUDA_OK(cudaMemsetAsync(tw_ctr.p, 0, 5 * sizeof(u64), stream));
+    }
 
     // 2. insert, boundary, finish
     for (auto& b : ba) { b.t = t; b.mutex_out = mut.p; }
     run_rows(1);
+    if (twin) {
+        // the same keys with the same sums, counts and least keys (placement follows the order of the atomics), and
+        // the same mutex violations
+        DevBuf cw; cw.alloc(3, stream);
+        CUDA_OK(cudaMemsetAsync(cw.p, 0, 3 * sizeof(u64), stream));
+        mk::launch_balance_compare(t, tw_t, (unsigned long long*)cw.p, stream);
+        u64 w[3], c1[5], c2[5];
+        CUDA_OK(cudaMemcpyAsync(w, cw.p, sizeof w, cudaMemcpyDeviceToHost, stream));
+        CUDA_OK(cudaMemcpyAsync(c1, ctr.p, sizeof c1, cudaMemcpyDeviceToHost, stream));
+        twin_counters(c2);
+        CUDA_OK(cudaGetLastError());
+        if (w[0] != w[1] || w[2] || c1[1] != c2[1] || sorted_triples(mut.p, c1[1]) != sorted_triples(tw_mut.p, c2[1])) {
+            std::swap(table, tw_table); std::swap(mut, tw_mut); std::swap(t, tw_t);
+            for (auto& b : ba) { b.t = t; b.mutex_out = mut.p; }
+            CUDA_OK(cudaMemcpyAsync(ctr.p, tw_ctr.p, 5 * sizeof(u64), cudaMemcpyDeviceToDevice, stream));
+            drop_jit(true);
+        }
+    }
     DevBuf bnd;
     if (n_boundary) {
         bnd.alloc(3 * n_boundary, stream);
@@ -2284,9 +2443,23 @@ void mdn_session::check_trace_balance(const mdn_statement* st, const mdn_matrix*
         DevBuf con; con.alloc(3 * n_contrib, stream);
         CUDA_OK(cudaMemsetAsync(ctr.p, 0, 5 * sizeof(u64), stream));
         for (auto& b : ba) b.contrib_out = con.p;
+        if (twin) {   // the twin collects from the finished table too
+            tw_t = t;
+            tw_con.alloc(3 * n_contrib, stream);
+            CUDA_OK(cudaMemsetAsync(tw_ctr.p, 0, 5 * sizeof(u64), stream));
+        }
         run_rows(2);
         CUDA_OK(cudaMemcpyAsync(cnt, ctr.p, sizeof cnt, cudaMemcpyDeviceToHost, stream));
         CUDA_OK(cudaStreamSynchronize(stream));
+        if (twin) {
+            u64 c2[5];
+            twin_counters(c2);
+            // a miscounting kernel may have written past the list: the interpreter's count bounds what is read
+            if (c2[2] != cnt[2] || sorted_triples(con.p, std::min(cnt[2], n_contrib)) != sorted_triples(tw_con.p, c2[2])) {
+                std::swap(con, tw_con); cnt[2] = c2[2];
+                drop_jit(true);
+            }
+        }
         std::vector<u64> ch(3 * cnt[2]);
         if (cnt[2]) CUDA_OK(cudaMemcpyAsync(ch.data(), con.p, ch.size() * sizeof(u64), cudaMemcpyDeviceToHost, stream));
         CUDA_OK(cudaStreamSynchronize(stream));
@@ -2308,6 +2481,9 @@ void mdn_session::check_trace_balance(const mdn_statement* st, const mdn_matrix*
             bal_contrib.push_back(p);
         }
     }
+    // every pass agreed: the kernels on their first use are checked (a call that lists no contributions checks the
+    // count and insert passes)
+    for (u32 i = 0; i < k; i++) if (bk[i] && twin) bk[i]->checked = 1;
     // mutex violations, (instance, row, column, group)
     std::vector<u64> mo(n_mutex);
     for (u64 v = 0; v < n_mutex; v++) mo[v] = v;
@@ -2420,6 +2596,7 @@ void mdn_session::prepare_folds(const mdn_statement* st, const mdn_matrix* trace
         build_logup_aux(pos[i], fs.main_cm[i], airs[i].raw_prep.p, aux_cm[i], fin, false);
         finals[i] = gl::e2(fin[0], fin[1]);
     }
+    load_lookup_check_jit();
 }
 
 void mdn_session::check_lookup_folds(const mdn_statement* st, const mdn_matrix* traces, const u64* rnd, const uint32_t* const* fold_marks,
@@ -2447,7 +2624,45 @@ void mdn_session::check_lookup_folds(const mdn_statement* st, const mdn_matrix* 
         f.folds_out = user && !on_device ? staging.p : user; f.folds_cm = cm;
         f.row0 = 0; f.n_rows = (size_t)1 << log_heights[i];
         f.first = (unsigned long long*)(res.p + 3 * i); f.failing_rows = f.first + 1; f.zero_u = f.first + 2;
-        if (mk::launch_fold_rows(f, stream) != 0) fail(MDN_ERR_UNSUPPORTED, "AIR %u: lookup program too large for the interpreter", i);
+        std::shared_ptr<jit::Kernel>& kn = airs[i].lkc_fold;
+        if (kn && kn->checked < 0) kn.reset();   // failed its self-check earlier in this session
+        if (!kn) {
+            if (mk::launch_fold_rows(f, stream) != 0) fail(MDN_ERR_UNSUPPORTED, "AIR %u: lookup program too large for the interpreter", i);
+        } else {
+            jit::LookupCheckJitArgs ja = fold_jit_args(f);
+            ja.folds_out = f.folds_out; ja.folds_cm = f.folds_cm; ja.row0 = f.row0; ja.n_rows = f.n_rows;
+            ja.first = f.first; ja.zero_u = f.zero_u;
+            try { kn->launch(ja, (unsigned)((f.n_rows + 127) / 128), 128, stream); }
+            catch (const std::exception& e) { fail(MDN_ERR_CUDA, "%s", e.what()); }
+            mk::count_launch();
+            jit_lookup_check_used[i] = 1;
+            if (kn->checked == 0) {
+                // first use of this kernel in the session: the interpreter runs the same rows into its own three
+                // words and folds; words and folds must agree word for word
+                const size_t fw = f.folds_out ? ((size_t)4 * f.n_cols) << f.log_n : 0;
+                DevBuf tw; tw.alloc(4 + fw, stream);
+                const u64 init[4] = {~0ull, 0, 0, 0};   // first, failing rows, zero U, the folds' comparison flag
+                CUDA_OK(cudaMemcpyAsync(tw.p, init, sizeof init, cudaMemcpyHostToDevice, stream));
+                mk::LookupFoldArgs t = f;
+                t.first = (unsigned long long*)tw.p; t.failing_rows = t.first + 1; t.zero_u = t.first + 2;
+                t.folds_out = fw ? tw.p + 4 : nullptr;
+                if (mk::launch_fold_rows(t, stream) != 0) fail(MDN_ERR_UNSUPPORTED, "AIR %u: lookup program too large for the interpreter", i);
+                if (fw) mk::launch_compare(f.folds_out, t.folds_out, fw, (u32*)(tw.p + 3), stream);
+                u64 wj[3], wi[4];
+                CUDA_OK(cudaMemcpyAsync(wj, res.p + 3 * i, sizeof wj, cudaMemcpyDeviceToHost, stream));
+                CUDA_OK(cudaMemcpyAsync(wi, tw.p, sizeof wi, cudaMemcpyDeviceToHost, stream));
+                CUDA_OK(cudaStreamSynchronize(stream));
+                CUDA_OK(cudaGetLastError());
+                if (wj[0] != wi[0] || wj[1] != wi[1] || wj[2] != wi[2] || wi[3]) {
+                    // a compiler defect: the interpreter's words and folds stand, the kernel is retired
+                    CUDA_OK(cudaMemcpyAsync(res.p + 3 * i, tw.p, 3 * sizeof(u64), cudaMemcpyDeviceToDevice, stream));
+                    if (fw) CUDA_OK(cudaMemcpyAsync(f.folds_out, t.folds_out, fw * sizeof(u64), cudaMemcpyDeviceToDevice, stream));
+                    CUDA_OK(cudaStreamSynchronize(stream));   // tw is released at the end of this block
+                    kn->checked = -1; jit_lookup_check_used[i] = 0;
+                    jit_note = LOOKUP_CHECK_DISAGREED;
+                } else kn->checked = 1;
+            }
+        }
         if (user && !on_device) {
             CUDA_OK(cudaMemcpyAsync(user, staging.p, (((size_t)4 * f.n_cols) << f.log_n) * sizeof(u64), cudaMemcpyDeviceToHost, stream));
             CUDA_OK(cudaStreamSynchronize(stream));   // the staging buffer serves the next AIR
@@ -2518,6 +2733,7 @@ void mdn_session::lookup_fold_census(const mdn_statement* st, const mdn_matrix* 
     CUDA_OK(cudaMemcpyAsync(tally.p, host_tally.data(), host_tally.size() * sizeof(u64), cudaMemcpyHostToDevice, stream));
     CUDA_OK(cudaMemsetAsync(words.p, 0, 2 * sizeof(u64), stream));
     u32* d_counts = reinterpret_cast<u32*>(counts.p);
+    u64 checked_rows = 0;   // rows with a disagreement of AIRs whose row pass was compared on first use (not in words[0])
     std::vector<mk::FoldCensusArgs> fa(k);
     for (u32 i = 0; i < k; i++) {
         if (!airs[i].has_lookup) continue;
@@ -2528,7 +2744,49 @@ void mdn_session::lookup_fold_census(const mdn_statement* st, const mdn_matrix* 
         f.tally = (unsigned long long*)(tally.p + tally_base[i]);
         f.failing_rows = (unsigned long long*)words.p;
         f.offsets = offsets.p + row_base[i];
-        if (mk::launch_fold_census_rows(f, stream) != 0) fail(MDN_ERR_UNSUPPORTED, "AIR %u: lookup program too large for the interpreter", i);
+        std::shared_ptr<jit::Kernel>& kn = airs[i].lkc_census;
+        if (kn && kn->checked < 0) kn.reset();   // failed its self-check earlier in this session
+        if (!kn) {
+            if (mk::launch_fold_census_rows(f, stream) != 0) fail(MDN_ERR_UNSUPPORTED, "AIR %u: lookup program too large for the interpreter", i);
+            continue;
+        }
+        const size_t N = (size_t)1 << f.log_n, nt = 4 * (size_t)f.n_cols;
+        jit::LookupCheckJitArgs ja = fold_jit_args(f);
+        ja.row_count = f.row_count; ja.tally = f.tally;
+        // first use of this kernel in the session: the kernel's failing rows go to a word of their own, and the
+        // interpreter runs the same rows into its own counts, tally and word; all three must agree word for word
+        DevBuf twin;
+        if (kn->checked == 0) {
+            twin.alloc((N + 1) / 2 + nt + 2, stream);
+            CUDA_OK(cudaMemcpyAsync(twin.p + (N + 1) / 2, host_tally.data() + tally_base[i], nt * sizeof(u64), cudaMemcpyHostToDevice, stream));
+            CUDA_OK(cudaMemsetAsync(twin.p + (N + 1) / 2 + nt, 0, 2 * sizeof(u64), stream));
+            ja.failing_rows = (unsigned long long*)(twin.p + (N + 1) / 2 + nt);
+        }
+        try { kn->launch(ja, (unsigned)((N + 127) / 128), 128, stream); }
+        catch (const std::exception& e) { fail(MDN_ERR_CUDA, "%s", e.what()); }
+        mk::count_launch();
+        jit_lookup_check_used[i] = 1;
+        if (kn->checked != 0) continue;
+        mk::FoldCensusArgs t = f;
+        t.row_count = reinterpret_cast<u32*>(twin.p); t.tally = (unsigned long long*)(twin.p + (N + 1) / 2);
+        t.failing_rows = (unsigned long long*)(twin.p + (N + 1) / 2 + nt + 1);
+        if (mk::launch_fold_census_rows(t, stream) != 0) fail(MDN_ERR_UNSUPPORTED, "AIR %u: lookup program too large for the interpreter", i);
+        std::vector<u32> cnt_j(N), cnt_i(N);
+        std::vector<u64> tw(nt + 2), tj(nt);
+        CUDA_OK(cudaMemcpyAsync(cnt_j.data(), f.row_count, N * sizeof(u32), cudaMemcpyDeviceToHost, stream));
+        CUDA_OK(cudaMemcpyAsync(cnt_i.data(), twin.p, N * sizeof(u32), cudaMemcpyDeviceToHost, stream));
+        CUDA_OK(cudaMemcpyAsync(tj.data(), f.tally, nt * sizeof(u64), cudaMemcpyDeviceToHost, stream));
+        CUDA_OK(cudaMemcpyAsync(tw.data(), twin.p + (N + 1) / 2, (nt + 2) * sizeof(u64), cudaMemcpyDeviceToHost, stream));
+        CUDA_OK(cudaStreamSynchronize(stream));
+        CUDA_OK(cudaGetLastError());
+        if (cnt_j != cnt_i || !std::equal(tj.begin(), tj.end(), tw.begin()) || tw[nt] != tw[nt + 1]) {
+            // a compiler defect: the interpreter's counts and tally stand, the kernel is retired
+            CUDA_OK(cudaMemcpyAsync(f.row_count, twin.p, N * sizeof(u32), cudaMemcpyDeviceToDevice, stream));
+            CUDA_OK(cudaMemcpyAsync(f.tally, twin.p + (N + 1) / 2, nt * sizeof(u64), cudaMemcpyDeviceToDevice, stream));
+            kn->checked = -1; jit_lookup_check_used[i] = 0;
+            jit_note = LOOKUP_CHECK_DISAGREED;
+        } else kn->checked = 1;
+        checked_rows += tw[nt + 1];
     }
     if (rows) mk::launch_count_exclusive_scan(d_counts, rows, offsets.p, words.p + 1, scratch.p, stream);
     u64 host_words[2];
@@ -2536,6 +2794,7 @@ void mdn_session::lookup_fold_census(const mdn_statement* st, const mdn_matrix* 
     CUDA_OK(cudaMemcpyAsync(host_words, words.p, sizeof host_words, cudaMemcpyDeviceToHost, stream));
     CUDA_OK(cudaStreamSynchronize(stream));
     CUDA_OK(cudaGetLastError());
+    host_words[0] += checked_rows;
 
     // the disagreeing (instance, column) pairs in order, and the least disagreement: the first failing instance's least
     // (first_row, column)
@@ -3598,6 +3857,7 @@ long long mdn_get_info(mdn_session* s, mdn_info what, uint64_t* out, size_t cap)
         case MDN_INFO_QUERY_INDICES: v = s->dbg_queries; break;
         case MDN_INFO_JIT: v = s->jit_used; break;
         case MDN_INFO_JIT_CHECK: v = s->jit_check_used; break;
+        case MDN_INFO_JIT_LOOKUP_CHECK: v = s->jit_lookup_check_used; break;
         case MDN_INFO_POOL: {
             cudaMemPool_t pool; uint64_t a[4] = {0, 0, 0, 0};
             if (cudaDeviceGetDefaultMemPool(&pool, s->device) == cudaSuccess) {
