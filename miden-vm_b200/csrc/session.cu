@@ -175,6 +175,17 @@ struct Committed {
     u64 root[4];
 };
 
+// The row passes that can run on an NVRTC-specialised kernel (jit.hpp) instead of the op-list interpreter, and the note
+// each leaves in jit_note when its kernel disagrees with the interpreter on its first use in a session.
+enum JitPass : u32 { JIT_PROOF, JIT_LOGUP, JIT_CHECK, JIT_CENSUS, JIT_BALANCE, JIT_FOLD, JIT_FOLD_CENSUS, JIT_PASSES };
+const char CHECK_DISAGREED[] = "NVRTC check kernel disagreed with the interpreter on its first use; interpreter kept";
+const char LOOKUP_CHECK_DISAGREED[] = "NVRTC lookup-check kernel disagreed with the interpreter on its first use; interpreter kept";
+const char* const JIT_DISAGREED[JIT_PASSES] = {
+    "NVRTC kernel disagreed with the interpreter on its first use; interpreter kept",          // constraint evaluation
+    "NVRTC lookup kernel disagreed with the interpreter on its first use; interpreter kept",   // LogUp aux build
+    CHECK_DISAGREED, CHECK_DISAGREED,                                                          // check and guard, census
+    LOOKUP_CHECK_DISAGREED, LOOKUP_CHECK_DISAGREED, LOOKUP_CHECK_DISAGREED};                   // balance, folds, fold census
+
 struct AirHost {
     mdn_air desc;
     DevBuf program;   // nodes | constraints | consts(lo,hi pairs as u64)
@@ -201,13 +212,10 @@ struct AirHost {
     u32 lookup_cols = 0, n_regs = 0;
     DevBuf reg_program;
     mk::AirDev reg_dev{};
-    // NVRTC-specialised constraint kernel (jit.hpp) for large programs; NULL = interpreter.  check_jit / census_jit:
-    // the two entry points of the program's trace-check cubin (k_jit_check, k_jit_census), loaded for the checks and
-    // for a guarded proof
-    std::shared_ptr<jit::Kernel> jit, lookup_jit, check_jit, census_jit;
-    // lkc_balance / lkc_fold / lkc_census: the three entry points of the lookup program's lookup-check cubin
-    // (k_jit_balance, k_jit_fold, k_jit_fold_census), loaded by the lookup checks only (load_lookup_check_jit)
-    std::shared_ptr<jit::Kernel> lkc_balance, lkc_fold, lkc_census;
+    // per row pass, the NVRTC kernel of a large program (mdn_session::load_jit); NULL = interpreter.  The proof's
+    // kernels are loaded for a proof, the check and census kernels for the checks and a guarded proof, the three
+    // lookup-check kernels by the lookup checks only (load_lookup_check_jit).
+    std::array<std::shared_ptr<jit::Kernel>, JIT_PASSES> jit;
     u32 n_constraints = 0;
 };
 
@@ -314,7 +322,26 @@ struct mdn_session {
     std::vector<u64> jit_used;       // per AIR of the last proof: 1 = JIT kernel, 0 = interpreter
     std::vector<u64> jit_check_used; // per AIR (instance order) of the last constraint check, census or guard run: the same
     std::vector<u64> jit_lookup_check_used;   // per AIR (instance order) of the last lookup check: the same
+    struct JitEntry { JitPass pass; const char* name; u64 salt; };
+    void load_jit(AirHost& h, const u32* w, u32 n_words, jit::Mode mode, u32 n_cols, std::initializer_list<JitEntry> entries);
     void load_lookup_check_jit();
+    // The first-use self-check shared by every NVRTC row pass.  row_kernel: AIR h's kernel for pass p, or NULL for the
+    // interpreter (a kernel that disagreed earlier in the session is dropped); launch_jit: one thread per row in
+    // 128-thread blocks; unchecked: its first use, when the caller runs the interpreter into twin buffers as well.
+    static jit::Kernel* row_kernel(AirHost& h, JitPass p) {
+        std::shared_ptr<jit::Kernel>& kn = h.jit[p];
+        if (kn && kn->checked < 0) kn.reset();
+        return kn.get();
+    }
+    static bool unchecked(const jit::Kernel& kn) { return kn.checked == 0; }
+    template <class Args> void launch_jit(const jit::Kernel& kn, const Args& a, size_t rows) {
+        try { kn.launch(a, (unsigned)((rows + 127) / 128), 128, stream); }
+        catch (const std::exception& e) { fail(MDN_ERR_CUDA, "%s", e.what()); }
+        mk::count_launch();
+    }
+    bool settle_jit(jit::Kernel& kn, JitPass p, bool differs, u64* used, bool promote = true);
+    struct Twin { u64* kernel; const u64* interp; size_t n; };   // n words the kernel and the interpreter wrote
+    bool compare_jit(jit::Kernel& kn, JitPass p, u64* used, std::initializer_list<Twin> twins, bool all_ranks = false);
     bool alloc_if_free(std::initializer_list<std::pair<DevBuf*, size_t>> bufs);
     std::string jit_note;            // why the JIT was not used, if it was wanted
     Committed prep_c; bool has_prep = false;
@@ -1263,37 +1290,12 @@ void mdn_session::bind_airs(const mdn_statement* st, const mdn_matrix* traces, b
         h.dev.periodic = a.num_periodic_columns ? h.program.p + per_off : nullptr;
         h.dev.n_instr = (u32)(code.size() / 4); h.dev.n_slots = std::max(1u, n_slots); h.dev.uses_selectors = uses_sel;
         h.dev.log_max_period = a.log_max_period; h.dev.n_periodic = a.num_periodic_columns;
-        // large programs: straight-line kernel compiled once per AIR (jit.hpp); the interpreter stays the fallback
-        h.jit.reset(); h.n_constraints = a.program[3];
-        if (jit && jit_min_nodes && a.program[2] >= jit_min_nodes) {
-            try {
-                u64 key = jit::fnv1a(a.program, a.program_words) ^ ((u64)a.program_words << 40);
-                auto it = jit_kernels.find(key);
-                if (it == jit_kernels.end()) {
-                    const std::vector<char>& cubin = jit::cubin_for(a.program, a.program_words, nullptr);
-                    auto kn = std::make_shared<jit::Kernel>();
-                    kn->load(cubin);
-                    it = jit_kernels.emplace(key, kn).first;
-                }
-                h.jit = it->second;
-            } catch (const std::exception& e) { jit_note = e.what(); }
-        }
-        h.check_jit.reset(); h.census_jit.reset();
-        if (check_jit && jit_min_nodes && a.program[2] >= jit_min_nodes) {
-            try {
-                // one cubin, two entry points; the keys carry the mode as the lookup kernel's carries "LKUP"
-                const u64 key = jit::fnv1a(a.program, a.program_words) ^ ((u64)a.program_words << 40);
-                const u64 k_check = key ^ 0x4348454Bull, k_census = key ^ 0x43454E53ull;   // "CHEK", "CENS"
-                if (!jit_kernels.count(k_check) || !jit_kernels.count(k_census)) {
-                    const std::vector<char>& cubin = jit::cubin_for(a.program, a.program_words, nullptr, jit::MODE_CHECK);
-                    auto kc = std::make_shared<jit::Kernel>(), ks = std::make_shared<jit::Kernel>();
-                    kc->load(cubin, "k_jit_check");
-                    ks->load(*kc, "k_jit_census");
-                    jit_kernels[k_check] = kc; jit_kernels[k_census] = ks;
-                }
-                h.check_jit = jit_kernels[k_check]; h.census_jit = jit_kernels[k_census];
-            } catch (const std::exception& e) { jit_note = e.what(); }
-        }
+        // large programs: straight-line kernels compiled once per program (jit.hpp); the interpreter stays the fallback
+        h.jit = {}; h.n_constraints = a.program[3];
+        if (jit) load_jit(h, a.program, a.program_words, jit::MODE_CONSTRAINTS, 0, {{JIT_PROOF, "k_jit", 0}});
+        if (check_jit)   // the keys carry the mode as the lookup kernel's carries "LKUP"
+            load_jit(h, a.program, a.program_words, jit::MODE_CHECK, 0,
+                     {{JIT_CHECK, "k_jit_check", 0x4348454Bull}, {JIT_CENSUS, "k_jit_census", 0x43454E53ull}});   // "CHEK", "CENS"
         // lowered LookupAir -> the aux trace of this AIR is built on the device (commit_aux)
         h.has_lookup = a.lookup != nullptr;
         if (h.has_lookup) {
@@ -1343,22 +1345,73 @@ void mdn_session::bind_airs(const mdn_statement* st, const mdn_matrix* traces, b
             h.lookup_prep = h.reg_prep = false;
             for (u32 j = 0; j < lk.program[2]; j++) h.lookup_prep |= lk.program[5 + 3 * (size_t)j] == 15;
             for (u32 j = 0; v2 && j < split.regs[2]; j++) h.reg_prep |= split.regs[5 + 3 * (size_t)j] == 15;
-            h.lookup_jit.reset();
-            if (jit && jit_min_nodes && lk.program[2] >= jit_min_nodes) {
-                try {
-                    u64 key = jit::fnv1a(lk.program, lk.program_words) ^ ((u64)lk.program_words << 40) ^ 0x4C4B5550ull;
-                    auto it = jit_kernels.find(key);
-                    if (it == jit_kernels.end()) {
-                        const std::vector<char>& cubin = jit::cubin_for(lk.program, lk.program_words, nullptr, jit::MODE_LOOKUP, lk.num_columns);
-                        auto kn = std::make_shared<jit::Kernel>();
-                        kn->load(cubin);
-                        it = jit_kernels.emplace(key, kn).first;
-                    }
-                    h.lookup_jit = it->second;
-                } catch (const std::exception& e) { jit_note = e.what(); }
-            }
+            if (jit) load_jit(h, lk.program, lk.program_words, jit::MODE_LOOKUP, lk.num_columns, {{JIT_LOGUP, "k_jit", 0x4C4B5550ull}});   // "LKUP"
         }
     }
+}
+
+// The entry points `entries` of the cubin of program w (n_words words, compiled in `mode` for n_cols columns) into AIR
+// h's kernel slots, when the program has at least jit_min_nodes nodes.  The session caches each entry point in
+// jit_kernels under the program's hash salted with the entry's salt, so AIRs with the same program share one kernel
+// and its first-use state.  A compile or load failure leaves the AIR on the interpreter and says why in jit_note.
+void mdn_session::load_jit(AirHost& h, const u32* w, u32 n_words, jit::Mode mode, u32 n_cols, std::initializer_list<JitEntry> entries) {
+    if (!jit_min_nodes || w[2] < jit_min_nodes) return;
+    try {
+        const u64 key = jit::fnv1a(w, n_words) ^ ((u64)n_words << 40);
+        bool cached = true;
+        for (const JitEntry& e : entries) cached &= jit_kernels.count(key ^ e.salt) != 0;
+        if (!cached) {
+            const std::vector<char>& cubin = jit::cubin_for(w, n_words, nullptr, mode, n_cols);
+            std::vector<std::shared_ptr<jit::Kernel>> kns;
+            for (const JitEntry& e : entries) {
+                kns.push_back(std::make_shared<jit::Kernel>());
+                if (kns.size() == 1) kns[0]->load(cubin, e.name);
+                else kns.back()->load(*kns[0], e.name);
+            }
+            size_t q = 0;
+            for (const JitEntry& e : entries) jit_kernels[key ^ e.salt] = kns[q++];
+        }
+        for (const JitEntry& e : entries) h.jit[e.pass] = jit_kernels[key ^ e.salt];
+    } catch (const std::exception& e) { jit_note = e.what(); }
+}
+
+// The verdict of kernel kn's first use in pass p: whether the interpreter's results stand.  A disagreement -- or any
+// comparison while MDN_JIT_FORCE_DISAGREE=1, which lets tests run every fallback -- retires the kernel for the rest of
+// the session, clears the caller's used flag and sets the pass's note; it wins over an agreement of an AIR sharing the
+// kernel.  An agreement marks a kernel on its first use as checked, unless `promote` is false (a pass with more
+// comparisons to come).
+bool mdn_session::settle_jit(jit::Kernel& kn, JitPass p, bool differs, u64* used, bool promote) {
+    const char* force = getenv("MDN_JIT_FORCE_DISAGREE");
+    if (differs || (force && !strcmp(force, "1"))) {
+        kn.checked = -1;
+        if (used) *used = 0;
+        jit_note = JIT_DISAGREED[p];
+        return true;
+    }
+    if (promote && kn.checked == 0) kn.checked = 1;
+    return false;
+}
+
+// The first-use comparison of pass p on the device: every twin's kernel words against its interpreter words (`all_ranks`:
+// the verdict of every rank of a split proof, which must all take the same branch), settled by settle_jit.  When the
+// interpreter's results stand they are copied over the kernel's, for exactly the words compared.
+bool mdn_session::compare_jit(jit::Kernel& kn, JitPass p, u64* used, std::initializer_list<Twin> twins, bool all_ranks) {
+    DevBuf word; word.alloc(1, stream);
+    CUDA_OK(cudaMemsetAsync(word.p, 0, sizeof(u64), stream));
+    for (const Twin& t : twins) if (t.n) mk::launch_compare(t.kernel, t.interp, t.n, (u32*)word.p, stream);
+    u64 differs = 0;
+    CUDA_OK(cudaMemcpyAsync(&differs, word.p, sizeof differs, cudaMemcpyDeviceToHost, stream));
+    CUDA_OK(cudaStreamSynchronize(stream));
+    CUDA_OK(cudaGetLastError());
+    if (all_ranks && sharded()) {
+        std::vector<u64> all(shard_world);
+        if (allgather(allgather_ctx, &differs, all.data(), 1) != 0) fail(MDN_ERR_INVALID_ARG, "all-gather callback failed");
+        for (u64 f : all) differs |= f;
+    }
+    if (!settle_jit(kn, p, differs != 0, used)) return false;
+    for (const Twin& t : twins) if (t.n) CUDA_OK(cudaMemcpyAsync(t.kernel, t.interp, t.n * sizeof(u64), cudaMemcpyDeviceToDevice, stream));
+    CUDA_OK(cudaStreamSynchronize(stream));
+    return true;
 }
 
 // public values, TraceOrder and the NTT tables of every height (`tables` false: the height limit only, for a check)
@@ -1590,39 +1643,20 @@ void mdn_session::build_logup_aux(u32 j, const u64* main_cm, const u64* prep_cm,
     la.publics = d_publics.p; la.challenges = d_randomness.p; la.aux_cm = aux_cm; la.totals = totals.p; la.bad_flag = (u32*)d_flag.p;
     {
         ProfScope ps(prof, PC_CONSTRAINTS);
-        if (h.lookup_jit && h.lookup_jit->checked < 0) h.lookup_jit.reset();
-        if (h.lookup_jit) {
+        if (jit::Kernel* kn = row_kernel(h, JIT_LOGUP)) {
             jit::LookupJitArgs ja{};
             ja.main_lde = la.main_cm; ja.prep_lde = prep_cm; ja.publics = la.publics; ja.challenges = la.challenges;
             ja.periodic = h.lookup_dev.periodic; ja.aux_cm = aux_cm; ja.totals = totals.p; ja.bad_flag = la.bad_flag;
             ja.log_n = ln; ja.n_periodic = h.lookup_dev.n_periodic; ja.log_max_period = h.lookup_dev.log_max_period;
-            try { h.lookup_jit->launch(ja, (unsigned)((N + 127) / 128), 128, stream); }
-            catch (const std::exception& e) { fail(MDN_ERR_CUDA, "%s", e.what()); }
-            mk::count_launch();
-            if (h.lookup_jit->checked == 0) {
-                // first use: the interpreter builds the same rows into scratch buffers; fraction columns and row totals
-                // must agree word for word, otherwise the interpreter's result is kept and the kernel is retired
+            launch_jit(*kn, ja, N);
+            if (unchecked(*kn)) {
+                // the interpreter builds the same rows into scratch buffers: fraction columns and row totals are compared
                 DevBuf aux2, tot2;
-                u32 C = h.lookup_cols;
-                aux2.alloc(2 * (size_t)C * N, stream); tot2.alloc(2 * N, stream);
+                const size_t C = h.lookup_cols;
+                aux2.alloc(2 * C * N, stream); tot2.alloc(2 * N, stream);
                 mk::LogupArgs lb2 = la; lb2.aux_cm = aux2.p; lb2.totals = tot2.p;
                 if (mk::launch_logup_rows(lb2, stream) != 0) fail(MDN_ERR_UNSUPPORTED, "lookup program too large for the interpreter");
-                if (C > 1) mk::launch_compare(aux2.p + 2 * N, aux_cm + 2 * N, 2 * (size_t)(C - 1) * N, (u32*)d_flag.p, stream);
-                mk::launch_compare(tot2.p, totals.p, 2 * N, (u32*)d_flag.p, stream);
-                u32 flag = 0;
-                CUDA_OK(cudaMemcpyAsync(&flag, d_flag.p, sizeof flag, cudaMemcpyDeviceToHost, stream));
-                CUDA_OK(cudaStreamSynchronize(stream));
-                if (flag & 4) {
-                    // clear the comparison bit only: a zero-denominator (2) or input (1) report raised by the same kernels stays
-                    u32 keep = flag & ~4u;
-                    CUDA_OK(cudaMemsetAsync(d_flag.p, 0, 8, stream));
-                    if (keep) { CUDA_OK(cudaMemcpyAsync(d_flag.p, &keep, sizeof keep, cudaMemcpyHostToDevice, stream)); CUDA_OK(cudaStreamSynchronize(stream)); }
-                    if (C > 1) CUDA_OK(cudaMemcpyAsync(aux_cm + 2 * N, aux2.p + 2 * N, 2 * (size_t)(C - 1) * N * sizeof(u64), cudaMemcpyDeviceToDevice, stream));
-                    CUDA_OK(cudaMemcpyAsync(totals.p, tot2.p, 2 * N * sizeof(u64), cudaMemcpyDeviceToDevice, stream));
-                    CUDA_OK(cudaStreamSynchronize(stream));
-                    h.lookup_jit->checked = -1;
-                    jit_note = "NVRTC lookup kernel disagreed with the interpreter on its first use; interpreter kept";
-                } else h.lookup_jit->checked = 1;
+                compare_jit(*kn, JIT_LOGUP, nullptr, {{aux_cm + 2 * N, aux2.p + 2 * N, 2 * (C - 1) * N}, {totals.p, tot2.p, 2 * N}});
             }
         } else if (mk::launch_logup_rows(la, stream) != 0) fail(MDN_ERR_UNSUPPORTED, "lookup program too large for the interpreter");
         mk::launch_ef_exclusive_scan(totals.p, N, aux_cm, aux_cm + N, fin.p, scratch.p, stream);
@@ -1764,28 +1798,18 @@ bool mdn_session::lookup_air(u32 i, const char* given, u32& skipped) {
 // The lookup checks' NVRTC kernels (jit.hpp MODE_LOOKUP_CHECK) of every AIR whose lookup program -- its interaction
 // part, for a version-2 program -- has at least jit_min_nodes nodes: one cubin per program and column count, cached in
 // jit_kernels with the keys "LKCB" / "LKCF" / "LKCC" (one per entry point, each with its own first-use state).  Proofs
-// and the constraint checks never call this.  A compile or load failure leaves the AIR on the interpreter and says why
-// in jit_note; the emulator build never specialises.
+// and the constraint checks never call this; the emulator build never specialises.
 void mdn_session::load_lookup_check_jit() {
     jit_lookup_check_used.assign(airs.size(), 0);
     for (AirHost& h : airs) {
-        h.lkc_balance.reset(); h.lkc_fold.reset(); h.lkc_census.reset();
+        for (JitPass p : {JIT_BALANCE, JIT_FOLD, JIT_FOLD_CENSUS}) h.jit[p].reset();
 #ifndef MDN_EMULATED
         const mdn_lookup& lk = h.lookup_v1;
-        if (!h.has_lookup || !jit_min_nodes || lk.program[2] < jit_min_nodes) continue;
-        try {
-            const u64 key = jit::fnv1a(lk.program, lk.program_words) ^ ((u64)lk.program_words << 40) ^ ((u64)lk.num_columns << 32);
-            const u64 kb = key ^ 0x4C4B4342ull, kf = key ^ 0x4C4B4346ull, kc = key ^ 0x4C4B4343ull;   // "LKCB", "LKCF", "LKCC"
-            if (!jit_kernels.count(kb) || !jit_kernels.count(kf) || !jit_kernels.count(kc)) {
-                const std::vector<char>& cubin = jit::cubin_for(lk.program, lk.program_words, nullptr, jit::MODE_LOOKUP_CHECK, lk.num_columns);
-                auto b = std::make_shared<jit::Kernel>(), f = std::make_shared<jit::Kernel>(), c = std::make_shared<jit::Kernel>();
-                b->load(cubin, "k_jit_balance");
-                f->load(*b, "k_jit_fold");
-                c->load(*b, "k_jit_fold_census");
-                jit_kernels[kb] = b; jit_kernels[kf] = f; jit_kernels[kc] = c;
-            }
-            h.lkc_balance = jit_kernels[kb]; h.lkc_fold = jit_kernels[kf]; h.lkc_census = jit_kernels[kc];
-        } catch (const std::exception& e) { jit_note = e.what(); }
+        const u64 c = (u64)lk.num_columns << 32;
+        if (h.has_lookup)
+            load_jit(h, lk.program, lk.program_words, jit::MODE_LOOKUP_CHECK, lk.num_columns,
+                     {{JIT_BALANCE, "k_jit_balance", c ^ 0x4C4B4342ull}, {JIT_FOLD, "k_jit_fold", c ^ 0x4C4B4346ull},
+                      {JIT_FOLD_CENSUS, "k_jit_fold_census", c ^ 0x4C4B4343ull}});
 #endif
     }
 }
@@ -1810,8 +1834,6 @@ bool mdn_session::alloc_if_free(std::initializer_list<std::pair<DevBuf*, size_t>
     }
     return true;
 }
-
-static const char LOOKUP_CHECK_DISAGREED[] = "NVRTC lookup-check kernel disagreed with the interpreter on its first use; interpreter kept";
 
 // ---------------------------------------------------------------------------------------------
 // check_constraints: every constraint of every AIR on every trace row, without a proof  (debug.rs:70-214)
@@ -1857,19 +1879,16 @@ void mdn_session::check_rows(std::vector<mk::CheckArgs>& ca, bool locate, mdn_co
         mk::CheckArgs& c = ca[i];
         c.row0 = 0; c.n_rows = (size_t)1 << c.log_n;
         c.first = (unsigned long long*)(res.p + 2 * i); c.failing_rows = (unsigned long long*)(res.p + 2 * i + 1);
-        std::shared_ptr<jit::Kernel>& kn = airs[i].check_jit;
-        if (kn && kn->checked < 0) kn.reset();   // failed its self-check earlier in this session
+        jit::Kernel* kn = row_kernel(airs[i], JIT_CHECK);
         if (!kn) {
             if (mk::launch_check_rows(c, stream) != 0) fail(MDN_ERR_UNSUPPORTED, "AIR %u: constraint program too large for the interpreter", i);
             continue;
         }
         jit::CheckJitArgs ja = check_jit_args(c);
         ja.first = c.first; ja.failing_rows = c.failing_rows; ja.row0 = c.row0; ja.n_rows = c.n_rows;
-        try { kn->launch(ja, (unsigned)((c.n_rows + 127) / 128), 128, stream); }
-        catch (const std::exception& e) { fail(MDN_ERR_CUDA, "%s", e.what()); }
-        mk::count_launch();
+        launch_jit(*kn, ja, c.n_rows);
         jit_check_used[i] = 1;
-        if (kn->checked == 0) {
+        if (unchecked(*kn)) {
             // first use of this kernel in the session: the interpreter checks the same rows into its own two words
             mk::CheckArgs t = c;
             t.first = (unsigned long long*)(res.p + twin + 2 * i); t.failing_rows = (unsigned long long*)(res.p + twin + 2 * i + 1);
@@ -1881,13 +1900,10 @@ void mdn_session::check_rows(std::vector<mk::CheckArgs>& ca, bool locate, mdn_co
     CUDA_OK(cudaStreamSynchronize(stream));
     CUDA_OK(cudaGetLastError());
     for (u32 i : first_use) {
-        jit::Kernel& kn = *airs[i].check_jit;
-        if (host_res[2 * i] != host_res[twin + 2 * i] || host_res[2 * i + 1] != host_res[twin + 2 * i + 1]) {
-            // a compiler defect: the interpreter's words stand, the kernel is retired
+        const bool differs = host_res[2 * i] != host_res[twin + 2 * i] || host_res[2 * i + 1] != host_res[twin + 2 * i + 1];
+        if (settle_jit(*airs[i].jit[JIT_CHECK], JIT_CHECK, differs, &jit_check_used[i])) {
             host_res[2 * i] = host_res[twin + 2 * i]; host_res[2 * i + 1] = host_res[twin + 2 * i + 1];
-            kn.checked = -1; jit_check_used[i] = 0;
-            jit_note = "NVRTC check kernel disagreed with the interpreter on its first use; interpreter kept";
-        } else if (kn.checked == 0) kn.checked = 1;
+        }
     }
 
     memset(out, 0, sizeof *out);
@@ -2092,8 +2108,7 @@ void mdn_session::constraint_census(const mdn_statement* st, const mdn_matrix* t
         c.tally = (unsigned long long*)(tally.p + tally_base[i]);
         c.failing_rows = (unsigned long long*)words.p;
         c.offsets = offsets.p + row_base[i];
-        std::shared_ptr<jit::Kernel>& kn = airs[i].census_jit;
-        if (kn && kn->checked < 0) kn.reset();   // failed its self-check earlier in this session
+        jit::Kernel* kn = row_kernel(airs[i], JIT_CENSUS);
         if (!kn) {
             if (mk::launch_census_rows(c, stream) != 0) fail(MDN_ERR_UNSUPPORTED, "AIR %u: constraint program too large for the interpreter", i);
             continue;
@@ -2103,18 +2118,17 @@ void mdn_session::constraint_census(const mdn_statement* st, const mdn_matrix* t
         ja.failing_rows = c.failing_rows; ja.row_count = c.row_count; ja.tally = c.tally; ja.n_cons = c.n_cons;
         // first use of this kernel in the session: the kernel's failing rows go to a word of their own, and the
         // interpreter runs the same rows into its own counts, tally and word; all three must agree word for word
+        const bool first_use = unchecked(*kn);
         DevBuf twin;
-        if (kn->checked == 0) {
+        if (first_use) {
             twin.alloc((N + 1) / 2 + nt + 2, stream);
             CUDA_OK(cudaMemcpyAsync(twin.p + (N + 1) / 2, host_tally.data() + tally_base[i], nt * sizeof(u64), cudaMemcpyHostToDevice, stream));
             CUDA_OK(cudaMemsetAsync(twin.p + (N + 1) / 2 + nt, 0, 2 * sizeof(u64), stream));
             ja.failing_rows = (unsigned long long*)(twin.p + (N + 1) / 2 + nt);
         }
-        try { kn->launch(ja, (unsigned)((N + 127) / 128), 128, stream); }
-        catch (const std::exception& e) { fail(MDN_ERR_CUDA, "%s", e.what()); }
-        mk::count_launch();
+        launch_jit(*kn, ja, N);
         jit_check_used[i] = 1;
-        if (kn->checked != 0) continue;
+        if (!first_use) continue;
         mk::CensusArgs t = c;
         t.row_count = reinterpret_cast<u32*>(twin.p); t.tally = (unsigned long long*)(twin.p + (N + 1) / 2);
         t.failing_rows = (unsigned long long*)(twin.p + (N + 1) / 2 + nt + 1);
@@ -2127,13 +2141,11 @@ void mdn_session::constraint_census(const mdn_statement* st, const mdn_matrix* t
         CUDA_OK(cudaMemcpyAsync(tw.data(), twin.p + (N + 1) / 2, (nt + 2) * sizeof(u64), cudaMemcpyDeviceToHost, stream));
         CUDA_OK(cudaStreamSynchronize(stream));
         CUDA_OK(cudaGetLastError());
-        if (cnt_j != cnt_i || !std::equal(tj.begin(), tj.begin() + nt, tw.begin()) || tw[nt] != tw[nt + 1]) {
-            // a compiler defect: the interpreter's counts and tally stand, the kernel is retired
+        const bool differs = cnt_j != cnt_i || !std::equal(tj.begin(), tj.begin() + nt, tw.begin()) || tw[nt] != tw[nt + 1];
+        if (settle_jit(*kn, JIT_CENSUS, differs, &jit_check_used[i])) {   // the interpreter's counts and tally stand
             CUDA_OK(cudaMemcpyAsync(c.row_count, twin.p, N * sizeof(u32), cudaMemcpyDeviceToDevice, stream));
             if (nt) CUDA_OK(cudaMemcpyAsync(c.tally, twin.p + (N + 1) / 2, nt * sizeof(u64), cudaMemcpyDeviceToDevice, stream));
-            kn->checked = -1; jit_check_used[i] = 0;
-            jit_note = "NVRTC check kernel disagreed with the interpreter on its first use; interpreter kept";
-        } else kn->checked = 1;
+        }
         checked_rows += tw[nt + 1];
     }
     mk::launch_count_exclusive_scan(d_counts, rows, offsets.p, words.p + 1, scratch.p, stream);
@@ -2282,37 +2294,36 @@ void mdn_session::check_trace_balance(const mdn_statement* st, const mdn_matrix*
     // the interpreter a second time, on every lookup AIR, into a table, counters and lists of its own (tw); the passes
     // compare the two and, on a disagreement, keep the interpreter's and retire the kernels on their first use.
     load_lookup_check_jit();
-    std::vector<std::shared_ptr<jit::Kernel>> bk(k);
-    bool twin = false;
+    std::vector<jit::Kernel*> bk(k);
+    std::vector<u32> first_use;   // the AIRs whose kernel is on its first use
     for (u32 i = 0; i < k; i++) {
-        std::shared_ptr<jit::Kernel>& kn = airs[i].lkc_balance;
-        if (kn && kn->checked < 0) kn.reset();   // failed its self-check earlier in this session
-        bk[i] = kn;
-        if (kn) { jit_lookup_check_used[i] = 1; twin |= kn->checked == 0; }
+        bk[i] = row_kernel(airs[i], JIT_BALANCE);
+        if (bk[i]) jit_lookup_check_used[i] = 1;
+        if (bk[i] && unchecked(*bk[i])) first_use.push_back(i);
     }
+    bool twin = !first_use.empty();
     DevBuf tw_ctr, tw_table, tw_mut, tw_con;
     mk::BalanceTable tw_t{};
     if (twin) { tw_ctr.alloc(5, stream); CUDA_OK(cudaMemsetAsync(tw_ctr.p, 0, 5 * sizeof(u64), stream)); }
-    auto drop_jit = [&](bool disagreed) {   // the interpreter's results stand from here on
-        for (u32 i = 0; i < k; i++) {
-            if (!bk[i]) continue;
-            if (disagreed && bk[i]->checked == 0) bk[i]->checked = -1;
-            bk[i].reset(); jit_lookup_check_used[i] = 0;
-        }
-        if (disagreed) jit_note = LOOKUP_CHECK_DISAGREED;
+    auto drop_jit = [&] {   // the interpreter's results stand from here on
+        for (u32 i = 0; i < k; i++) if (bk[i]) { bk[i] = nullptr; jit_lookup_check_used[i] = 0; }
         twin = false;
+    };
+    // the verdict of a pass the twin compared: a disagreement retires the kernels on their first use and drops them all;
+    // the kernels count as checked when the last pass of the call agrees
+    auto settle = [&](bool differs, bool last) {
+        bool fallback = false;
+        for (u32 i : first_use) fallback |= settle_jit(*bk[i], JIT_BALANCE, differs, &jit_lookup_check_used[i], last);
+        if (fallback) drop_jit();
+        return fallback;
     };
     auto run_rows = [&](u32 mode) {
         for (u32 i = 0; i < k; i++) {
             if (!airs[i].has_lookup) continue;
             mk::BalanceArgs& b = ba[i];
             b.mode = mode;
-            if (bk[i]) {
-                const jit::LookupCheckJitArgs ja = balance_jit_args(b);
-                try { bk[i]->launch(ja, (unsigned)((((size_t)1 << b.log_n) + 127) / 128), 128, stream); }
-                catch (const std::exception& e) { fail(MDN_ERR_CUDA, "%s", e.what()); }
-                mk::count_launch();
-            } else if (mk::launch_balance_rows(b, stream) != 0) fail(MDN_ERR_UNSUPPORTED, "AIR %u: lookup program too large for the interpreter", i);
+            if (bk[i]) launch_jit(*bk[i], balance_jit_args(b), (size_t)1 << b.log_n);
+            else if (mk::launch_balance_rows(b, stream) != 0) fail(MDN_ERR_UNSUPPORTED, "AIR %u: lookup program too large for the interpreter", i);
             if (!twin) continue;
             mk::BalanceArgs c = b;
             c.t = tw_t; c.counters = (unsigned long long*)tw_ctr.p; c.mutex_out = tw_mut.p; c.contrib_out = tw_con.p;
@@ -2354,7 +2365,7 @@ void mdn_session::check_trace_balance(const mdn_statement* st, const mdn_matrix*
     if (twin) {
         u64 c2[5];
         twin_counters(c2);
-        if (c2[0] != cnt[0] || c2[1] != cnt[1]) { cnt[0] = c2[0]; cnt[1] = c2[1]; drop_jit(true); }
+        if (settle(c2[0] != cnt[0] || c2[1] != cnt[1], false)) { cnt[0] = c2[0]; cnt[1] = c2[1]; }
     }
     const u64 n_push = cnt[0] + n_boundary, n_mutex = cnt[1];
     u64 slots = 1024;
@@ -2370,7 +2381,7 @@ void mdn_session::check_trace_balance(const mdn_statement* st, const mdn_matrix*
     CUDA_OK(cudaMemsetAsync(t.first, 0xFF, slots * sizeof(u64), stream));
     CUDA_OK(cudaMemsetAsync(ctr.p, 0, 5 * sizeof(u64), stream));
     // the twin's table of the same size; without the room for it this call runs the interpreter, the kernels unchecked
-    if (twin && !alloc_if_free({{&tw_table, 6 * slots}, {&tw_mut, 3 * std::max<u64>(1, n_mutex)}})) drop_jit(false);
+    if (twin && !alloc_if_free({{&tw_table, 6 * slots}, {&tw_mut, 3 * std::max<u64>(1, n_mutex)}})) drop_jit();
     if (twin) {
         tw_t.keys = tw_table.p; tw_t.sums = tw_table.p + 2 * slots;
         tw_t.count = (unsigned long long*)(tw_table.p + 4 * slots); tw_t.first = (unsigned long long*)(tw_table.p + 5 * slots); tw_t.mask = slots - 1;
@@ -2394,11 +2405,10 @@ void mdn_session::check_trace_balance(const mdn_statement* st, const mdn_matrix*
         CUDA_OK(cudaMemcpyAsync(c1, ctr.p, sizeof c1, cudaMemcpyDeviceToHost, stream));
         twin_counters(c2);
         CUDA_OK(cudaGetLastError());
-        if (w[0] != w[1] || w[2] || c1[1] != c2[1] || sorted_triples(mut.p, c1[1]) != sorted_triples(tw_mut.p, c2[1])) {
+        if (settle(w[0] != w[1] || w[2] || c1[1] != c2[1] || sorted_triples(mut.p, c1[1]) != sorted_triples(tw_mut.p, c2[1]), false)) {
             std::swap(table, tw_table); std::swap(mut, tw_mut); std::swap(t, tw_t);
             for (auto& b : ba) { b.t = t; b.mutex_out = mut.p; }
             CUDA_OK(cudaMemcpyAsync(ctr.p, tw_ctr.p, 5 * sizeof(u64), cudaMemcpyDeviceToDevice, stream));
-            drop_jit(true);
         }
     }
     DevBuf bnd;
@@ -2455,9 +2465,8 @@ void mdn_session::check_trace_balance(const mdn_statement* st, const mdn_matrix*
             u64 c2[5];
             twin_counters(c2);
             // a miscounting kernel may have written past the list: the interpreter's count bounds what is read
-            if (c2[2] != cnt[2] || sorted_triples(con.p, std::min(cnt[2], n_contrib)) != sorted_triples(tw_con.p, c2[2])) {
+            if (settle(c2[2] != cnt[2] || sorted_triples(con.p, std::min(cnt[2], n_contrib)) != sorted_triples(tw_con.p, c2[2]), false)) {
                 std::swap(con, tw_con); cnt[2] = c2[2];
-                drop_jit(true);
             }
         }
         std::vector<u64> ch(3 * cnt[2]);
@@ -2483,7 +2492,7 @@ void mdn_session::check_trace_balance(const mdn_statement* st, const mdn_matrix*
     }
     // every pass agreed: the kernels on their first use are checked (a call that lists no contributions checks the
     // count and insert passes)
-    for (u32 i = 0; i < k; i++) if (bk[i] && twin) bk[i]->checked = 1;
+    if (twin) settle(false, true);
     // mutex violations, (instance, row, column, group)
     std::vector<u64> mo(n_mutex);
     for (u64 v = 0; v < n_mutex; v++) mo[v] = v;
@@ -2624,45 +2633,25 @@ void mdn_session::check_lookup_folds(const mdn_statement* st, const mdn_matrix* 
         f.folds_out = user && !on_device ? staging.p : user; f.folds_cm = cm;
         f.row0 = 0; f.n_rows = (size_t)1 << log_heights[i];
         f.first = (unsigned long long*)(res.p + 3 * i); f.failing_rows = f.first + 1; f.zero_u = f.first + 2;
-        std::shared_ptr<jit::Kernel>& kn = airs[i].lkc_fold;
-        if (kn && kn->checked < 0) kn.reset();   // failed its self-check earlier in this session
-        if (!kn) {
-            if (mk::launch_fold_rows(f, stream) != 0) fail(MDN_ERR_UNSUPPORTED, "AIR %u: lookup program too large for the interpreter", i);
-        } else {
+        if (jit::Kernel* kn = row_kernel(airs[i], JIT_FOLD)) {
             jit::LookupCheckJitArgs ja = fold_jit_args(f);
             ja.folds_out = f.folds_out; ja.folds_cm = f.folds_cm; ja.row0 = f.row0; ja.n_rows = f.n_rows;
             ja.first = f.first; ja.zero_u = f.zero_u;
-            try { kn->launch(ja, (unsigned)((f.n_rows + 127) / 128), 128, stream); }
-            catch (const std::exception& e) { fail(MDN_ERR_CUDA, "%s", e.what()); }
-            mk::count_launch();
+            launch_jit(*kn, ja, f.n_rows);
             jit_lookup_check_used[i] = 1;
-            if (kn->checked == 0) {
-                // first use of this kernel in the session: the interpreter runs the same rows into its own three
-                // words and folds; words and folds must agree word for word
+            if (unchecked(*kn)) {
+                // the interpreter runs the same rows into its own three words and folds: both are compared
                 const size_t fw = f.folds_out ? ((size_t)4 * f.n_cols) << f.log_n : 0;
                 DevBuf tw; tw.alloc(4 + fw, stream);
-                const u64 init[4] = {~0ull, 0, 0, 0};   // first, failing rows, zero U, the folds' comparison flag
+                const u64 init[3] = {~0ull, 0, 0};   // first, failing rows, zero U
                 CUDA_OK(cudaMemcpyAsync(tw.p, init, sizeof init, cudaMemcpyHostToDevice, stream));
                 mk::LookupFoldArgs t = f;
                 t.first = (unsigned long long*)tw.p; t.failing_rows = t.first + 1; t.zero_u = t.first + 2;
-                t.folds_out = fw ? tw.p + 4 : nullptr;
+                t.folds_out = fw ? tw.p + 4 : nullptr;   // 16-byte aligned: the kernels store folds in pairs of words
                 if (mk::launch_fold_rows(t, stream) != 0) fail(MDN_ERR_UNSUPPORTED, "AIR %u: lookup program too large for the interpreter", i);
-                if (fw) mk::launch_compare(f.folds_out, t.folds_out, fw, (u32*)(tw.p + 3), stream);
-                u64 wj[3], wi[4];
-                CUDA_OK(cudaMemcpyAsync(wj, res.p + 3 * i, sizeof wj, cudaMemcpyDeviceToHost, stream));
-                CUDA_OK(cudaMemcpyAsync(wi, tw.p, sizeof wi, cudaMemcpyDeviceToHost, stream));
-                CUDA_OK(cudaStreamSynchronize(stream));
-                CUDA_OK(cudaGetLastError());
-                if (wj[0] != wi[0] || wj[1] != wi[1] || wj[2] != wi[2] || wi[3]) {
-                    // a compiler defect: the interpreter's words and folds stand, the kernel is retired
-                    CUDA_OK(cudaMemcpyAsync(res.p + 3 * i, tw.p, 3 * sizeof(u64), cudaMemcpyDeviceToDevice, stream));
-                    if (fw) CUDA_OK(cudaMemcpyAsync(f.folds_out, t.folds_out, fw * sizeof(u64), cudaMemcpyDeviceToDevice, stream));
-                    CUDA_OK(cudaStreamSynchronize(stream));   // tw is released at the end of this block
-                    kn->checked = -1; jit_lookup_check_used[i] = 0;
-                    jit_note = LOOKUP_CHECK_DISAGREED;
-                } else kn->checked = 1;
+                compare_jit(*kn, JIT_FOLD, &jit_lookup_check_used[i], {{res.p + 3 * i, tw.p, 3}, {f.folds_out, t.folds_out, fw}});
             }
-        }
+        } else if (mk::launch_fold_rows(f, stream) != 0) fail(MDN_ERR_UNSUPPORTED, "AIR %u: lookup program too large for the interpreter", i);
         if (user && !on_device) {
             CUDA_OK(cudaMemcpyAsync(user, staging.p, (((size_t)4 * f.n_cols) << f.log_n) * sizeof(u64), cudaMemcpyDeviceToHost, stream));
             CUDA_OK(cudaStreamSynchronize(stream));   // the staging buffer serves the next AIR
@@ -2744,8 +2733,7 @@ void mdn_session::lookup_fold_census(const mdn_statement* st, const mdn_matrix* 
         f.tally = (unsigned long long*)(tally.p + tally_base[i]);
         f.failing_rows = (unsigned long long*)words.p;
         f.offsets = offsets.p + row_base[i];
-        std::shared_ptr<jit::Kernel>& kn = airs[i].lkc_census;
-        if (kn && kn->checked < 0) kn.reset();   // failed its self-check earlier in this session
+        jit::Kernel* kn = row_kernel(airs[i], JIT_FOLD_CENSUS);
         if (!kn) {
             if (mk::launch_fold_census_rows(f, stream) != 0) fail(MDN_ERR_UNSUPPORTED, "AIR %u: lookup program too large for the interpreter", i);
             continue;
@@ -2755,18 +2743,17 @@ void mdn_session::lookup_fold_census(const mdn_statement* st, const mdn_matrix* 
         ja.row_count = f.row_count; ja.tally = f.tally;
         // first use of this kernel in the session: the kernel's failing rows go to a word of their own, and the
         // interpreter runs the same rows into its own counts, tally and word; all three must agree word for word
+        const bool first_use = unchecked(*kn);
         DevBuf twin;
-        if (kn->checked == 0) {
+        if (first_use) {
             twin.alloc((N + 1) / 2 + nt + 2, stream);
             CUDA_OK(cudaMemcpyAsync(twin.p + (N + 1) / 2, host_tally.data() + tally_base[i], nt * sizeof(u64), cudaMemcpyHostToDevice, stream));
             CUDA_OK(cudaMemsetAsync(twin.p + (N + 1) / 2 + nt, 0, 2 * sizeof(u64), stream));
             ja.failing_rows = (unsigned long long*)(twin.p + (N + 1) / 2 + nt);
         }
-        try { kn->launch(ja, (unsigned)((N + 127) / 128), 128, stream); }
-        catch (const std::exception& e) { fail(MDN_ERR_CUDA, "%s", e.what()); }
-        mk::count_launch();
+        launch_jit(*kn, ja, N);
         jit_lookup_check_used[i] = 1;
-        if (kn->checked != 0) continue;
+        if (!first_use) continue;
         mk::FoldCensusArgs t = f;
         t.row_count = reinterpret_cast<u32*>(twin.p); t.tally = (unsigned long long*)(twin.p + (N + 1) / 2);
         t.failing_rows = (unsigned long long*)(twin.p + (N + 1) / 2 + nt + 1);
@@ -2779,13 +2766,11 @@ void mdn_session::lookup_fold_census(const mdn_statement* st, const mdn_matrix* 
         CUDA_OK(cudaMemcpyAsync(tw.data(), twin.p + (N + 1) / 2, (nt + 2) * sizeof(u64), cudaMemcpyDeviceToHost, stream));
         CUDA_OK(cudaStreamSynchronize(stream));
         CUDA_OK(cudaGetLastError());
-        if (cnt_j != cnt_i || !std::equal(tj.begin(), tj.end(), tw.begin()) || tw[nt] != tw[nt + 1]) {
-            // a compiler defect: the interpreter's counts and tally stand, the kernel is retired
+        const bool differs = cnt_j != cnt_i || !std::equal(tj.begin(), tj.end(), tw.begin()) || tw[nt] != tw[nt + 1];
+        if (settle_jit(*kn, JIT_FOLD_CENSUS, differs, &jit_lookup_check_used[i])) {   // the interpreter's counts and tally stand
             CUDA_OK(cudaMemcpyAsync(f.row_count, twin.p, N * sizeof(u32), cudaMemcpyDeviceToDevice, stream));
             CUDA_OK(cudaMemcpyAsync(f.tally, twin.p + (N + 1) / 2, nt * sizeof(u64), cudaMemcpyDeviceToDevice, stream));
-            kn->checked = -1; jit_lookup_check_used[i] = 0;
-            jit_note = LOOKUP_CHECK_DISAGREED;
-        } else kn->checked = 1;
+        }
         checked_rows += tw[nt + 1];
     }
     if (rows) mk::launch_count_exclusive_scan(d_counts, rows, offsets.p, words.p + 1, scratch.p, stream);
@@ -3016,9 +3001,9 @@ void mdn_session::finish() {
         ca.T = &ntt(ln).T;
         ca.t0 = t0(); ca.nt = nt();            // this rank's cosets (all of them on one GPU)
         ProfScope ps(prof, PC_CONSTRAINTS);
-        if (air.jit && air.jit->checked < 0) air.jit.reset();   // failed its self-check earlier in this session
-        jit_used.push_back(air.jit ? 1 : 0);
-        if (air.jit) {
+        jit::Kernel* kn = row_kernel(air, JIT_PROOF);
+        jit_used.push_back(kn ? 1 : 0);
+        if (kn) {
             // alpha^(K-1-k) for the K constraints in emission order
             u32 K = air.n_constraints;
             std::vector<E2> apow(std::max(1u, K));
@@ -3038,37 +3023,16 @@ void mdn_session::finish() {
             ja.log_n = ln; ja.log_b = lb; ja.acc_in_log_n = ca.acc_in_log_n; ja.lo_bits = ca.T->lo_bits; ja.log_max_period = air.dev.log_max_period;
             size_t Lj = (size_t)1 << (ln + lb), own = (size_t)ca.nt << ln;
             ja.pad = ca.t0 | (ca.nt << 8);
-            try { air.jit->launch(ja, (unsigned)((own + 127) / 128), 128, stream); }
-            catch (const std::exception& e) { fail(MDN_ERR_CUDA, "%s", e.what()); }
-            mk::count_launch();
-            if (air.jit->checked == 0) {
-                // first use of this compiled kernel in the session: the interpreter evaluates the same points and
-                // the two accumulators must agree word for word; on disagreement (a compiler defect) the interpreter's
-                // result is kept, the kernel is retired and the reason is recorded
+            launch_jit(*kn, ja, own);
+            if (unchecked(*kn)) {
+                // the interpreter evaluates the same points: those of this rank's cosets are compared, on every rank
+                // alike (the ranks' allocation sequences have to stay identical).  The other cosets of both
+                // accumulators are never read: the next AIR and the quotient read this rank's cosets only.
                 DevBuf chk; chk.alloc(2 * Lj, stream);
                 mk::ConstraintArgs cb = ca; cb.acc_out = chk.p;
                 if (mk::launch_constraints(cb, stream) != 0) fail(MDN_ERR_UNSUPPORTED, "constraint program too large for the interpreter");
-                for (u32 coord = 0; coord < 2; coord++) {     // the points this rank evaluated
-                    size_t o = (size_t)coord * Lj + ((size_t)ca.t0 << ln);
-                    mk::launch_compare(chk.p + o, ca.acc_out + o, own, (u32*)d_flag.p, stream);
-                }
-                u32 flag = 0;
-                CUDA_OK(cudaMemcpyAsync(&flag, d_flag.p, sizeof flag, cudaMemcpyDeviceToHost, stream));
-                CUDA_OK(cudaStreamSynchronize(stream));
-                if (sharded()) {
-                    // every rank must take the same branch (the ranks' allocation sequences have to stay identical)
-                    std::vector<u64> mine(1, flag & 4), all(shard_world);
-                    if (allgather(allgather_ctx, mine.data(), all.data(), 1) != 0) fail(MDN_ERR_INVALID_ARG, "all-gather callback failed");
-                    for (u64 f : all) flag |= (u32)f;
-                }
-                if (flag & 4) {
-                    CUDA_OK(cudaMemsetAsync(d_flag.p, 0, 8, stream));
-                    if (flag & ~4u) { u32 keep = flag & ~4u; CUDA_OK(cudaMemcpyAsync(d_flag.p, &keep, sizeof keep, cudaMemcpyHostToDevice, stream)); CUDA_OK(cudaStreamSynchronize(stream)); }
-                    CUDA_OK(cudaMemcpyAsync(ca.acc_out, chk.p, 2 * Lj * sizeof(u64), cudaMemcpyDeviceToDevice, stream));
-                    CUDA_OK(cudaStreamSynchronize(stream));
-                    air.jit->checked = -1; jit_used.back() = 0;
-                    jit_note = "NVRTC kernel disagreed with the interpreter on its first use; interpreter kept";
-                } else air.jit->checked = 1;
+                const size_t o = (size_t)ca.t0 << ln;
+                compare_jit(*kn, JIT_PROOF, &jit_used.back(), {{ca.acc_out + o, chk.p + o, own}, {ca.acc_out + Lj + o, chk.p + Lj + o, own}}, true);
             }
         } else if (mk::launch_constraints(ca, stream) != 0) fail(MDN_ERR_UNSUPPORTED, "constraint program too large for the interpreter");
         acc_cur = nxt; acc_prev_log = ln;
@@ -3612,7 +3576,7 @@ void mdn_session_destroy(mdn_session* s) {
     s->prep_c = Committed();
     s->d_publics.release(); s->d_randomness.release(); s->d_aux_values.release(); s->d_flag.release();
     s->ntt_plans.clear(); s->premul_plans.clear();
-    for (auto& a : s->airs) { a.jit.reset(); a.check_jit.reset(); a.census_jit.reset(); }
+    for (auto& a : s->airs) a.jit = {};
     s->jit_kernels.clear();
     cudaStreamSynchronize(s->stream);
     s->arena.destroy();
