@@ -684,6 +684,7 @@ typedef enum {
     MDN_INFO_BUILD = 10,           /* { generation of the field arithmetic, generation of the NTT kernels }: always { 2, 2 } (poseidon2_fast2.cuh, ntt2.cuh) */
     MDN_INFO_JIT_CHECK = 11,       /* per AIR (instance order) of the last mdn_check_constraints / mdn_constraint_census call or constraint-guard run: 1 = NVRTC row kernel, 0 = interpreter */
     MDN_INFO_JIT_LOOKUP_CHECK = 12, /* per AIR (instance order) of the last mdn_check_trace_balance / mdn_check_lookup_folds / mdn_lookup_fold_census call: 1 = NVRTC row kernel, 0 = interpreter (also for an AIR without mdn_air.lookup) */
+    MDN_INFO_JIT_CACHE = 13,       /* process-wide, session may be NULL: { disk hits, disk misses (no usable file: compiled), rejected files, write failures, NVRTC compiles, NVRTC wall ms } (mdn_jit_set_cache_dir); the last two count every compile, cache on or off */
 } mdn_info;
 /* QUOTIENT_ACC / DEEP_EVALS are only recorded (extra device->host copies) after mdn_set_debug(s, 1). */
 int mdn_set_debug(mdn_session* s, int enable);
@@ -707,9 +708,26 @@ int mdn_session_set_jit(mdn_session* s, uint32_t min_nodes);
 /* "nvrtc <version>" or why it is unavailable, plus the reason the last JIT attempt was dropped (compile error,
  * or the first-use comparison against the interpreter failed -- the interpreter's result is then kept). */
 const char* mdn_jit_status(mdn_session* s);
-/* Codegen + NVRTC only, no device needed: cubin size (> 0) or a negative mdn_status with *err set. */
+/* Codegen + NVRTC only, no device needed: cubin size (> 0) or a negative mdn_status with *err set.  Fills the
+ * mdn_jit_set_cache_dir cache for the constraint mode (a constraint program) or the LogUp mode (a lookup program). */
 long long mdn_jit_compile_check(const uint32_t* program, uint32_t program_words, const char** err);
-/* Copies at most cap u64 into out; returns the number of u64 available (or <0). */
+/* Keeps the NVRTC cubins on disk, so that later processes load them instead of compiling again (a Miden-size program
+ * takes NVRTC tens of seconds per mode).  Process-wide, like the in-memory cubin cache it extends: call it once at
+ * start-up.  `dir` must be an existing directory; NULL or "" turns the disk cache off, which is the default.  A bad
+ * `dir` returns MDN_ERR_INVALID_ARG with the reason in mdn_last_error(NULL).  The setting applies to later cubins the
+ * process has not compiled or read yet.
+ * Each cubin is <dir>/<key>.cubin, the key a BLAKE3 digest of the file format version, the NVRTC version, the
+ * compile options (MDN_JIT_PTXAS applied) and the generated source, so a changed program, generator, chunk size
+ * (MDN_JIT_CHUNK) or NVRTC gives a new file.  A file that fails its header, size or BLAKE3 check is ignored, and the
+ * cubin is compiled and the file replaced; a file is written through a temporary file and rename(2), so concurrent
+ * processes leave one whole file; a failed write (read-only directory, full disk) is counted and is not an error.
+ * mdn_get_info(NULL, MDN_INFO_JIT_CACHE) counts all of this.
+ * Trust: the BLAKE3 check detects corruption, not a hostile writer.  The files are loaded as GPU code, so only trusted
+ * users may be able to write to `dir`.  Each kernel, fresh or read from disk, is still compared with the interpreter on
+ * its first use in each session. */
+int mdn_jit_set_cache_dir(const char* dir);
+/* Copies at most cap u64 into out; returns the number of u64 available (or <0).  s may be NULL only for
+ * MDN_INFO_JIT_CACHE. */
 long long mdn_get_info(mdn_session* s, mdn_info what, uint64_t* out, size_t cap);
 
 /* Per-phase device timings of the last prove, in milliseconds (CUDA events on the session's

@@ -471,6 +471,9 @@ unsafe extern "C" {
     pub fn mdn_session_set_hash_challenger(s: *mut MdnSession, c: *const MdnHashChallenger) -> c_int;
     pub fn mdn_session_set_jit(s: *mut MdnSession, min_nodes: u32) -> c_int;
     pub fn mdn_jit_compile_check(program: *const u32, program_words: u32, err: *mut *const c_char) -> c_longlong;
+    /// Process-wide on-disk cubin cache in the existing directory `dir` (NULL or "": off, the default). Only trusted
+    /// users may be able to write to it: its files are loaded as GPU code.
+    pub fn mdn_jit_set_cache_dir(dir: *const c_char) -> c_int;
     pub fn mdn_get_timings(s: *mut MdnSession, out: *mut MdnTimings) -> c_int;
     pub fn mdn_abi_layout(out: *mut u32, cap: usize) -> usize;
 }

@@ -45,6 +45,8 @@ HASH_POSEIDON2, HASH_BLAKE3, HASH_KECCAK, HASH_RPO, HASH_RPX = 0, 1, 2, 3, 4
 # Session.info(INFO_JIT_LOOKUP_CHECK): per AIR (instance order) of the last check_trace_balance / check_lookup_folds /
 # lookup_fold_census call, 1 where the row passes ran on the NVRTC kernel, 0 on the interpreter (mdn_get_info 12)
 INFO_JIT_LOOKUP_CHECK = 12
+# mdn_get_info 13, process-wide (no session): see jit_cache_stats
+INFO_JIT_CACHE = 13
 
 
 class Matrix(C.Structure):
@@ -186,7 +188,7 @@ EXPORTS = [
     "mdn_session_set_external_check", "mdn_session_set_hash", "mdn_session_set_hash_challenger",
     "mdn_check_constraints", "mdn_session_set_device_aux_builder", "mdn_check_trace_balance",
     "mdn_check_lookup_folds", "mdn_constraint_census", "mdn_session_set_constraint_guard", "mdn_last_constraint_report",
-    "mdn_lookup_fold_census",
+    "mdn_lookup_fold_census", "mdn_jit_set_cache_dir",
 ]
 ERR_CONSTRAINT_VIOLATED = -8
 
@@ -201,6 +203,24 @@ def jit_compile_check(program: np.ndarray) -> int:
     if n < 0:
         raise ProverError(n, (err.value or b"").decode())
     return n
+
+
+def set_jit_cache_dir(path) -> None:
+    """Keep NVRTC cubins in the existing directory `path` for later processes (mdn_jit_set_cache_dir; None: off, the
+    default).  Process-wide: call it once at start-up.  Only trusted users may be able to write to `path`."""
+    rc = lib().mdn_jit_set_cache_dir(None if path is None else os.fsencode(path))
+    if rc != 0:
+        raise ProverError(f"[{rc}] {lib().mdn_last_error(None).decode()}")
+
+
+def jit_cache_stats() -> dict:
+    """The process-wide counts of mdn_get_info(NULL, MDN_INFO_JIT_CACHE)."""
+    out = np.zeros(6, dtype=np.uint64)
+    n = lib().mdn_get_info(None, INFO_JIT_CACHE, ptr(out), 6)
+    if n != 6:
+        raise ProverError(f"mdn_get_info(INFO_JIT_CACHE) returned {n}")
+    keys = ("disk_hits", "disk_misses", "rejected", "write_failures", "compiles", "compile_ms")
+    return {k: int(v) for k, v in zip(keys, out)}
 
 
 class BackendMissing(RuntimeError):
@@ -267,6 +287,7 @@ def lib():
         L.mdn_jit_status.argtypes = [C.c_void_p]
         L.mdn_jit_compile_check.restype = C.c_longlong
         L.mdn_jit_compile_check.argtypes = [u32p, C.c_uint32, C.POINTER(C.c_char_p)]
+        L.mdn_jit_set_cache_dir.argtypes = [C.c_char_p]
         L.mdn_get_timings.argtypes = [C.c_void_p, C.POINTER(Timings)]
         L.mdn_challenger_observe.argtypes = [C.POINTER(Challenger), u64p, C.c_size_t]
         L.mdn_challenger_sample.restype = C.c_uint64

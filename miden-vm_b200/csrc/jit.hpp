@@ -10,19 +10,29 @@
 // (asserted in tests/test_gpu_parity.py).  libnvrtc / libcuda are dlopen'ed on first use; when NVRTC is
 // missing the session keeps using the interpreter and says so in mdn_get_info(MDN_INFO_JIT).  The same lowering also
 // gives the LogUp row kernel (MODE_LOOKUP), the trace-check row kernels (MODE_CHECK, MDN_INFO_JIT_CHECK) and the
-// lookup-check row kernels (MODE_LOOKUP_CHECK, MDN_INFO_JIT_LOOKUP_CHECK).
+// lookup-check row kernels (MODE_LOOKUP_CHECK, MDN_INFO_JIT_LOOKUP_CHECK).  Cubins live for the process in cubin_for's
+// map and, with mdn_jit_set_cache_dir, across processes in a directory of files keyed by what NVRTC is given.
 #pragma once
 #include <cuda_runtime.h>
 #include <dlfcn.h>
+#include <sys/stat.h>
+#include <unistd.h>
+#include <algorithm>
+#include <atomic>
+#include <cerrno>
+#include <chrono>
+#include <climits>
 #include <cstdint>
 #include <cstdio>
 #include <cstdlib>
+#include <cstring>
 #include <map>
 #include <memory>
 #include <mutex>
 #include <stdexcept>
 #include <string>
 #include <vector>
+#include "blake3.cuh"
 
 namespace jit {
 
@@ -822,18 +832,38 @@ inline Nvrtc& nvrtc() {
     return n;
 }
 
+// Process-wide counts of the cubin cache (mdn_get_info(MDN_INFO_JIT_CACHE)): the disk counts are taken under the
+// cubin_for mutex; compiles and their wall time cover every NVRTC compile of the process.
+struct CacheStats {
+    std::atomic<uint64_t> disk_hits{0}, disk_misses{0}, rejected{0}, write_failures{0}, compiles{0}, compile_ns{0};
+};
+inline CacheStats& cache_stats() { static CacheStats s; return s; }
+
+// the options passed to nvrtcCompileProgram, MDN_JIT_PTXAS applied.  Chunked functions keep NVRTC + ptxas -O3 linear
+// (10 k nodes: 7 s); MDN_JIT_PTXAS overrides the level.
+inline std::vector<std::string> compile_options() {
+    return {"--gpu-architecture=sm_90a", "-std=c++17", "-lineinfo", "-default-device",
+            std::string("--ptxas-options=") + (getenv("MDN_JIT_PTXAS") ? getenv("MDN_JIT_PTXAS") : "-O3"), "--device-int128"};
+}
+
 // source -> sm_90a cubin (throws std::runtime_error with the compiler log on failure)
 inline std::vector<char> compile(const std::string& src) {
     Nvrtc& n = nvrtc();
     if (!n.ok()) throw std::runtime_error("NVRTC unavailable: " + n.why);
+    const auto t0 = std::chrono::steady_clock::now();
+    struct Timed {   // counts the compile and its wall time however it ends
+        std::chrono::steady_clock::time_point t0;
+        ~Timed() {
+            cache_stats().compiles++;
+            cache_stats().compile_ns += (uint64_t)std::chrono::duration_cast<std::chrono::nanoseconds>(std::chrono::steady_clock::now() - t0).count();
+        }
+    } timed{t0};
     void* prog = nullptr;
     int rc = n.CreateProgram(&prog, src.c_str(), "mdn_constraints.cu", 0, nullptr, nullptr);
     if (rc) throw std::runtime_error(std::string("nvrtcCreateProgram: ") + n.GetErrorString(rc));
-    // chunked functions keep NVRTC + ptxas -O3 linear (10 k nodes: 7 s); MDN_JIT_PTXAS overrides the level
-    std::vector<const char*> opts = {"--gpu-architecture=sm_90a", "-std=c++17", "-lineinfo", "-default-device"};
-    std::string po = std::string("--ptxas-options=") + (getenv("MDN_JIT_PTXAS") ? getenv("MDN_JIT_PTXAS") : "-O3");
-    opts.push_back(po.c_str());
-    opts.push_back("--device-int128");
+    const std::vector<std::string> os = compile_options();
+    std::vector<const char*> opts;
+    for (const std::string& o : os) opts.push_back(o.c_str());
     rc = n.CompileProgram(prog, (int)opts.size(), opts.data());
     if (rc) {
         size_t ls = 0; n.GetProgramLogSize(prog, &ls);
@@ -912,21 +942,161 @@ inline uint64_t fnv1a(const uint32_t* w, size_t n) {
     for (size_t i = 0; i < n; i++) { h ^= w[i]; h *= 1099511628211ull; }
     return h;
 }
-inline const std::vector<char>& cubin_for(const uint32_t* w, size_t n_words, GenInfo* info, Mode mode = MODE_CONSTRAINTS, uint32_t n_cols = 0) {
-    static std::mutex mu;
-    static std::map<uint64_t, std::pair<std::vector<char>, GenInfo>> cache;
-    uint64_t key = fnv1a(w, n_words) ^ (uint64_t)n_words << 40 ^ (uint64_t)chunk_nodes() << 20 ^ (uint64_t)n_cols << 8 ^ (uint64_t)mode;
-    std::lock_guard<std::mutex> g(mu);
-    auto it = cache.find(key);
-    if (it == cache.end()) {
-        GenInfo gi;
-        std::string src = generate(w, &gi, mode, n_cols);
-        if (const char* dump = getenv("MDN_JIT_DUMP")) { if (FILE* f = fopen(dump, "w")) { fwrite(src.data(), 1, src.size(), f); fclose(f); } }
-        it = cache.emplace(key, std::make_pair(compile(src), gi)).first;
-        if (const char* dump = getenv("MDN_JIT_DUMP_CUBIN")) { if (FILE* f = fopen(dump, "wb")) { fwrite(it->second.first.data(), 1, it->second.first.size(), f); fclose(f); } }
+// ---------------------------------------------------------------------------------------------
+// Persistent cubin cache (mdn_jit_set_cache_dir): one file per cubin, <dir>/<hex key>.cubin, the key a BLAKE3 digest
+// of everything NVRTC is given -- the file format version, the NVRTC version, the option list and the generated source
+// (which encodes the mode, the column count, the chunk size and every generator change).  A file is a DiskHeader
+// followed by the cubin; one that fails any check is ignored, and the cubin is compiled and the file replaced.  The
+// hash detects corruption, not a hostile writer: the files are loaded as GPU code.
+// ---------------------------------------------------------------------------------------------
+static constexpr uint32_t DISK_FORMAT = 1;
+static constexpr char DISK_MAGIC[8] = {'M', 'D', 'N', 'C', 'U', 'B', 'I', 'N'};
+struct DiskHeader {
+    char magic[8];
+    uint32_t format, reserved;
+    uint32_t key[8];          // the digest the file is named after
+    uint64_t cubin_bytes;
+    uint32_t cubin_hash[8];   // BLAKE3 of the cubin that follows
+};
+static_assert(sizeof(DiskHeader) == 88, "DiskHeader layout");
+
+// BLAKE3 of a list of byte strings.  b3::Hasher takes whole words and at most 256 KiB, so each string enters as its
+// length and the digests of its 64 KiB segments (zero-padded to whole words); generated sources and cubins are larger.
+inline void digest(std::initializer_list<std::pair<const void*, size_t>> parts, uint32_t out[8]) {
+    b3::Hasher outer; outer.init();
+    for (const auto& p : parts) {
+        const unsigned char* b = (const unsigned char*)p.first;
+        outer.push64(p.second);
+        const size_t segments = p.second ? (p.second + 65535) / 65536 : 1;
+        for (size_t s = 0; s < segments; s++) {
+            const size_t at = s * 65536, n = std::min<size_t>(65536, p.second - at);
+            b3::Hasher h; h.init();
+            for (size_t i = 0; i < n; i += 4) {
+                uint32_t v = 0;
+                for (size_t k = 0; k < 4 && i + k < n; k++) v |= (uint32_t)b[at + i + k] << (8 * k);
+                h.push(v);
+            }
+            uint32_t d[8];
+            h.finish(d);
+            for (uint32_t x : d) outer.push(x);
+        }
     }
-    if (info) *info = it->second.second;
-    return it->second.first;
+    outer.finish(out);
+}
+
+struct CubinEntry {
+    std::vector<char> cubin;
+    GenInfo info;
+    std::string file;   // the cache file the cubin was read from, or empty (compiled by this process)
+};
+struct CubinCache {
+    std::mutex mu;
+    std::map<uint64_t, CubinEntry> entries;
+    std::string dir;    // empty: no disk cache
+    uint64_t writes = 0;
+};
+inline CubinCache& cubin_cache() { static CubinCache c; return c; }
+
+// the process-wide cache directory for later misses of cubin_for (NULL or "": none); false with *err when `dir` is not
+// an existing directory
+inline bool set_cache_dir(const char* dir, std::string* err) {
+    std::string d;
+    if (dir && *dir) {
+        struct stat st;
+        if (stat(dir, &st) != 0) { *err = std::string("JIT cache directory ") + dir + ": " + strerror(errno); return false; }
+        if (!S_ISDIR(st.st_mode)) { *err = std::string("JIT cache directory ") + dir + ": not a directory"; return false; }
+        char abs[PATH_MAX];
+        d = realpath(dir, abs) ? abs : dir;   // absolute, so that a later chdir does not move the cache
+    }
+    std::lock_guard<std::mutex> g(cubin_cache().mu);
+    cubin_cache().dir = d;
+    return true;
+}
+
+inline std::string hex(const uint32_t* w, int n) {
+    std::string s;
+    char b[9];
+    for (int i = 0; i < n; i++) { snprintf(b, sizeof b, "%08x", w[i]); s += b; }
+    return s;
+}
+
+// the cubin stored under `key` at `path`, or false (no file: a plain miss; a file that fails a check: counted as rejected)
+inline bool read_cached(const std::string& path, const uint32_t key[8], std::vector<char>& cubin) {
+    FILE* f = fopen(path.c_str(), "rb");
+    if (!f) return false;
+    std::vector<char> raw;
+    char buf[1 << 16];
+    size_t got;
+    while ((got = fread(buf, 1, sizeof buf, f)) > 0) raw.insert(raw.end(), buf, buf + got);
+    const bool io_ok = !ferror(f);
+    fclose(f);
+    DiskHeader h;
+    bool ok = io_ok && raw.size() >= sizeof h;
+    if (ok) {
+        memcpy(&h, raw.data(), sizeof h);
+        uint32_t hash[8];
+        ok = !memcmp(h.magic, DISK_MAGIC, 8) && h.format == DISK_FORMAT && !memcmp(h.key, key, 32) && h.cubin_bytes > 0 &&
+             h.cubin_bytes == raw.size() - sizeof h &&
+             (digest({{raw.data() + sizeof h, (size_t)h.cubin_bytes}}, hash), !memcmp(hash, h.cubin_hash, 32));
+    }
+    if (!ok) { cache_stats().rejected++; return false; }
+    cubin.assign(raw.begin() + sizeof h, raw.end());
+    return true;
+}
+
+// writes the entry through a temporary file of this process and call, renamed onto `path` (concurrent writers of one
+// key leave one whole file); a failure is counted, not raised
+inline void write_cached(const std::string& dir, const std::string& path, const uint32_t key[8], const std::vector<char>& cubin, uint64_t call) {
+    DiskHeader h{};
+    memcpy(h.magic, DISK_MAGIC, 8);
+    h.format = DISK_FORMAT;
+    memcpy(h.key, key, 32);
+    h.cubin_bytes = cubin.size();
+    digest({{cubin.data(), cubin.size()}}, h.cubin_hash);
+    const std::string tmp = dir + "/." + hex(key, 8) + "." + std::to_string((long long)getpid()) + "." + std::to_string((unsigned long long)call) + ".tmp";
+    FILE* f = fopen(tmp.c_str(), "wb");
+    bool ok = f != nullptr;
+    if (ok) {
+        ok = fwrite(&h, sizeof h, 1, f) == 1 && fwrite(cubin.data(), 1, cubin.size(), f) == cubin.size();
+        ok = (fclose(f) == 0) && ok;
+        ok = ok && rename(tmp.c_str(), path.c_str()) == 0;
+        if (!ok) unlink(tmp.c_str());
+    }
+    if (!ok) cache_stats().write_failures++;
+}
+
+// process-wide cubin cache keyed by a hash of the program words (AIRs are fixed per deployment), backed by the disk
+// cache when a directory is set.  *file names the cache file the cubin was read from (empty: compiled here).
+inline const std::vector<char>& cubin_for(const uint32_t* w, size_t n_words, GenInfo* info, Mode mode = MODE_CONSTRAINTS,
+                                          uint32_t n_cols = 0, std::string* file = nullptr) {
+    CubinCache& cc = cubin_cache();
+    uint64_t key = fnv1a(w, n_words) ^ (uint64_t)n_words << 40 ^ (uint64_t)chunk_nodes() << 20 ^ (uint64_t)n_cols << 8 ^ (uint64_t)mode;
+    std::lock_guard<std::mutex> g(cc.mu);
+    auto it = cc.entries.find(key);
+    if (it == cc.entries.end()) {
+        CubinEntry e;
+        std::string src = generate(w, &e.info, mode, n_cols);
+        if (const char* dump = getenv("MDN_JIT_DUMP")) { if (FILE* f = fopen(dump, "w")) { fwrite(src.data(), 1, src.size(), f); fclose(f); } }
+        uint32_t dkey[8];
+        std::string path;
+        if (!cc.dir.empty() && nvrtc().ok()) {
+            const uint32_t head[2] = {DISK_FORMAT, (uint32_t)nvrtc().version};
+            std::string opts;
+            for (const std::string& o : compile_options()) { opts += o; opts += '\0'; }
+            digest({{head, sizeof head}, {opts.data(), opts.size()}, {src.data(), src.size()}}, dkey);
+            path = cc.dir + "/" + hex(dkey, 8) + ".cubin";
+            if (read_cached(path, dkey, e.cubin)) { e.file = path; cache_stats().disk_hits++; }
+        }
+        if (e.file.empty()) {
+            e.cubin = compile(src);
+            if (!path.empty()) { cache_stats().disk_misses++; write_cached(cc.dir, path, dkey, e.cubin, cc.writes++); }
+        }
+        it = cc.entries.emplace(key, std::move(e)).first;
+        if (const char* dump = getenv("MDN_JIT_DUMP_CUBIN")) { if (FILE* f = fopen(dump, "wb")) { fwrite(it->second.cubin.data(), 1, it->second.cubin.size(), f); fclose(f); } }
+    }
+    if (info) *info = it->second.info;
+    if (file) *file = it->second.file;
+    return it->second.cubin;
 }
 
 }  // namespace jit

@@ -1361,12 +1361,18 @@ void mdn_session::load_jit(AirHost& h, const u32* w, u32 n_words, jit::Mode mode
         bool cached = true;
         for (const JitEntry& e : entries) cached &= jit_kernels.count(key ^ e.salt) != 0;
         if (!cached) {
-            const std::vector<char>& cubin = jit::cubin_for(w, n_words, nullptr, mode, n_cols);
+            std::string file;
+            const std::vector<char>& cubin = jit::cubin_for(w, n_words, nullptr, mode, n_cols, &file);
             std::vector<std::shared_ptr<jit::Kernel>> kns;
-            for (const JitEntry& e : entries) {
-                kns.push_back(std::make_shared<jit::Kernel>());
-                if (kns.size() == 1) kns[0]->load(cubin, e.name);
-                else kns.back()->load(*kns[0], e.name);
+            try {
+                for (const JitEntry& e : entries) {
+                    kns.push_back(std::make_shared<jit::Kernel>());
+                    if (kns.size() == 1) kns[0]->load(cubin, e.name);
+                    else kns.back()->load(*kns[0], e.name);
+                }
+            } catch (const std::exception& e) {
+                if (file.empty()) throw;
+                throw std::runtime_error(std::string(e.what()) + " (cubin read from " + file + ")");
             }
             size_t q = 0;
             for (const JitEntry& e : entries) jit_kernels[key ^ e.salt] = kns[q++];
@@ -3808,9 +3814,15 @@ uint64_t mdn_challenger_sample(mdn_challenger* c) {
 }
 
 long long mdn_get_info(mdn_session* s, mdn_info what, uint64_t* out, size_t cap) {
-    if (!s) return -1;
+    if (!s && what != MDN_INFO_JIT_CACHE) return -1;
     std::vector<u64> v;
     switch (what) {
+        case MDN_INFO_JIT_CACHE: {
+            const jit::CacheStats& c = jit::cache_stats();
+            v = {c.disk_hits.load(), c.disk_misses.load(), c.rejected.load(), c.write_failures.load(), c.compiles.load(),
+                 c.compile_ns.load() / 1000000};
+            break;
+        }
         case MDN_INFO_MAIN_ROOT: v.assign(s->dbg_roots[0], s->dbg_roots[0] + 4); break;
         case MDN_INFO_AUX_ROOT: v.assign(s->dbg_roots[1], s->dbg_roots[1] + 4); break;
         case MDN_INFO_QUOTIENT_ROOT: v.assign(s->dbg_roots[2], s->dbg_roots[2] + 4); break;
@@ -3946,6 +3958,12 @@ const char* mdn_jit_status(mdn_session* s) {
 int mdn_session_set_jit(mdn_session* s, uint32_t min_nodes) {
     if (!s) return MDN_ERR_INVALID_ARG;
     s->jit_min_nodes = min_nodes;
+    return MDN_OK;
+}
+
+int mdn_jit_set_cache_dir(const char* dir) {
+    std::string err;
+    if (!jit::set_cache_dir(dir, &err)) { g_create_error = err; return MDN_ERR_INVALID_ARG; }
     return MDN_OK;
 }
 
